@@ -1,4 +1,4 @@
-"""Learner grad-steps/s of the recurrent QMIX update path (BASELINE.json metric) on N B200s.
+"""Learner grad-steps/s of the recurrent QMIX update path (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus N --steps K --warmup W            # this engine (one process per GPU; torchrun for N>1)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on the host cores
@@ -45,7 +45,7 @@ NO_AVAIL = {"qmix_mpe_spread"}       # MPE passes avail_acts = None (runner/rnn/
 
 
 def ncu_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed `ncu --set full` capture (profiles/ncu_traffic.json), or None."""
+    """DRAM bytes per launch of `kernel` from an `ncu --set full` capture summarised into profiles/ncu_traffic.json, or None."""
     path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     try:
         return json.load(open(path)).get(kernel, {}).get("dram_bytes")
@@ -58,7 +58,7 @@ def peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return dict(hbm=d["hbm_gbs"], tflops=d["bf16_tflops"], tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tflops=1590.0, tflops_sustained=1400.0, src="fallback")
+    return dict(hbm=3350.0, tflops=989.0, tflops_sustained=989.0, src="H100 SXM data sheet (dense BF16, HBM3), not measured")
 
 
 MADDPG_WORKLOADS = {
@@ -243,7 +243,7 @@ def synth_episodes(cfg, T, n, rs, avail=True):
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -327,7 +327,7 @@ def cpu_learner_steps_per_s(cfg, T, B, E, steps, warmup, threads, avail=True):
 
 
 def torch_eager_gpu_steps_per_s(cfg, T, B, E, steps, warmup, avail=True):
-    """Secondary baseline (SURVEY.md section 8(d)): the reference learner's own eager PyTorch ops on the SAME B200 (what
+    """Secondary baseline (SURVEY.md section 8(d)): the reference learner's own eager PyTorch ops on the SAME GPU (what
     `--cuda` gives the reference): the oracle port with its networks on cuda:0, batches sampled by the NumPy replay on the host and
     copied up per step like the reference's to_torch(...).to(device).  ~10^4 small ATen launches per step."""
     from oracle.qmix import QmixLearner
@@ -523,6 +523,13 @@ def run_engine(args):
     launches = int(lib.mx_launch_count() - launches0)
     if tgraph is not None:
         launches = kernels_per_step * args.steps
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        # what the last timed step left for its caller: train_info, the updated live / target parameters, the new PER priorities
+        v = tr._info_views
+        out = dict(loss=v[0], grad_norm=v[1], Q_tot=v[2], theta=tr.theta, theta_tgt=tr.theta_tgt)
+        if cfg.use_per:
+            out["priorities"] = tr._prio_view[:B]
+        dump_outputs(args.dump_outputs, out)
 
     if args.quick:          # tuning sweeps: the device-resident number only (not a bench line)
         if rank == 0:
@@ -651,24 +658,16 @@ def run_engine(args):
         ach = fl[top] / (kavg[top] * 1e-3) / 1e12
         roof = dict(bound="tensor", kernel=top, achieved=ach, peak=pk["tflops_sustained"], unit="TFLOP/s", frac=ach / pk["tflops_sustained"],
                     traffic=ncu_traffic(top), peak_source=pk["src"] + " bf16 sustained (kernel timed inside the step)",
-                    note="FP32 FFMA kernel (1e-4 parity budget); serial-recurrence / latency bound at these sizes, see DESIGN.md")
+                    note="FP32 FFMA kernel (1e-4 parity budget); serial-recurrence / latency bound at these sizes")
     else:
         ach = by.get(top, 0.0) / (kavg[top] * 1e-3) / 1e9
         roof = dict(bound="hbm", kernel=top, achieved=ach, peak=pk["hbm"], unit="GB/s", frac=ach / pk["hbm"], traffic=ncu_traffic(top), peak_source=pk["src"])
-    # latency model of the serial recurrences (SURVEY.md 8(d): "give the latency model alongside the roofline fraction"): the step
-    # contains (T+1) dependent GRU steps forward (live and target nets side by side) and T backward; `floor` = the dependency chain of
-    # one step counted from the SASS (LDS -> 4 FFMA2 -> 2 shuffles -> sigmoid -> tanh -> blend -> STS -> barrier; DESIGN.md section 4)
-    csum = clocks.summary()
-    sm_hz = 1e6 * float(csum.get("sm_mhz") or csum.get("sm_max_mhz") or 1965.0)
+    # latency view of the serial recurrences (SURVEY.md 8(d): "give the latency model alongside the roofline fraction"): the step
+    # contains (T+1) dependent GRU steps forward (live and target nets side by side) and T backward; measured time per dependent step
     t_f, t_b = kavg.get("k_gru_fwd"), kavg.get("k_gru_bwd")
     if t_f and t_b:
-        FLOOR_F, FLOOR_B = 330.0, 230.0
-        cyc_f, cyc_b = t_f * 1e-3 * sm_hz / (T + 1), t_b * 1e-3 * sm_hz / T
-        floor_ms = ((T + 1) * FLOOR_F + T * FLOOR_B) / sm_hz * 1e3
-        roof["latency_model"] = dict(serial_steps=2 * T + 1, t_step_cycles=dict(fwd=round(cyc_f, 1), bwd=round(cyc_b, 1)),
-                                     floor_cycles=dict(fwd=FLOOR_F, bwd=FLOOR_B), chain_ms=round(t_f + t_b, 5), floor_ms=round(floor_ms, 5),
-                                     frac=round(floor_ms / (t_f + t_b), 4), share_of_step=round((t_f + t_b) / ms_step, 4),
-                                     sm_mhz=round(sm_hz / 1e6, 1))
+        roof["latency_model"] = dict(serial_steps=2 * T + 1, us_per_serial_step=dict(fwd=round(t_f * 1e3 / (T + 1), 3), bwd=round(t_b * 1e3 / T, 3)),
+                                     chain_ms=round(t_f + t_b, 5), share_of_step=round((t_f + t_b) / ms_step, 4))
     gather_gbs = by["k_gather"] / (kavg.get("k_gather", 1e9) * 1e-3) / 1e9
     breakdown = {k: dict(ms=round(v, 5), share=round(v / ksum, 4)) for k, v in sorted(kavg.items(), key=lambda kv: -kv[1])}
 
@@ -920,6 +919,20 @@ def run_mlp(args):
 
 
 _REAL_STDOUT = None
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, arrays):
+    """`--dump-outputs DIR`: each array as DIR/<name>.npy in float32 (float64 stays float64); an array larger than its share of the
+    64 MB budget is replaced by the same fixed, seeded sample of its elements in every run."""
+    os.makedirs(dirname, exist_ok=True)
+    share = DUMP_MAX_BYTES // max(1, len(arrays))
+    for name, x in arrays.items():
+        a = (x.detach().cpu().numpy() if torch.is_tensor(x) else np.asarray(x)).reshape(-1)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if a.nbytes > share:
+            a = a[np.sort(np.random.default_rng(12345).choice(a.size, size=share // a.itemsize, replace=False))]
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def emit(line):
@@ -947,7 +960,11 @@ def main():
     ap.add_argument("--buffer", type=int, default=5000, help="replay episodes (scripts/train_smac_qmix.sh default 5000)")
     ap.add_argument("--quick", action="store_true", help="device-resident timing only (tuning sweeps; not the bench contract line)")
     ap.add_argument("--opt", action="append", default=[], help="engine option name=int (mx_set_option), e.g. --opt pdl=0 --opt front_tc=0")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last step computed (train_info, parameters, priorities) as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.dump_outputs and (a.impl == "reference" or a.workload not in WORKLOADS):
+        ap.error("--dump-outputs: only the engine arm of the recurrent QMIX workloads (%s) writes its outputs" % ", ".join(sorted(WORKLOADS)))
     if a.impl != "reference" and a.opt:
         from offpolicy._b200 import capi
         for kv in a.opt:

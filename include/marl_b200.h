@@ -1,4 +1,4 @@
-/* marl_b200.h -- C-ABI of the B200-native recurrent off-policy MARL update engine (libmarl_b200.so).
+/* marl_b200.h -- C-ABI of the H100-native recurrent off-policy MARL update engine (libmarl_b200.so).
  *
  * The reference (marlbenchmark/off-policy) is pure Python and has NO FFI/plugin interface
  * (SURVEY.md section 8(b)): the seam is Python class construction by dotted module path inside
@@ -47,7 +47,7 @@ int64_t mx_sizeof(const char* struct_name);
 int mx_host_fence_alloc(void);
 int mx_host_fence_record(int id, void* stream);
 int mx_host_fence_wait(int id);
-/* 1 when built by nvcc for sm_100a, 0 for the CPU-emulated unit-test build (tests/emu; never shipped) */
+/* 1 when built by nvcc for sm_90a, 0 for the CPU-emulated unit-test build (tests/emu; never shipped) */
 int mx_is_cuda_build(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -356,20 +356,20 @@ int mx_graph_capture(mx_replay* r, mx_qmix* q, int32_t B, double beta, uint32_t 
 int mx_graph_launch(mx_graph* g, void* stream);
 void mx_graph_destroy(mx_graph* g);
 
-/* tcgen05 building block probe (parity tests): Y[M][N] = X[M][K] . W[N][K]^T on the 5th-gen tensor cores with TF32
+/* Tensor-core building block probe (parity tests): Y[M][N] = X[M][K] . W[N][K]^T with wgmma on TF32
  * operands; passes = 1 (plain TF32) or 3 (3xTF32 hi/lo split, fp32-level accuracy); swap_ls selects which descriptor field
  * carries the K-direction core-matrix stride.  N % 16 == 0, N <= 256, K % 8 == 0, K <= 64. */
 int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int32_t N, int32_t K, int32_t passes, int32_t swap_ls, void* stream);
 
-/* Runtime options (process-wide tuning switches; defaults = the configuration measured on the B200, profiles/r02_option_sweeps.md).
+/* Runtime options (process-wide tuning switches; the defaults are not yet re-measured on the H100).
  * Returns 1 for an unknown name.  (default)
- *   front_tc (1)            time-batched front layers on the tcgen05 3xTF32 kernels; 0 = the FFMA kernel
+ *   front_tc (1)            time-batched front layers on the wgmma 3xTF32 kernels; 0 = the FFMA kernel
  *   front_tc_threads (256)  inputs <= 56: two threads per accumulator row (k_front_fwd_tc2); 128 = one (k_front_fwd_tc)
- *   front_tc_wide (1)       64 < input width <= 128 on tcgen05 too; front_tc_wide2 (1): weights streamed, two CTAs per SM (0: resident weights)
- *   wgrad_tc (-1)           backward of the front layers on tcgen05: -1 = by input width (inputs > 64: mode 2), 0 = FFMA k_front_bwd,
+ *   front_tc_wide (1)       64 < input width <= 128 on the tensor cores too; front_tc_wide2 (1): weights streamed, two CTAs per SM (0: resident weights)
+ *   wgrad_tc (-1)           backward of the front layers on the tensor cores: -1 = by input width (inputs > 64: mode 2), 0 = FFMA k_front_bwd,
  *                           1 = k_wgrad_tc beside k_front_bwd, 2 = k_front_bwd_tc + k_wgrad_tc; wgrad_tc_wide (1) = allow 64 < width <= 128;
  *                           front_bwd_tc_stream (1) = streamed transposed weights, two CTAs per SM
- *   front_bwd_mma (0)       mma.sync m16n8k8 3xTF32 inside k_front_bwd (measured slower)
+ *   front_bwd_mma (0)       mma.sync m16n8k8 3xTF32 inside k_front_bwd
  *   gru_wgrad_split (1)     GRU weight gradients as k_gru_wgrad on the forked branch beside k_front_bwd (QMIX step)
  *   gru_threads (0)         0 = 128-thread recurrences for sequences of >= 8 steps, 128 / 256 force a kernel family; gru_rows (1) rows per
  *                           128-thread CTA (2; 0 = by grid size); gru_fwd_rpc / gru_bwd_rpc (0 = automatic) rows per 256-thread CTA

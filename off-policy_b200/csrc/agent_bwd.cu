@@ -948,8 +948,8 @@ static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_
 
 extern int g_mx_front_bwd_rm;
 int g_mx_gru_wgrad_split = 1;    // 1 (default): the QMIX step runs the GRU weight gradients as k_gru_wgrad on the forked branch beside k_front_bwd
-int g_mx_front_bwd_mma = 0;      // 1: the GEMMs of k_front_bwd on mma.sync 3xTF32 tiles (mx_mma.cuh); 0 (default): FFMA micro-kernels.  Measured on B200
-                                 // (profiles/r02_option_sweeps.md): the legacy mma.sync TF32 path is SLOWER here -- k_front_bwd 60.3 vs 50.0 us at 3m, 8m step 2.22 vs 1.52 ms
+int g_mx_front_bwd_mma = 0;      // 1: the GEMMs of k_front_bwd on mma.sync 3xTF32 tiles (mx_mma.cuh); 0 (default): FFMA micro-kernels
+                                 // (default not yet measured on the H100)
 bool mx_front_bwd_tc_usable(const FrontBwdArgs& a);
 int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s);
 int mx_launch_front_bwd(const FrontBwdArgs& a_in, int* nparts_used, cudaStream_t s) {

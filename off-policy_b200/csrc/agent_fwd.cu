@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) k_gru_fwd(GruFwdArgs a) {
 // thread = 2*i + q owns, for unit i, the r/z/n rows of W_hh restricted to the interleaved k-slice {8m + 4q + c : m < 8, c < 4} (3 x 32
 // weights in registers).  Half the warps of k_gru_fwd per row: on an SM that hosts two rows (192 row-CTAs on 148 SMs at the 3m shapes)
 // every scheduler sees two warps instead of four, and on the others one -- the step is a dependent chain, fewer co-resident warps means
-// less issue and LSU contention; one xor-shuffle level instead of two.  Measured against the 256-thread kernel in profiles/ (r02).
+// less issue and LSU contention; one xor-shuffle level instead of two.
 #define GRU2_THREADS 128
 // ROWS = 2: the CTA carries two sequence rows through the same register-resident weights (their two dependent chains interleave), for
 // shapes with more row-CTAs than two per SM can hold at once (SMAC 8m: 1 024 row-CTAs = 3.5 waves of 296; option gru_rows)

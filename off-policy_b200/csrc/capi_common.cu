@@ -9,8 +9,8 @@ static thread_local char g_err[512] = "";
 long long g_mx_launches = 0;
 #if !MX_EMU
 int g_mx_pdl = -1;    // programmatic dependent launch: -1 (default) = for latency-bound learner steps only (rows <= g_mx_pdl_rows; set per step by the
-                      // learner), 1 = every launch, 0 = never.  B200, visit 16: 3m 172.0 -> 164.5 us with PDL; 2s3z 463 -> 478, 8m 1126 -> 1156 (the
-                      // dependents' prologues then take SM resources from kernels that are throughput-bound)
+                      // learner), 1 = every launch, 0 = never (the dependents' prologues take SM resources from kernels that are
+                      // throughput-bound, so PDL is meant for the small steps; the row threshold is not yet measured on the H100)
 int g_mx_pdl_rows = 12288;
 int g_mx_pdl_auto = 0;      // the learner's per-step decision in automatic mode
 int g_mx_pdl_skip_next = 0;
@@ -19,7 +19,6 @@ int g_mx_pdl_skip_next = 0;
 // runtime options shared by the product and the emulated build (mx_set_option)
 int g_mx_p2p_timeout_ms = 10000;      // how long a rank waits for a peer's gradient before it sets the sticky abort word (tests shorten it)
 int g_mx_gru_rows = 1;        // rows per CTA of the 128-thread recurrences: 1 (default), 2, 0 = 2 when there are more row-CTAs than two per SM hold at once.
-                              // B200, visit 20: two rows per CTA do not pay -- 8m 1 060 vs 1 049 us (k_gru_bwd2 105 -> 86 us alone, k_gru_fwd2 unchanged at 156), 2s3z 438 vs 430
 int g_mx_p2p_ll = 1;          // data-parallel exchange inside k_optim_fused: 1 = flag-in-data lines (no fence / counter / flag hop), 0 = slots + per-rank flags
 int g_mx_mixer_split = 1;      // 1: split mixer (hypernet-forward / core / hypernet-backward kernels) whenever the forked branch is
                                //    in use; 2: always; 0: always the single fused k_mixer
@@ -28,14 +27,13 @@ int g_mx_overlap = 1;          // state-only kernels (weight-image prep, mixer h
                                // kernels: 1 = when the step is latency-bound (rows <= g_mx_overlap_rows), 2 = always, 0 = never
 int g_mx_gru_threads = 0;
 int g_mx_side_prio = 0;         // priority of a learner's forked branch (read when the learner is created): 0 default, 1 lower, -1 higher
-int g_mx_hyper_late = 0;        // 0 (default): the hypernet branch forks before the front kernel; 1: after it, beside the recurrence -- measured slower
-                                // (3m 198.7 vs 184.3 us, MPE 159.7 vs 128.2 us, profiles/r02_option_sweeps.md: the recurrence is the kernel that suffers most from co-residents)
+int g_mx_hyper_late = 0;        // 0 (default): the hypernet branch forks before the front kernel; 1: after it, beside the recurrence
+                                // (the recurrence is the kernel that suffers most from co-resident CTAs)
 int g_mx_mid_fused = 1;        // 1: k_qhead + k_mix_core + k_qhead_bwd as ONE kernel (k_mid) when the split mixer is in use and no debug
                                //    outputs are requested; 0: three launches
 int g_mx_gru_fwd_rpc = 0;      // tuning overrides: sequence rows per CTA of the recurrence kernels (0 = automatic; 1, 2 or 4)
 int g_mx_gru_bwd_rpc = 0;
-int g_mx_overlap_rows = 1 << 20; // measured on B200 with the fused k_mid in place (profiles/r02_option_sweeps.md, visit 12): forked branch 3m +16 %, 2s3z (19 360 rows) +12 %,
-                               // 8m (61 952 rows) +7 %; round 1 (without k_mid for 8 agents) had 8m at -8 % and a 12 288-row limit.  Beyond 1M rows: unmeasured, serial
+int g_mx_overlap_rows = 1 << 20; // forked branch up to this many rows, serial beyond (not yet measured on the H100)
 int mx_set_option_common(const char* name, int value) {
   if (!strcmp(name, "mixer_split")) { g_mx_mixer_split = value; return 0; }
   if (!strcmp(name, "mixer_split_rm")) { g_mx_mixer_split_rm = value; return 0; }

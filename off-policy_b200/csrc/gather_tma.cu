@@ -213,8 +213,8 @@ int g_mx_gather_tma = 1;
 int mx_launch_gather_tma(void* p, const int64_t* idx_dev, int B, cudaStream_t s) {
   if (!p || !g_mx_gather_tma) return -1;
   MxGatherTma* g = reinterpret_cast<MxGatherTma*>(p);
-  // Measured (tools/gather_sweep.py, 8m shapes, profiles/README.md): the TMA copy wins for small batches (B = 64: 65 % vs 61 % of the HBM peak),
-  // the vectorised loads for large ones (B = 1024: 83 % vs 93 %); crossover near 100 MB per gather.  gather_tma = 2 forces TMA at any size.
+  // The TMA copy is for small batches, the vectorised loads for large ones (tools/gather_sweep.py measures the crossover; the 96 MB
+  // threshold is not yet measured on the H100).  gather_tma = 2 forces TMA at any size.
   if (g_mx_gather_tma == 1 && (long long)g->bytes_per_episode * B > (96ll << 20)) return -1;
   GatherTmaArgs a = g->args;
   a.B = B;

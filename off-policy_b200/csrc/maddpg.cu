@@ -351,7 +351,7 @@ struct MxMaddpgWs {
   // actor-phase branch (rows Mr = N*B*T)
   int64_t r_x, r_h0, r_gi, r_h, r_u1, r_u2, r_st0, r_st1, r_st2, r_sto, r_gates, r_hn, r_q, r_dout, r_dh, r_dgi, r_dx;
   int64_t gpart_a, gpart_c, grad_a, grad_c, spart, info, prio, adam_ta, adam_tc, scal_c, scal_a;
-  int64_t tc_da2, tc_da1, tc_imgT;      // scratch of the tensor-core backward (option wgrad_tc), shared by the critic and actor updates
+  int64_t tc_da2, tc_da1, tc_imgT, tc_acc, tc_acc_cols;      // scratch of the tensor-core backward (option wgrad_tc), shared by the critic and actor updates
   int64_t cent_acts, cent_nacts;        // [B*T][ca_ld] centralised action vectors assembled from all policies (cent_act_dim > 0)
   int64_t total;
 };
@@ -459,6 +459,7 @@ static int64_t maddpg_ws_layout(const mx_maddpg_cfg* c, int64_t Pa, int64_t Pc, 
     const int64_t Mx = Ma > Mc ? Ma : Mc;
     const size_t ia = mx_tc_imageT_floats(c->obs_dim), ic = mx_tc_imageT_floats(critic_in_dim(c));
     W->tc_da2 = tk(Mx * MX_H); W->tc_da1 = tk(Mx * MX_H); W->tc_imgT = tk((int64_t)(ia > ic ? ia : ic));
+    W->tc_acc = tk((int64_t)mx_tc_acc_floats(Mx)); W->tc_acc_cols = (int64_t)mx_tc_acc_floats(Mx) / 128;
   }
   {
     const int64_t ca_ld = c->cent_act_dim > 0 ? mx_round_up(c->cent_act_dim, 4) : 0;
@@ -579,6 +580,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   // ---------- A. actor: live + target over the T+1 steps ----------
   FrontFwdArgs ff;
   memset(&ff, 0, sizeof(ff));
+  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
   ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
   ff.theta[0] = h->th_a; ff.theta[1] = h->th_a_tgt; ff.L = LA;
   ff.gi[0] = ws + W.a_gi[0]; ff.gi[1] = ws + W.a_gi[1];
@@ -615,6 +617,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
   FrontFwdArgs fc;
   memset(&fc, 0, sizeof(fc));
+  fc.tc_acc = ws + W.tc_acc; fc.tc_acc_cols = (int)W.tc_acc_cols;
   fc.X = ws + W.c_x; fc.ldx = ldc; fc.M = Mc; fc.feature_norm = c.no_feature_norm ? 0 : 1; fc.act_tanh = c.use_tanh;
   fc.theta[0] = h->th_c; fc.theta[1] = h->th_c_tgt; fc.L = LC;
   fc.gi[0] = ws + W.c_gi[0]; fc.gi[1] = ws + W.c_gi[1];
@@ -637,6 +640,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
   FrontFwdArgs ft;
   memset(&ft, 0, sizeof(ft));
+  ft.tc_acc = ws + W.tc_acc; ft.tc_acc_cols = (int)W.tc_acc_cols;
   ft.X = ws + W.t_x; ft.ldx = ldc; ft.M = Mc; ft.feature_norm = c.no_feature_norm ? 0 : 1; ft.act_tanh = c.use_tanh; ft.theta[0] = h->th_c_tgt; ft.L = LC; ft.gi[0] = ws + W.t_gi;
   if (mx_launch_front_fwd(ft, 1, s)) return 1;
   GruFwdArgs gt;
@@ -675,6 +679,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   fb.u1 = fc.u1; fb.u2 = fc.u2; fb.st0 = fc.st0; fb.st1 = fc.st1; fb.st2 = fc.st2; fb.dgi = gb.dgi; fb.gates = gc.gates; fb.hall = gc.hall[0];
   fb.gpart = ws + W.gpart_c; fb.P = h->Pc;
   fb.da2_out = ws + W.tc_da2; fb.da1_out = ws + W.tc_da1; fb.tc_imgT = ws + W.tc_imgT;      // (option wgrad_tc)
+  fb.tc_acc = ws + W.tc_acc; fb.tc_acc_cols = (int)W.tc_acc_cols;
   if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
   if (optimise(h, false, parts, head_grid, s)) return 1;
 
@@ -683,6 +688,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     // live critic recurrence over the buffer sequence again (its parameters just changed)
     FrontFwdArgs f2;
     memset(&f2, 0, sizeof(f2));
+    f2.tc_acc = ws + W.tc_acc; f2.tc_acc_cols = (int)W.tc_acc_cols;
     f2.X = ws + W.c_x; f2.ldx = ldc; f2.M = Mc; f2.feature_norm = c.no_feature_norm ? 0 : 1; f2.act_tanh = c.use_tanh; f2.theta[0] = h->th_c; f2.L = LC; f2.gi[0] = ws + W.c_gi[0];
     if (mx_launch_front_fwd(f2, 1, s)) return 1;
     GruFwdArgs g2;
@@ -701,6 +707,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mr * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
     FrontFwdArgs fr;
     memset(&fr, 0, sizeof(fr));
+    fr.tc_acc = ws + W.tc_acc; fr.tc_acc_cols = (int)W.tc_acc_cols;
     fr.X = ws + W.r_x; fr.ldx = ldc; fr.M = Mr; fr.feature_norm = c.no_feature_norm ? 0 : 1; fr.act_tanh = c.use_tanh; fr.theta[0] = h->th_c; fr.L = LC; fr.gi[0] = ws + W.r_gi;
     fr.u1 = ws + W.r_u1; fr.u2 = ws + W.r_u2; fr.st0 = ws + W.r_st0; fr.st1 = ws + W.r_st1; fr.st2 = ws + W.r_st2;
     if (mx_launch_front_fwd(fr, 1, s)) return 1;
@@ -753,6 +760,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     fba.u1 = ff.u1; fba.u2 = ff.u2; fba.st0 = ff.st0; fba.st1 = ff.st1; fba.st2 = ff.st2; fba.dgi = gba.dgi; fba.gates = gf.gates; fba.hall = gf.hall[0];
     fba.gpart = ws + W.gpart_a; fba.P = h->Pa;
     fba.da2_out = ws + W.tc_da2; fba.da1_out = ws + W.tc_da1; fba.tc_imgT = ws + W.tc_imgT;
+    fba.tc_acc = ws + W.tc_acc; fba.tc_acc_cols = (int)W.tc_acc_cols;
     int aparts[2] = {0, 0};
     if (mx_launch_front_bwd(fba, &aparts[0], s)) return 1;
     if (optimise(h, true, aparts, ahead_grid, s)) return 1;
@@ -801,6 +809,7 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
   const MxNetLayout& LA = src->actor;
   FrontFwdArgs ff;
   memset(&ff, 0, sizeof(ff));
+  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
   ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
   ff.theta[0] = src->th_a_tgt; ff.L = LA; ff.gi[0] = ws + W.a_gi[1];
   if (mx_launch_front_fwd(ff, 1, s)) return 1;

@@ -1,7 +1,7 @@
-// Common device/host helpers for the B200 (sm_100a) off-policy MARL update engine.
+// Common device/host helpers for the H100 (sm_90a) off-policy MARL update engine.
 //
 // Build modes:
-//   * product:  nvcc -gencode arch=compute_100a,code=sm_100a  (the only thing shipped / loaded / timed)
+//   * product:  nvcc -gencode arch=compute_90a,code=sm_90a  (the only thing shipped / loaded / timed)
 //   * MARL_EMU: g++ with tests/emu/emu_runtime.h -- CPU fiber emulation of the SIMT kernels, used by the
 //               `-m "not gpu"` unit tests only (kernel-logic checks in a container without a GPU).
 #pragma once
@@ -20,7 +20,7 @@
 
 // Programmatic dependent launch (PDL).  A kernel launched with MX_LAUNCH_PDL may begin while its stream predecessor is still
 // running; everything it does before MX_PDL_WAIT() overlaps the predecessor's tail, so that part may only touch state the
-// predecessor does not write: its own shared memory / TMEM and the parameter vectors theta / theta_target.  Those are written
+// predecessor does not write: its own shared memory / tensor-core accumulator and the parameter vectors theta / theta_target.  Those are written
 // only by the optimiser kernels, which call MX_PDL_THETA_WRITTEN() so that the NEXT launch is a plain, fully ordered one.
 // MX_PDL_WAIT() = griddepcontrol.wait (returns at once in a plain launch) followed by launch_dependents, i.e. a dependent may
 // start as soon as every CTA of this grid is past its own wait -- never before this grid's predecessor has completed.
@@ -180,21 +180,9 @@ MX_DEVINL float mx_rcp(float x) {
 MX_DEVINL float mx_sigmoid_fast(float x) { return mx_rcp(1.0f + mx_ex2(-1.4426950408889634f * x)); }
 MX_DEVINL float mx_tanh_fast(float x) { return fmaf(2.0f, mx_rcp(1.0f + mx_ex2(-2.8853900817779268f * x)), -1.0f); }   // 2*sigmoid(2x) - 1
 
-// packed two-lane fp32 FMA (Blackwell FFMA2: one issue slot for two multiply-adds)
-MX_DEVINL float2 mx_ffma2(float2 a, float2 b, float2 c) {
-#if MX_EMU
-  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#else
-  return __ffma2_rn(a, b, c);
-#endif
-}
-MX_DEVINL float2 mx_fadd2(float2 a, float2 b) {
-#if MX_EMU
-  return make_float2(a.x + b.x, a.y + b.y);
-#else
-  return __fadd2_rn(a, b);
-#endif
-}
+// two-lane fp32 FMA / add on float2 (sm_90 has no packed FFMA2: two FFMAs, the same rounding per lane)
+MX_DEVINL float2 mx_ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+MX_DEVINL float2 mx_fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 
 // LayerNorm statistics the way ATen's CPU/CUDA kernels define them: biased variance, eps inside the sqrt.
 #define MX_LN_EPS 1e-5f

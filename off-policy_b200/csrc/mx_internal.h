@@ -106,6 +106,7 @@ struct MxQmixWs {           // offsets in floats into the workspace
   int64_t tcimg[2];         // pre-split TF32 weight images of the agent front layers (live, target)
   int64_t xin;              // prev_act_inp: packed network input rows [M][round_up(O + A, 4)]
   int64_t tcimgT;           // transposed TF32 weight images for k_front_bwd_tc
+  int64_t tcacc, tcacc_cols; // tensor-core accumulators (mx_tc_acc_floats of the largest batch) and their columns
   int64_t da2, da1;         // [M][H] each: row gradients handed from k_front_bwd to k_wgrad_tc (option wgrad_tc)
   // split mixer pipeline: per-element hypernet outputs (live: kept for backward; target: forward only) and core's gradients
   int64_t hyp_h1, hyp_h2, hyp_hb;               // live [E][gH]

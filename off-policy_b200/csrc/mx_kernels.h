@@ -11,10 +11,14 @@ struct FrontFwdArgs {
   float* gi[2];            // [M][3H]
   float *u1, *u2;          // live: post-ReLU pre-LN activations [M][H]
   float *st0, *st1, *st2;  // live: (mean, rstd) per row for the three LayerNorms
-  const float* tc_img[2];  // optional: pre-split TF32 hi/lo weight images in UMMA layout (mx_launch_tc_prep_weights)
+  const float* tc_img[2];  // optional: pre-split TF32 hi/lo weight images in the wgmma operand layout (mx_launch_tc_prep_weights)
+  float* tc_acc;           // with tc_img: the tensor-core accumulators, tc_acc_cols x 128 floats (CTAs x columns per CTA <= tc_acc_cols)
+  int tc_acc_cols;
   int act_tanh;            // 1: tanh instead of ReLU after fc1 / fc2 (--use_ReLU switched off)
 };
 size_t mx_tc_image_floats(int in_dim);
+// accumulator floats a learner's tensor-core launches over at most M rows need (FrontFwdArgs / FrontBwdArgs tc_acc); columns = floats / 128
+size_t mx_tc_acc_floats(int64_t M);
 int mx_launch_tc_prep_weights(const float* const theta[2], const MxNetLayout& L, float* const img[2], int nets, cudaStream_t s);
 size_t mx_front_fwd_smem(int in_dim, int RM);
 int mx_launch_front_fwd(const FrontFwdArgs& a, int nets, cudaStream_t s);
@@ -171,6 +175,8 @@ struct FrontBwdArgs {
   int use_mma;             // set by the launcher: GEMMs of k_front_bwd on mma.sync 3xTF32 tiles (mx_mma.cuh) instead of the FFMA micro-kernels
   float* tc_imgT;          // scratch for the transposed TF32 weight images of the all-tensor-core backward (option wgrad_tc = 2)
   int tc_imgT_ready;       // 1: the caller already built them for the current parameters (mx_launch_tc_prep_weights_T)
+  float* tc_acc;           // with tc_imgT or the tensor-core weight gradients: accumulators, as FrontFwdArgs::tc_acc
+  int tc_acc_cols;
   int act_tanh;            // 1: tanh instead of ReLU (the saved u1 / u2 are the activations' outputs: tanh' = 1 - u^2)
   float* ln_part;          // optional [ln_part_rows][512] side array: lets k_front_bwd_tc run more CTAs than there are gradient partial rows (streamed mode)
   int ln_part_rows;

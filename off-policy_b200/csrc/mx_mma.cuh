@@ -1,6 +1,6 @@
 // Warp-level tensor-core tiles for the FP32-accurate backward GEMMs: mma.sync.m16n8k8 TF32 with the 3xTF32 split
 // (hi = cvt.rna.tf32(x), lo = x - hi; D += lo*hi + hi*lo + hi*hi, fp32 accumulate in registers: relative error ~2^-21, the same
-// accuracy class as the tcgen05 forward).  The FFMA micro-kernels of mx_tile.cuh are bound by the shared-memory pipe (one 16-byte
+// accuracy class as the wgmma forward).  The FFMA micro-kernels of mx_tile.cuh are bound by the shared-memory pipe (one 16-byte
 // load per 6-8 FFMAs, and a wide load occupies the LSU for four cycles); a fragment loaded once here feeds 3 x 1024 MACs.
 //
 // Fragment layout of mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 (g = lane >> 2, t = lane & 3):

@@ -161,6 +161,7 @@ static int64_t ws_layout(const mx_qmix_cfg* c, int64_t P, int npart, MxQmixWs* W
   W->xin = tk(c->prev_act_inp ? M * mx_round_up(agent_in_dim(c), 4) : 0);
   W->da2 = tk(M * MX_H); W->da1 = tk(M * MX_H);
   W->tcimgT = tk((int64_t)mx_tc_imageT_floats(agent_in_dim(c)));
+  W->tcacc = tk((int64_t)mx_tc_acc_floats(M)); W->tcacc_cols = (int64_t)mx_tc_acc_floats(M) / 128;
   {
     const int64_t gH = mx_round_up(c->hyper_hidden, 4), gM = mx_round_up(c->mixer_hidden, 4), gP = mx_round_up(c->n_agents * c->mixer_hidden, 4);
     const int64_t En = c->vdn ? 0 : E;
@@ -397,6 +398,7 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
       q->prep_pending = 0;
     } else if (launch_prep(q, s)) return 1;
     ff.tc_img[0] = ws + W.tcimg[0]; ff.tc_img[1] = ws + W.tcimg[1];
+    ff.tc_acc = ws + W.tcacc; ff.tc_acc_cols = (int)W.tcacc_cols;
   }
   // the mixer's hypernetworks depend on the sampled states and the parameters only: forked branch beside the agent nets.
   // Default: fork before the front kernel.  hyper_late = 1 moves the fork AFTER the tensor-core front kernel (which fills an SM's shared
@@ -443,6 +445,7 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
     fbm.dgi = ws + W.dgi; fbm.gpart = mx.gpart; fbm.P = q->P;
     fbm.ln_part = ws + W.lnpart; fbm.ln_part_rows = 2 * q->npart;
     fbm.da2_out = ws + W.da2; fbm.da1_out = ws + W.da1; fbm.tc_imgT = ws + W.tcimgT; fbm.tc_imgT_ready = q->imgT_fresh; q->imgT_fresh = 0;      // (option wgrad_tc)
+    fbm.tc_acc = ws + W.tcacc; fbm.tc_acc_cols = (int)W.tcacc_cols;
     if (mx_launch_front_bwd(fbm, &parts[0], s)) return 1;
 #if !MX_EMU
     if (split && overlap) join_from_side(q, q->ev_hbwd, s);
@@ -527,6 +530,7 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
   fb.dgi = gb.dgi; fb.gates = gf.gates; fb.hall = gf.hall[0]; fb.gpart = mx.gpart; fb.P = q->P;
   fb.ln_part = ws + W.lnpart; fb.ln_part_rows = 2 * q->npart;
   fb.da2_out = ws + W.da2; fb.da1_out = ws + W.da1; fb.tc_imgT = ws + W.tcimgT; fb.tc_imgT_ready = q->imgT_fresh; q->imgT_fresh = 0;      // used when the tensor-core weight-gradient kernel is enabled (option wgrad_tc)
+  fb.tc_acc = ws + W.tcacc; fb.tc_acc_cols = (int)W.tcacc_cols;
   const bool gsplit = mx_gru_wgrad_split_usable(fb);      // GRU weight gradients as their own kernel, beside k_front_bwd when forked
   if (gsplit) {
     fb.gru_wgrad_ext = 1;

@@ -1,4 +1,4 @@
-// Weight gradients of the agent network's time-batched layers on tcgen05 (3xTF32): k_wgrad_tc.
+// Weight gradients of the agent network's time-batched layers on the wgmma tensor cores (3xTF32): k_wgrad_tc.
 //
 //   dW_ih = dgi^T x2     dW_hh = [dgi_r, dgi_z, dgi_n * r]^T h_{t-1}     dW2 = da2^T x1     dW1 = da1^T x0     + every bias gradient
 //
@@ -7,7 +7,7 @@
 // L2-resident activations, TF32 hi / lo split, two 16-byte stores into the core-matrix layout; within a warp the 32 pairs are
 // (8 features) x (4 row quads), which is 512 contiguous bytes of the tile -- no bank conflicts, every store a full wavefront.
 // Normalised activations (x2, x1, x0) are recomputed from the saved pre-norm rows and statistics while staging; bias gradients fall out
-// of a column of ones appended to B.  Three accumulators live in TMEM for the whole CTA (rows are split over CTAs in chunks of 64):
+// of a column of ones appended to B.  Three accumulators live in the CTA's accumulator (mx_tc.cuh) for the whole CTA (rows are split over CTAs in chunks of 64):
 //   D1[128][144] = [dgi_r | dgi_z]^T     . [x2 | h_prev | 1]   -> dW_ih[0:128], dW_hh[0:128], db_ih[0:128] (= db_hh[0:128])
 //   D2[128][144] = [dgi_n | dgi_n * r]^T . [x2 | h_prev | 1]   -> dW_ih[128:192] (rows 0-63, cols 0-63), dW_hh[128:192] (rows 64-127, cols 64-127)
 //   D3[128][..]  = [da2   | da1]^T       . [x1 | x0]           -> dW2 (rows 0-63, cols 0-63), dW1 (rows 64-127, cols 64..)
@@ -20,15 +20,15 @@
 
 #include <string.h>
 
-int g_mx_wgrad_tc = -1;       // -1 (default): by input width -- measured on B200 (profiles/r02_option_sweeps.md): inputs <= 64 (3m, MPE) are faster on the
-                              // FFMA backward (185 vs 212 us), wider inputs (8m / 2s3z, obs 80) on k_front_bwd_tc + k_wgrad_tc (1.51 vs 1.59 ms); 0 / 1 / 2 force a mode
+int g_mx_wgrad_tc = -1;       // -1 (default): by input width -- inputs <= 64 (3m, MPE) on the FFMA backward, wider inputs (8m / 2s3z, obs 80) on
+                              // k_front_bwd_tc + k_wgrad_tc (split not yet measured on the H100); 0 / 1 / 2 force a mode
 static inline int wgrad_mode(int in_dim) { return g_mx_wgrad_tc >= 0 ? g_mx_wgrad_tc : (in_dim > 64 ? 2 : 0); }
 int g_mx_wgrad_tc_wide = 1;   // with wgrad_tc: input widths 65 .. 112 too (SMAC 8m / 2s3z observations are 80 wide)
 
 #define WG_ROWS 64            // rows per MMA group (the K extent of one staged tile)
-#define WG_DSTRIDE 160        // TMEM column stride between the three accumulators
+#define WG_DSTRIDE 160        // accumulator column stride between the three accumulators
 
-#define WG_MAX_IN 128          // input widths up to here: D3 = [x1 | x0] is 64 + round_up(I, 16) <= 192 columns, the rest of TMEM
+#define WG_MAX_IN 128          // input widths up to here: D3 = [x1 | x0] is 64 + round_up(I, 16) <= 192 columns, the rest of the 512 accumulator columns
 #define WG_ONES_COL 144        // db2 / db1 = [da2 | da1]^T . 1: a 16-column accumulator in the padding between D1 (144 wide) and D2 (at 160)
 struct WgradSmem { int o_ahi, o_alo, o_bhi, o_blo, o_ones, total; };
 static WgradSmem wgrad_smem(int n3) {
@@ -67,7 +67,7 @@ struct WgradArgs {
   int ln_parts;          // > 0: k_front_bwd_tc left its LayerNorm sums in f.ln_part[ln_parts][512] (streamed mode) instead of the partial rows
 };
 
-#define WG_THREADS 512        // staging is load-latency bound: 16 warps keep enough loads in flight; warps 0-3 own the TMEM lanes in the epilogue
+#define WG_THREADS 512        // staging is load-latency bound: 16 warps keep enough loads in flight; warps 0-3 own the accumulator rows in the epilogue
 __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSmem sm, int swap_ls) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
@@ -84,9 +84,9 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo, *b_hi = base + sm.o_bhi, *b_lo = base + sm.o_blo;
   char *o_hi = base + sm.o_ones, *o_lo = o_hi + 16 * WG_ROWS * 4;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<512>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<512>(&tmem_s, tc::cta_slice(a.tc_acc, 512));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   for (int i = tid; i < 64; i += blockDim.x) {
@@ -189,7 +189,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer_acc(tmem_base + pass * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, 144, WG_ROWS, swap_ls, acc0, bar);
+      tc::issue_layer_acc(tmem_base + pass * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, 144, WG_ROWS, swap_ls, acc0, bar);
       tc::mbar_wait(bar, phase);      // the MMAs have read the tiles: A (and after the second pass B) may be refilled
       phase ^= 1;
       tc::fence_after();
@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
     tc::fence_before();
     __syncthreads();
     tc::fence_after();
-    if (tid == 0) {
+    {
       tc::issue_layer_acc(tmem_base + 2 * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, N3, WG_ROWS, swap_ls, acc0, bar, false);
       tc::issue_layer_acc(tmem_base + WG_ONES_COL, a_hi, a_lo, o_hi, o_lo, 16, WG_ROWS, swap_ls, acc0, bar, true);      // one commit for both
     }
@@ -279,7 +279,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
   float* gp = a.gpart + (size_t)blockIdx.x * a.P;
   if (warp < 4) {
   const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-  const bool any = iter > 0;      // a CTA without rows writes zeros (its TMEM was never written)
+  const bool any = iter > 0;      // a CTA without rows writes zeros (its accumulator was never written)
   const int r = tid;
   float v[64];
   float t[32];
@@ -355,6 +355,10 @@ extern int g_mx_tc_swap;
 static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, cudaStream_t s, int ln_parts = 0);
 int mx_launch_wgrad_tc(const FrontBwdArgs& a, int nparts, cudaStream_t s) { return launch_wgrad_tc(a, nparts, -1, s); }
 static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, cudaStream_t s, int ln_parts) {
+  {   // CTAs beyond the last 64-row chunk have no rows and never touch their accumulator
+    const int busy = nparts < mx_ceil_div(a.M, WG_ROWS) ? nparts : mx_ceil_div(a.M, WG_ROWS);
+    if (!a.tc_acc || (int64_t)busy * 512 > a.tc_acc_cols) { mx_set_error("wgrad_tc: accumulator region missing or too small"); return 1; }
+  }
   WgradArgs w;
   w.f = a;
   w.ln_zero_from = ln_zero_from;
@@ -377,10 +381,10 @@ static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, 
 
 
 // =====================================================================================================
-// k_front_bwd_tc: the data-gradient chain of the front layers on tcgen05 (option wgrad_tc = 2; with k_wgrad_tc it replaces
+// k_front_bwd_tc: the data-gradient chain of the front layers on wgmma (option wgrad_tc = 2; with k_wgrad_tc it replaces
 // k_front_bwd for input widths <= 64).  Mirror image of k_front_fwd_tc: a 128-row tile per CTA, thread r owns row r, so the three
-// LayerNorm backward passes and ReLU masks run on registers after tcgen05.ld:
-//   dx2 = dgi . W_ih (K = 192 fed as three gate chunks that accumulate in TMEM) -> LN2' , ReLU' -> da2
+// LayerNorm backward passes and ReLU masks run on registers after the accumulator row is read:
+//   dx2 = dgi . W_ih (K = 192 fed as three gate chunks that accumulate) -> LN2' , ReLU' -> da2
 //   dx1 = da2 . W2 -> LN1', ReLU' -> da1 ;  dx0 = da1 . W1 -> the feature LayerNorm's gain / bias gradients
 // B operands are TRANSPOSED weight images (k_tc_prep_weights_T).  da2 / da1 go to global memory for k_wgrad_tc.  LayerNorm gain / bias
 // gradients are column sums over rows = over threads: each tile writes [dy * xhat | dy] through an XOR-swizzled scratch (the A
@@ -511,9 +515,9 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
   const bool restage = !stream && sm.o_w1 == sm.o_w2;
   const float* img_w2 = a.tc_imgT + 2 * 3 * 4096;
   const float* img_w1 = img_w2 + 2 * 4096;
-  if (warp == 0) tc::tmem_alloc<128>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<128>(&tmem_s, tc::cta_slice(a.tc_acc, 128));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   for (int i = tid; i < 64; i += blockDim.x) { par_s[i] = th[L.ln2_g + i]; par_s[64 + i] = th[L.ln1_g + i]; }
@@ -557,7 +561,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
       __syncthreads();
       tc::fence_after();
       const char* wch = stream ? wih : wih + ch * 2 * 4096 * 4;
-      if (tid == 0) tc::issue_layer_acc(tmem_base, a_hi, a_lo, wch, wch + 4096 * 4, 64, 64, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::issue_layer_acc(tmem_base, a_hi, a_lo, wch, wch + 4096 * 4, 64, 64, swap_ls, ch > 0 ? 1u : 0u, bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
       tc::fence_after();
@@ -591,7 +595,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) {
+      {
         if (layer == 0) tc::issue_layer(tmem_base, a_hi, a_lo, w2, w2 + 4096 * 4, 64, 64, 3, swap_ls, bar);
         else tc::issue_layer(tmem_base, a_hi, a_lo, w1, w1 + Kp16 * 64 * 4, Kp16, 64, 3, swap_ls, bar);
       }
@@ -628,7 +632,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
       }
     }
     tc::fence_before();
-    __syncthreads();     // TMEM reads drained before the next tile's MMAs
+    __syncthreads();     // accumulator reads drained before the next tile's MMAs
     tc::fence_after();
   }
   // ---- this CTA's partial of the LayerNorm gain / bias gradients ----
@@ -688,6 +692,9 @@ int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t
   if (stream && 2 * (sm.total + 2048) <= 227 * 1024) ga = 2 * mx_num_sms();      // two CTAs per SM fit
   if (ga > ntiles) ga = ntiles;
   if (gb > nchunks) gb = nchunks;
+  if (!a.tc_acc || a.tc_acc_cols < 512) { mx_set_error("front_bwd_tc: accumulator region missing or too small"); return 1; }
+  if (ga * 128 > a.tc_acc_cols) ga = a.tc_acc_cols / 128;      // accumulator columns per CTA: 128 here, 512 in k_wgrad_tc
+  if (gb * 512 > a.tc_acc_cols) gb = a.tc_acc_cols / 512;
   FrontBwdArgs b = a;
   b.wgrad_external = 1;
   if (!stream) b.ln_part = nullptr;

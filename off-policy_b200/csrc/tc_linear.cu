@@ -1,22 +1,23 @@
-// tcgen05 (5th-generation tensor core) dense layer with fp32-level accuracy: Y[M][N] = X[M][K] . W[N][K]^T (+ bias)
+// Tensor-core (wgmma) dense layers with fp32-level accuracy: Y[M][N] = X[M][K] . W[N][K]^T (+ bias)
 //
 // Operands are split on the fly into TF32 hi / lo parts (hi = cvt.rna.tf32, lo = x - hi) and three MMAs accumulate
-// hi*hi + lo*hi + hi*lo in the fp32 TMEM accumulator ("3xTF32": relative error ~2^-21, inside the 1e-4 gradient parity
-// budget that rules single-pass TF32/BF16 out).  One CTA = one 128-row tile (UMMA M = 128, cta_group::1), 128 threads:
-//   threads  : fill A (and W) hi/lo tiles in shared memory in the canonical K-major no-swizzle core-matrix layout
-//              (8 rows x 16 bytes per core matrix), fence.proxy.async, barrier
-//   thread 0 : K/8 x 3 tcgen05.mma.kind::tf32 (operands straight from shared memory), tcgen05.commit -> mbarrier
-//   all      : mbarrier wait, tcgen05.ld (thread = accumulator row), epilogue, coalesced-enough global stores
-// This file holds the building block and a probe entry point (mx_tc_linear_probe) used by the GPU tests to pin the
-// descriptor conventions against an fp64 reference; the front-layer kernels are built on the same helpers.
+// hi*hi + lo*hi + hi*lo in fp32 ("3xTF32": relative error ~2^-21, inside the 1e-4 gradient parity budget that rules single-pass
+// TF32/BF16 out).  One CTA = one 128-row tile:
+//   all threads : fill A (and W) hi/lo tiles in shared memory in the canonical K-major no-swizzle core-matrix layout
+//                 (8 rows x 16 bytes per core matrix), fence.proxy.async, barrier
+//   warpgroups  : wgmma.mma_async m64nNk8 kind tf32 over their share of the tile (mx_tc.cuh), fragments -> the CTA's accumulator,
+//                 mbarrier arrival
+//   all threads : mbarrier wait, read the accumulator row (thread = row), epilogue, global stores
+// This file holds the front-layer kernels and a probe entry point (mx_tc_linear_probe) used by the GPU tests to pin the
+// descriptor conventions against an fp64 reference.
 #include "mx_internal.h"
 
 #include "mx_tc.cuh"
 #include <string.h>
 
 // =====================================================================================================
-// front forward on tcgen05: LN -> fc1 -> ReLU -> LN -> fc2 -> ReLU -> LN -> W_ih for a 128-row tile per CTA.
-// Thread r owns accumulator row r (TMEM lane r): after tcgen05.ld a whole 64-wide layer output sits in that thread's
+// front forward on the tensor cores: LN -> fc1 -> ReLU -> LN -> fc2 -> ReLU -> LN -> W_ih for a 128-row tile per CTA.
+// Thread r owns accumulator row r: after tmem_ld64 a whole 64-wide layer output sits in that thread's
 // registers, so bias / ReLU / LayerNorm need no cross-thread traffic at all; the normalised row is split into TF32
 // hi/lo and written straight back into the A operand tiles for the next layer.
 // =====================================================================================================
@@ -45,7 +46,7 @@ __device__ __forceinline__ void tc_stage_weight(char* hi, char* lo, const float*
   }
 }
 
-// Weight images: [w1 hi | w1 lo | w2 hi | w2 lo | w_ih hi | w_ih lo], each already in the UMMA core-matrix layout, so a CTA
+// Weight images: [w1 hi | w1 lo | w2 hi | w2 lo | w_ih hi | w_ih lo], each already in the wgmma core-matrix layout, so a CTA
 // stages all three layers with straight 16-byte cp.async copies (no per-CTA conversion).  Rebuilt once per step.
 struct TcPrepArgs { const float* th[2]; float* img[2]; };
 // fc1 image: in_dim <= 64: one [64][Kp] tile.  64 < in_dim <= 128 ("wide"): K is fed in chunks of 64 columns, each chunk its own
@@ -81,6 +82,11 @@ __global__ void __launch_bounds__(256) k_tc_prep_weights(TcPrepArgs p, MxNetLayo
   }
 }
 
+size_t mx_tc_acc_floats(int64_t M) {
+  // the widest user is k_wgrad_tc: 512 columns per CTA, at most one CTA per 64-row chunk (the forward: 2 nets x 256 per 128-row tile)
+  const int64_t need = (M > 0 ? (M + 63) / 64 : 1) * 512;
+  return (size_t)(need < MX_TC_ACC_SLOTS ? need : MX_TC_ACC_SLOTS) * 128;
+}
 size_t mx_tc_image_floats(int in_dim) {
   const int Kp = mx_round_up(in_dim, 8);
   return (size_t)2 * (MX_H * Kp + MX_H * MX_H + MX_G * MX_H);
@@ -146,9 +152,9 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w1l = base + sm.o_w1l, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   for (int i = tid; i < MX_H; i += blockDim.x) {
@@ -157,7 +163,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
     par_s[6 * MX_H + MX_G + i] = i < I ? th[L.fn_g + i] : 0.f; par_s[6 * MX_H + MX_G + 64 + i] = i < I ? th[L.fn_b + i] : 0.f;
   }
   for (int i = tid; i < MX_G; i += blockDim.x) par_s[6 * MX_H + i] = th[L.bih + i];
-  MX_PDL_WAIT();        // TMEM, the mbarrier and the parameter rows are private / parameter data; the images and inputs are not
+  MX_PDL_WAIT();        // the accumulator address, the mbarrier and the parameter rows are private / parameter data; the images and inputs are not
   if (a.tc_img[net]) {
     // the image is byte-identical to the shared-memory weight region: straight 16-byte async copies
     // two groups: fc1+fc2 first, W_ih (two thirds of the bytes) lands while the first two layers run
@@ -177,7 +183,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
   const float* fng_s = par_s + 6 * MX_H + MX_G;
   const float* fnb_s = fng_s + 64;
   tc::fence_before();
-  __syncthreads();        // parameters, TMEM address and the mbarrier are visible; the weight copies are still in flight
+  __syncthreads();        // parameters, accumulator address and the mbarrier are visible; the weight copies are still in flight
   tc::fence_after();
   const uint32_t tmem_base = tmem_s;
   const uint32_t tmem_row = tmem_base + ((uint32_t)(warp * 32) << 16);
@@ -225,7 +231,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
+      tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
       tc::fence_after();
@@ -253,7 +259,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
     tc::fence_before();
     __syncthreads();
     tc::fence_after();
-    if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
     tc::fence_after();
@@ -271,7 +277,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
       }
     }
     tc::fence_before();
-    __syncthreads();     // every thread has drained its TMEM reads before the next tile's MMAs overwrite the accumulator
+    __syncthreads();     // every thread has drained its accumulator reads before the next tile's MMAs overwrite the accumulator
     tc::fence_after();
   }
   tc::fence_before();
@@ -281,10 +287,10 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
 
 
 // ---- 256-thread variant: TWO threads per accumulator row ------------------------------------------------------------------------------------
-// Warps w and w + 4 share TMEM lane quadrant w & 3, so thread (r, half) reads columns [32 half, 32 half + 32) of row r: every epilogue
+// Warps w and w + 4 share accumulator row quadrant w & 3, so thread (r, half) reads columns [32 half, 32 half + 32) of row r: every epilogue
 // (bias, activation, LayerNorm, TF32 split, operand write-back, activation stores) is half as long per thread, eight warps instead of four
 // hide each other's latencies, and the unrolled code a warp walks through is half as large (the 128-thread kernel spends ~30 % of its
-// time on instruction-cache misses: profiles/r02c).  LayerNorm statistics cross the pair through shared memory (four values per layer).
+// time on instruction-cache misses).  LayerNorm statistics cross the pair through shared memory (four values per layer).
 __device__ __forceinline__ float tc_pair_sum(float v, float (*ex)[2][128], int& buf, int half, int r) {
   ex[buf][half][r] = v;
   __syncthreads();
@@ -342,9 +348,9 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w1l = base + sm.o_w1l, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   for (int i = tid; i < MX_H; i += blockDim.x) {
@@ -420,7 +426,7 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
+      tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
       tc::fence_after();
@@ -448,7 +454,7 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
     tc::fence_before();
     __syncthreads();
     tc::fence_after();
-    if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
     tc::fence_after();
@@ -477,7 +483,7 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
 
 // =====================================================================================================
 // Wide inputs (64 < in_dim <= 128: SMAC 8m / 2s3z observations): same pipeline, but fc1's K dimension is fed in chunks of 64
-// columns that accumulate in TMEM -- the A tile stays [128][64] and only one fc1 weight chunk is resident (restaged per tile from
+// columns that accumulate in the accumulator -- the A tile stays [128][64] and only one fc1 weight chunk is resident (restaged per tile from
 // the L2-resident image), so that fc2 and W_ih (96 KB as hi / lo) still fit beside them: 224 KB of dynamic shared memory.
 // =====================================================================================================
 __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, FrontTcSmem sm, int swap_ls) {
@@ -496,9 +502,9 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   for (int i = tid; i < MX_H; i += blockDim.x) {
@@ -603,7 +609,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer_acc(tmem_base, a_hi, a_lo, w1h, w1h + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::issue_layer_acc(tmem_base, a_hi, a_lo, w1h, w1h + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
       tc::mbar_wait(bar, phase);        // the MMAs have read the A tile and the weight chunk: both may be refilled
       phase ^= 1;
       tc::fence_after();
@@ -615,7 +621,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
         tc::fence_before();
         __syncthreads();
         tc::fence_after();
-        if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, w2h, w2l, MX_H, MX_H, 3, swap_ls, bar);
+        tc::issue_layer(tmem_base, a_hi, a_lo, w2h, w2l, MX_H, MX_H, 3, swap_ls, bar);
         tc::mbar_wait(bar, phase);
         phase ^= 1;
         tc::fence_after();
@@ -637,7 +643,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
 #pragma unroll
       for (int c = 0; c < 64; ++c) v[c] = (v[c] - mu) * rs * bs[MX_H + c] + bs[2 * MX_H + c];
       tc::fence_before();
-      __syncthreads();          // every thread has drained its TMEM reads before the next layer's MMAs overwrite the accumulator
+      __syncthreads();          // every thread has drained its accumulator reads before the next layer's MMAs overwrite the accumulator
       tc::fence_after();
       tc_put_row64(a_hi, a_lo, tid, v);
     }
@@ -646,7 +652,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
     tc::fence_before();
     __syncthreads();
     tc::fence_after();
-    if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
     tc::fence_after();
@@ -664,7 +670,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
       }
     }
     tc::fence_before();
-    __syncthreads();     // TMEM reads drained; the A tile and the fc1 chunk buffer are free for the next tile
+    __syncthreads();     // accumulator reads drained; the A tile and the fc1 chunk buffer are free for the next tile
     tc::fence_after();
   }
   tc::fence_before();
@@ -675,10 +681,10 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
 // =====================================================================================================
 // k_front_fwd_tc_wide2: the wide-input pipeline with EVERY weight operand streamed through one 32 KB chunk buffer (fc1 chunk 0, fc1
 // chunk 1, fc2, W_ih gate r, z, n -- six [64][K] hi | lo pairs per tile, copied from the L2-resident image with cp.async), so a CTA needs
-// 96 KB of shared memory and 256 TMEM columns and TWO CTAs share an SM: while one waits for an MMA, a copy or its row loads, the other
+// 96 KB of shared memory and 256 accumulator columns and TWO CTAs share an SM: while one waits for an MMA, a copy or its row loads, the other
 // runs its epilogue (ncu on k_front_fwd_tc_wide at 8m: 4 warps per SM, issue-active 11 %, long-scoreboard 5 warps per issue).  The copy
 // of chunk i + 1 is issued as soon as the MMAs of chunk i have completed, i.e. it flies during the epilogue between them; the three gate
-// blocks of gi accumulate in their own TMEM columns, so the epilogue of gate g overlaps the copy of gate g + 1.
+// blocks of gi accumulate in their own accumulator columns, so the epilogue of gate g overlaps the copy of gate g + 1.
 // =====================================================================================================
 struct FrontTcWide2Smem { int o_ahi, o_alo, o_wc, total; };
 static FrontTcWide2Smem front_tc_wide2_smem() {
@@ -704,9 +710,9 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
   char* base = reinterpret_cast<char*>(smem_raw);
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo, *wc = base + sm.o_wc;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s);
+  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
   if (tid == 0) {
-    tc::mbar_init(bar, 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
   float* bih_s = par_s + 6 * MX_H;
@@ -802,7 +808,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer_acc(tmem_base, a_hi, a_lo, wc, wc + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::issue_layer_acc(tmem_base, a_hi, a_lo, wc, wc + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
       tc::mbar_wait(bar, phase);        // the MMAs have read the A tile and the chunk buffer: both may be refilled
       phase ^= 1;
       tc::fence_after();
@@ -817,7 +823,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
         tc::fence_before();
         __syncthreads();
         tc::fence_after();
-        if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
+        tc::issue_layer(tmem_base, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
         tc::mbar_wait(bar, phase);
         phase ^= 1;
         tc::fence_after();
@@ -841,11 +847,11 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
 #pragma unroll
       for (int c = 0; c < 64; ++c) v[c] = (v[c] - mu) * rs * bs[MX_H + c] + bs[2 * MX_H + c];
       tc::fence_before();
-      __syncthreads();          // every thread has drained its TMEM reads before the next layer's MMAs overwrite the accumulator
+      __syncthreads();          // every thread has drained its accumulator reads before the next layer's MMAs overwrite the accumulator
       tc::fence_after();
       tc_put_row64(a_hi, a_lo, tid, v);
     }
-    // ---- gi = x2 . W_ih^T + b_ih, one gate block (64 columns) at a time into TMEM columns 64 + 64 g ----
+    // ---- gi = x2 . W_ih^T + b_ih, one gate block (64 columns) at a time into accumulator columns 64 + 64 g ----
     float* gi = a.gi[net];
 #pragma unroll 1
     for (int g = 0; g < 3; ++g) {
@@ -854,7 +860,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       tc::fence_before();
       __syncthreads();
       tc::fence_after();
-      if (tid == 0) tc::issue_layer(tmem_base + 64 + 64 * g, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
+      tc::issue_layer(tmem_base + 64 + 64 * g, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
       tc::fence_after();
@@ -877,7 +883,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       }
     }
     tc::fence_before();
-    __syncthreads();     // TMEM reads drained; the A tile is free for the next tile
+    __syncthreads();     // accumulator reads drained; the A tile is free for the next tile
     tc::fence_after();
   }
   mx_cp_wait<0>();
@@ -886,10 +892,11 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
   if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
-int g_mx_front_tc = 1;        // 1: tcgen05 3xTF32 kernel (default), 0: FFMA kernel (mx_set_option("front_tc", 0))
+int g_mx_front_tc = 1;        // 1: tensor-core 3xTF32 kernels (default), 0: FFMA kernel (mx_set_option("front_tc", 0))
 int g_mx_front_tc_threads = 256;   // inputs <= 64: 256 = two threads per accumulator row (k_front_fwd_tc2), 128 = one (k_front_fwd_tc)
-int g_mx_front_tc_wide = 1;   // 1 (default): 64 < in_dim <= 128 also runs on tcgen05 (k_front_fwd_tc_wide): 8m 1.76 -> 1.59 ms, 2s3z 0.683 -> 0.647 ms (r02 sweeps)
+int g_mx_front_tc_wide = 1;   // 1 (default): 64 < in_dim <= 128 also runs on the tensor cores (k_front_fwd_tc_wide[2])
 int g_mx_front_tc_wide2 = 1;  // wide inputs: 1 (default) = k_front_fwd_tc_wide2 (weights streamed, two CTAs per SM), 0 = k_front_fwd_tc_wide (weights resident, one CTA per SM)
+                              // (these defaults are not yet measured on the H100)
 int g_mx_tc_swap = 0;
 extern int g_mx_wgrad_tc, g_mx_wgrad_tc_wide, g_mx_front_bwd_tc_stream;      // tc_bwd.cu
 int g_mx_mixer_rm = 0;        // tuning overrides (0 = automatic): rows per thread of the mixer / backward front tiles
@@ -908,6 +915,8 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
   const int ntiles = mx_ceil_div(a.M, 128);
   int gx = mx_num_sms() / nets;
   if (gx > ntiles) gx = ntiles;
+  if (!a.tc_acc || a.tc_acc_cols < 256 * nets) { mx_set_error("front_fwd_tc: accumulator region missing or too small"); return 1; }
+  if (gx * nets * 256 > a.tc_acc_cols) gx = a.tc_acc_cols / (256 * nets);      // 256 accumulator columns per CTA
   if (gx < 1) gx = 1;
   if (wide) {
     if (!a.tc_img[0] || (nets > 1 && !a.tc_img[1])) { mx_set_error("front_fwd_tc_wide: weight images missing"); return 1; }
@@ -915,6 +924,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
       FrontTcWide2Smem s2 = front_tc_wide2_smem();
       int g2 = 2 * mx_num_sms() / nets;
       if (g2 > ntiles) g2 = ntiles;
+      if (g2 * nets * 256 > a.tc_acc_cols) g2 = a.tc_acc_cols / (256 * nets);
       if (g2 < 1) g2 = 1;
 #if !MX_EMU
       static bool configured_w2 = false;
@@ -993,6 +1003,7 @@ struct TcProbeArgs {
   int M, N, K, passes, swap_ls;
 };
 
+// N is taken in blocks of up to 64 columns: the B block and the block's accumulator live in shared memory beside the A tile
 __global__ void __launch_bounds__(128) k_tc_linear_probe(TcProbeArgs a) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
@@ -1002,48 +1013,56 @@ __global__ void __launch_bounds__(128) k_tc_linear_probe(TcProbeArgs a) {
   char* a_hi = reinterpret_cast<char*>(smem_raw);
   char* a_lo = a_hi + 128 * K * 4;
   char* b_hi = a_lo + 128 * K * 4;
-  char* b_lo = b_hi + 256 * K * 4;
+  char* b_lo = b_hi + 64 * K * 4;
+  float* acc = reinterpret_cast<float*>(b_lo + 64 * K * 4);      // [64 columns][128 rows]
   const int m0 = blockIdx.x * 128;
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s);
+  const uint32_t bar = tc::bar_addr(&bar_s);
+  if (warp == 0) tc::tmem_alloc<64>(&tmem_s, acc);
   if (tid == 0) {
-    tc::mbar_init(tc::bar_addr(&bar_s), 1);
+    tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
   }
-  // operand tiles (zero rows beyond M / N)
+  // A tile (zero rows beyond M)
   for (int idx = tid; idx < 128 * K; idx += 128) {
     const int r = idx / K, k = idx % K;
     const float x = (m0 + r < a.M) ? a.X[(size_t)(m0 + r) * K + k] : 0.f;
     tc::put_split(a_hi, a_lo, r, k, K, x);
   }
-  for (int idx = tid; idx < N * K; idx += 128) {
-    const int r = idx / K, k = idx % K;
-    tc::put_split(b_hi, b_lo, r, k, K, a.W[(size_t)r * K + k]);
-  }
-  tc::fence_async_smem();
-  tc::fence_before();
-  __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  if (tid == 0) tc::issue_layer(tmem_base, a_hi, a_lo, b_hi, b_lo, N, K, a.passes, a.swap_ls, tc::bar_addr(&bar_s));
-  tc::mbar_wait(tc::bar_addr(&bar_s), 0);
-  tc::fence_after();
   const int row = m0 + warp * 32 + lane;
-  for (int c0 = 0; c0 < N; c0 += 32) {
-    float v[32];
-    tc::tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-    if (row < a.M)
-      for (int c = 0; c < 32 && c0 + c < N; ++c) a.Y[(size_t)row * N + c0 + c] = v[c];
+  uint32_t phase = 0;
+  for (int n0 = 0; n0 < N; n0 += 64) {
+    const int nc = N - n0 < 64 ? N - n0 : 64;
+    for (int idx = tid; idx < nc * K; idx += 128) {
+      const int r = idx / K, k = idx % K;
+      tc::put_split(b_hi, b_lo, r, k, K, a.W[(size_t)(n0 + r) * K + k]);
+    }
+    tc::fence_async_smem();
+    tc::fence_before();
+    __syncthreads();
+    tc::fence_after();
+    const uint32_t tmem_base = tmem_s;
+    tc::issue_layer(tmem_base, a_hi, a_lo, b_hi, b_lo, nc, K, a.passes, a.swap_ls, bar);
+    tc::mbar_wait(bar, phase);
+    phase ^= 1;
+    tc::fence_after();
+    for (int c0 = 0; c0 < nc; c0 += 32) {
+      float v[32];
+      tc::tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
+      if (row < a.M)
+        for (int c = 0; c < 32 && c0 + c < nc; ++c) a.Y[(size_t)row * N + n0 + c0 + c] = v[c];
+    }
+    tc::fence_before();
+    __syncthreads();      // accumulator reads done before the next block's MMAs overwrite it; B block free
+    tc::fence_after();
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
+  if (warp == 0) tc::tmem_dealloc<64>(tmem_s);
 }
 
 extern "C" int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int32_t N, int32_t K, int32_t passes, int32_t swap_ls,
                                   void* stream) {
-  if (N % 16 || N < 16 || N > 256 || K % 8 || K < 8 || K > 64) { mx_set_error("tc probe: N %% 16, N <= 256, K %% 8, K <= 64 required"); return 1; }
+  if (N % 16 || N < 16 || N > 256 || K % 8 || K < 8 || K > 64 || M < 1) { mx_set_error("tc probe: M >= 1, N %% 16, N <= 256, K %% 8, K <= 64 required"); return 1; }
   TcProbeArgs a{X, W, Y, M, N, K, passes, swap_ls};
-  const size_t smem = (size_t)(2 * 128 + 2 * 256) * K * 4;
+  const size_t smem = (size_t)(2 * 128 + 2 * 64) * K * 4 + 64 * 128 * 4;
 #if !MX_EMU
   static size_t configured = 0;
   if (smem > configured) { cudaFuncSetAttribute(k_tc_linear_probe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); configured = smem; }

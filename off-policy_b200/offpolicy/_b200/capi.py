@@ -185,7 +185,7 @@ def lib():
         raise MxError("marl_b200: no CUDA device visible; this engine has no CPU path")
     handle = _declare(C.CDLL(LIB_PATH))
     if handle.mx_is_cuda_build() != 1:
-        raise MxError("marl_b200: %s is not the nvcc sm_100a build" % LIB_PATH)
+        raise MxError("marl_b200: %s is not the nvcc sm_90a build" % LIB_PATH)
     _lib = handle
     _device = torch.device("cuda", torch.cuda.current_device())
     return _lib

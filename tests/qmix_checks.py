@@ -190,35 +190,41 @@ def grad_failures(gv, coef, L, cfg, tol):
 
 
 def compare_step(L, pol, tr, batch, cfg, steps=1, tol=1e-4, param_tol=5e-3, mlp=False):
-    import kink
-    B, T = (batch[0].shape[2], batch[2].shape[1])
     for s in range(steps):
-        L0 = kink.snapshot(L) if getattr(cfg, "relu", True) else None
         info, prio, _ = tr.train_policy_on_batch(ref_tuple(batch))
         gv = {k: v.clone() for k, v in tr.grad_views().items()}
-        ref, rprio, _ = L.step(batch)
+        check_engine_step(L, pol, tr, batch, cfg, info, prio, gv, s, tol, param_tol)
+
+
+def check_engine_step(L, pol, tr, batch, cfg, info, prio, gv, s=0, tol=1e-4, param_tol=5e-3):
+    """Step `s` of compare_step after the engine ran it (train_info `info`, priorities `prio`, gradient views `gv`): the oracle
+    steps on the same batch and both are compared; then both apply the soft target update."""
+    import kink
+    B, T = (batch[0].shape[2], batch[2].shape[1])
+    L0 = kink.snapshot(L) if getattr(cfg, "relu", True) else None
+    ref, rprio, _ = L.step(batch)
+    coef = min(1.0, cfg.max_grad_norm / (float(ref["grad_norm"]) + 1e-6))
+    bad = grad_failures(gv, coef, L, cfg, tol)
+    if bad and L0 is not None:
+        # ReLU kink? re-run the oracle step with the engine's ReLU masks (tests/kink.py): only units within round-off of zero may differ
+        masks = kink.engine_masks(tr, B, T, cfg.n_agents, mlp=False)
+        (ref, rprio, _), flips, max_pre = kink.redo_with_engine_masks(L0, lambda LL: LL.step(batch), masks)
+        assert flips > 0 and max_pre < kink.KINK_TOL, (s, "gradient mismatch not explained by ReLU kinks", flips, max_pre, bad[:3])
+        kink.adopt(L, L0)
         coef = min(1.0, cfg.max_grad_norm / (float(ref["grad_norm"]) + 1e-6))
         bad = grad_failures(gv, coef, L, cfg, tol)
-        if bad and L0 is not None:
-            # ReLU kink? re-run the oracle step with the engine's ReLU masks (tests/kink.py): only units within round-off of zero may differ
-            masks = kink.engine_masks(tr, B, T, cfg.n_agents, mlp=False)
-            (ref, rprio, _), flips, max_pre = kink.redo_with_engine_masks(L0, lambda LL: LL.step(batch), masks)
-            assert flips > 0 and max_pre < kink.KINK_TOL, (s, "gradient mismatch not explained by ReLU kinks", flips, max_pre, bad[:3])
-            kink.adopt(L, L0)
-            coef = min(1.0, cfg.max_grad_norm / (float(ref["grad_norm"]) + 1e-6))
-            bad = grad_failures(gv, coef, L, cfg, tol)
-            print("kink-aware comparison: %d ReLU unit(s) within %.1e of zero flipped" % (flips, max_pre))
-        assert not bad, (s, bad[:4])
-        tr.soft_target_updates()
-        L.soft_update()
-        for k in ("loss", "grad_norm", "Q_tot"):
-            assert rel_err(info[k].cpu(), ref[k]) < tol, (s, k, float(info[k]), float(ref[k]))
-        if rprio is not None:
-            assert rel_err(np.asarray(prio), rprio) < tol
-        for k, v in pol.q_network.state_dict().items():
-            assert float((v.cpu() - L.agent.state_dict()[k]).abs().max()) <= param_tol * cfg.lr * (s + 1) + 1e-7, (s, k)
-        for k, v in tr.target_q_network.state_dict().items():
-            assert float((v.cpu() - L.tgt_agent.state_dict()[k]).abs().max()) <= 1e-6, (s, k)
+        print("kink-aware comparison: %d ReLU unit(s) within %.1e of zero flipped" % (flips, max_pre))
+    assert not bad, (s, bad[:4])
+    tr.soft_target_updates()
+    L.soft_update()
+    for k in ("loss", "grad_norm", "Q_tot"):
+        assert rel_err(info[k].cpu(), ref[k]) < tol, (s, k, float(info[k]), float(ref[k]))
+    if rprio is not None:
+        assert rel_err(np.asarray(prio), rprio) < tol
+    for k, v in pol.q_network.state_dict().items():
+        assert float((v.cpu() - L.agent.state_dict()[k]).abs().max()) <= param_tol * cfg.lr * (s + 1) + 1e-7, (s, k)
+    for k, v in tr.target_q_network.state_dict().items():
+        assert float((v.cpu() - L.tgt_agent.state_dict()[k]).abs().max()) <= 1e-6, (s, k)
 
 
 def check_mpe_shapes_without_avail_masks(steps=2, B=32):

@@ -82,6 +82,30 @@ def test_config5_2s3z_vs_oracle(gpu_engine):
     _compare_step(L, pol, tr, batch, cfg, steps=1)
 
 
+def test_two_learners_on_two_streams_vs_oracle(gpu_engine):
+    """Two learners whose steps run at the same time on two streams (2s3z sizes: every tensor-core kernel of the forward, the
+    data-gradient chain and the weight gradients): each handle's accumulators are its own, both match their oracle."""
+    from oracle.qmix import QmixConfig, synth_batch
+    torch.set_num_threads(8)
+    cfg = QmixConfig(n_agents=5, obs_dim=80, act_dim=11, state_dim=120)
+    runs = []
+    for seed in (7, 6):          # two different batches, each within the one-step Adam parameter tolerance on its own
+        L, args, pol, tr = _oracle_and_trainer(cfg, 32, 120)
+        runs.append((L, pol, tr, synth_batch(cfg, 32, 120, seed=seed, avail_p=0.8, var_len=False) + (None, None)))
+    dev = torch.device("cuda", 0)
+    streams = [torch.cuda.Stream(device=dev) for _ in runs]
+    for st in streams:
+        st.wait_stream(torch.cuda.current_stream(dev))
+    outs = []
+    for (L, pol, tr, batch), st in zip(runs, streams):
+        with torch.cuda.stream(st):
+            outs.append(tr.train_policy_on_batch(qc.ref_tuple(batch)))
+    torch.cuda.synchronize()
+    for (L, pol, tr, batch), (info, prio, _) in zip(runs, outs):
+        gv = {k: v.clone() for k, v in tr.grad_views().items()}
+        qc.check_engine_step(L, pol, tr, batch, cfg, info, prio, gv)
+
+
 @pytest.mark.parametrize("mode", ["forked", "fused"])
 def test_config5_2s3z_branch_modes_vs_oracle(gpu_engine, mode):
     """2s3z sizes with the forked branch forced on (split mixer beside the agent nets; the default at this size is the in-line

@@ -1,4 +1,4 @@
-"""GPU probe of the tcgen05 3xTF32 building block against an fp64 reference (descriptor-convention check)."""
+"""GPU probe of the wgmma 3xTF32 building block against an fp64 reference (descriptor-convention check)."""
 import os
 import sys
 
