@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MX_ABI_VERSION 3
+#define MX_ABI_VERSION 4
 #define MX_MAX_NAME 64
 
 typedef struct mx_replay mx_replay;   /* one policy's episode store + sampler (RecPolicyBuffer + PER trees) */
@@ -278,8 +278,16 @@ typedef struct mx_maddpg_cfg {
    * actions of all agents.  cent_act_dim = total action width over all agents (policy_info['cent_act_dim']), act_offset = first
    * column of this policy's agents inside it.  0 / 0 = one shared policy (cent_act_dim = n_agents * act_dim). */
   int32_t cent_act_dim, act_offset;
+  /* 1: transition-level MADDPG / MATD3 (algorithms/maddpg/maddpg.py:90-249, maddpg/algorithm/actor_critic.py): MLP actor and critic
+   * without recurrence, a batch = B transitions stored as episodes of length 1 (episode_len must be 1; step 0 = obs, step 1 = next
+   * obs).  The critic's K Q heads are not trained (a plain list in the reference, SURVEY.md App. D-6): the live and the target heads
+   * are two fixed initialisations kept behind the critic's trunk, outside the range Adam, clipping and the target updates touch.
+   * The actor loss is masked by valid_transition (mx_maddpg_set_valid).  One shared policy only (cent_act_dim = 0). */
+  int32_t mlp;
 } mx_maddpg_cfg;
-/* which = 0: actor ("rnn.*", "act.action_out.*"), 1: critic ("rnn.*", "q_outs.k.*"); names = reference state_dict keys */
+/* which = 0: actor ("rnn.*", "act.action_out.*"), 1: critic ("rnn.*", "q_outs.k.*"); names = reference state_dict keys.
+ * cfg.mlp: actor "mlp.*", "act.action_out.*"; critic "mlp.*" (the trained trunk); which = 2: the critic's frozen heads "q_outs.k.*",
+ * located in the live and in the target critic vector alike. */
 int mx_maddpg_param_layout(const mx_maddpg_cfg* cfg, int32_t which, mx_param_entry* out, int32_t max_entries, int64_t* total_floats);
 int64_t mx_maddpg_workspace_bytes(const mx_maddpg_cfg* cfg);
 /* actor_vecs / critic_vecs: {theta, theta_target, adam_m, adam_v}, each of the layout's total_floats; workspace zero-filled */
@@ -305,6 +313,10 @@ int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* src_batch, const f
 struct mx_graph;
 int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                             const float* actor_noise_dev, int32_t update_actor, void* stream, struct mx_graph** out);
+/* cfg.mlp: valid_transition of the transition store, device fp32 [rows][n_agents] (mlp_buffer.py:156).  The actor loss of a batch
+ * reads row batch->idx[b] (row b when the batch has no indices); NULL: every transition is valid.  The pointer is kept, so a
+ * captured graph reads the store as it is at replay time. */
+int mx_maddpg_set_valid(mx_maddpg* h, const float* valid_dev);
 int64_t mx_maddpg_num_updates(const mx_maddpg* h);   /* updates done so far (self.num_updates[p_id], r_maddpg.py:125) */
 /* device fp32[8]: critic_loss, critic_grad_norm, -, denom, actor_loss, actor_grad_norm, -, denom */
 const float* mx_maddpg_info(mx_maddpg* h);

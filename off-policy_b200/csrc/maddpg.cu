@@ -5,6 +5,9 @@
 //
 // reference: offpolicy/algorithms/r_maddpg/r_maddpg.py:114-331, r_maddpg/algorithm/{rMADDPGPolicy,r_actor_critic}.py,
 // r_matd3/* (K = 2 heads, actor every 2nd update, Gaussian target noise handed in by the host from torch's CPU RNG).
+//
+// cfg.mlp: the transition-level MADDPG / MATD3 (algorithms/maddpg/maddpg.py:90-249, maddpg/algorithm/actor_critic.py) on the same
+// kernels, see maddpg_step_mlp.
 #include <string.h>
 
 #include <vector>
@@ -65,7 +68,7 @@ __global__ void __launch_bounds__(256) k_pack_critic_in(PackArgs a) {
     }
     a.x[idx] = v;
   }
-  if (a.mode == 2) {
+  if (a.mode == 2 && a.h0) {
     const long long th = rows * MX_H;
     for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < th; idx += (long long)gridDim.x * blockDim.x) {
       const long long row = idx / MX_H;
@@ -195,6 +198,7 @@ struct CriticLossArgs {
   const float* weights;     // [B] or null
   float gamma, huber_delta, per_nu, per_eps;
   int use_huber;
+  int prio_mean_k;          // 1: priority = mean_k |err_k| + per_eps (T = 1, maddpg.py:144); 0: the recurrent formula below
   float* dq;                // [B*T][K]
   float* err;               // [K][B*T]
   float* scal;              // [4]: sum(1-bad), loss numerator, -, elements
@@ -237,6 +241,12 @@ __global__ void __launch_bounds__(256) k_critic_loss(CriticLossArgs a) {   // ON
   if (a.prio) {
     __syncthreads();
     for (int b = tid; b < a.B; b += blockDim.x) {
+      if (a.prio_mean_k) {
+        float sm = 0.f;
+        for (int k = 0; k < a.K; ++k) sm += fabsf(a.err[(size_t)k * E + b]);
+        a.prio[b] = sm / (float)a.K + a.per_eps;
+        continue;
+      }
       float acc = 0.f;
       for (int k = 0; k < a.K; ++k) {
         float mx = 0.f, sm = 0.f;
@@ -253,6 +263,8 @@ struct ActorLossArgs {
   int ld_tn;                // floats between consecutive episodes of dones (>= T*N)
   const float* qa;          // [N*B*T][K] critic outputs on the agent-replaced copies (head 0 is used)
   const float* dones;       // [B][T][N]
+  const float* valid;       // T = 1 (cfg.mlp): valid_transition [rows][N] read at row valid_idx[b] (b when null), maddpg.py:197-232; or null
+  const int64_t* valid_idx;
   float* dout;              // [N*B*T][K]
   float* scal;              // [4]: sum(1-done_mask), loss numerator = -sum Q (1-done_mask)
 };
@@ -265,7 +277,7 @@ __global__ void __launch_bounds__(256) k_actor_loss(ActorLossArgs a) {   // ONE 
     const int i = row / (a.B * a.T), bt = row % (a.B * a.T);
     const int b = bt / a.T, t = bt % a.T;
     const float dm = t > 0 ? a.dones[(size_t)b * a.ld_tn + (size_t)(t - 1) * a.N + i] : 0.f;    // r_maddpg.py:268-272
-    const float keep = 1.f - dm;
+    const float keep = a.valid ? a.valid[(size_t)(a.valid_idx ? a.valid_idx[b] : b) * a.N + i] : 1.f - dm;
     den += keep;
     ls -= a.qa[(size_t)row * a.K] * keep;
     for (int k = 0; k < a.K; ++k) a.dout[(size_t)row * a.K + k] = k == 0 ? -keep : 0.f;
@@ -282,7 +294,9 @@ __global__ void __launch_bounds__(256) k_actor_loss(ActorLossArgs a) {   // ONE 
 // d(actor action of agent i at (b,t)) = dX[(i,b,t)][S + i*Ac + k]   ->   dense head gradient of the actor [M_a][Ac].
 // Discrete actors (soft != null): the action is the straight-through hard Gumbel-softmax sample, so the gradient reaches the
 // logits through the soft sample y = softmax(logits + g):  dlogit_k = y_k (d_k - sum_j d_j y_j)            (util.py:160-165)
-__global__ void __launch_bounds__(256) k_scatter_actor_grad(const float* dX, int ldx, int B, int T, int N, int S, int Ac, const float* soft, float* dact, int off) {
+// dact rows have dact_ld >= Ac columns, the ones past Ac are zero-filled (cfg.mlp: the actor's "gi" gradient rows, dact_ld = 3H).
+__global__ void __launch_bounds__(256) k_scatter_actor_grad(const float* dX, int ldx, int B, int T, int N, int S, int Ac, const float* soft, float* dact, int off,
+                                                            int dact_ld) {
   const long long rows = (long long)B * (T + 1) * N;
   for (long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x; m < rows; m += (long long)gridDim.x * blockDim.x) {
     const int n = (int)(m % N);
@@ -295,7 +309,7 @@ __global__ void __launch_bounds__(256) k_scatter_actor_grad(const float* dX, int
       for (int k = 0; k < Ac; ++k) dot += d[k] * soft[m * Ac + k];
       for (int k = 0; k < Ac; ++k) d[k] = soft[m * Ac + k] * (d[k] - dot);
     }
-    for (int k = 0; k < Ac; ++k) dact[m * Ac + k] = d[k];
+    for (int k = 0; k < dact_ld; ++k) dact[m * dact_ld + k] = k < Ac ? d[k] : 0.f;
   }
 }
 
@@ -338,6 +352,32 @@ __global__ void __launch_bounds__(256) k_act_transform(ActXformArgs a) {
   }
 }
 
+// ---- cfg.mlp: the heads sit in the weight_ih slot, so the front kernel's "gi" rows [M][3H] carry the head outputs in columns [0, K) ----
+// out[m][k] = gi[m][k] (+ noise[m][k]), out_min[m] = min_k of the same values; either output may be null
+__global__ void __launch_bounds__(256) k_mlp_head_cols(const float* __restrict__ gi, int M, int K, const float* __restrict__ noise,
+                                                       float* __restrict__ out, float* __restrict__ out_min) {
+  for (long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x; m < M; m += (long long)gridDim.x * blockDim.x) {
+    float mn = 0.f;
+    for (int k = 0; k < K; ++k) {
+      float v = gi[m * MX_G + k];
+      if (noise) v += noise[m * K + k];
+      if (out) out[m * K + k] = v;
+      mn = (k == 0 || v < mn) ? v : mn;      // torch.min over the heads (maddpg.py:117)
+    }
+    if (out_min) out_min[m] = mn;
+  }
+}
+
+// dgi[m][j] = j < K ? src[m][j] : 0 over [M][3H]: the gradient at the head outputs as the "gi" gradient rows k_front_bwd reads
+__global__ void __launch_bounds__(256) k_mlp_dgi_cols(const float* __restrict__ src, int K, int M, float* __restrict__ dgi) {
+  const long long total = (long long)M * MX_G;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long m = i / MX_G;
+    const int j = (int)(i - m * MX_G);
+    dgi[i] = j < K ? src[m * K + j] : 0.f;
+  }
+}
+
 // =====================================================================================================
 // handle
 // =====================================================================================================
@@ -365,6 +405,7 @@ struct mx_maddpg {
   float* ws;
   MxMaddpgWs W;
   int64_t num_updates;
+  const float* valid = nullptr;     // cfg.mlp: valid_transition store [rows][n_agents] (mx_maddpg_set_valid)
   int force_update_actor = -1;      // graph capture: -1 = decide from num_updates, 0 / 1 = record this variant
 };
 
@@ -382,12 +423,18 @@ static int maddpg_check(const mx_maddpg_cfg* c) {
     mx_set_error("mx_maddpg: act_offset %d + n_agents*act_dim %d exceeds cent_act_dim %d", c->act_offset, c->n_agents * c->act_dim, c->cent_act_dim); return 1;
   }
   if (c->cent_act_dim == 0 && c->act_offset != 0) { mx_set_error("mx_maddpg: act_offset needs cent_act_dim"); return 1; }
+  if (c->mlp && (c->episode_len != 1 || c->cent_act_dim != 0)) {
+    mx_set_error("mx_maddpg: the MLP (transition-level) variant takes transitions as episodes of length 1 and one shared policy"); return 1;
+  }
   return 0;
 }
 
 // critic: q_outs.k are K separate Linear(H,1): weights [K][H] contiguous, then K biases (each padded to 4 floats)
+// cfg.mlp: both nets keep their head in the first rows of the weight_ih slot (the actor's trained head; the critic's K frozen heads,
+// whose live and target copies are the tails of the two critic vectors past the trunk [0, wih))
 static void maddpg_layouts(const mx_maddpg_cfg* c, MxNetLayout* A, MxNetLayout* Cr) {
   mx_net_layout(c->obs_dim, c->act_dim, 0, A);
+  if (c->mlp) { mx_net_layout(critic_in_dim(c), c->num_q, 0, Cr); return; }
   // critic head: out_dim = K rows of H, but each q_outs.k is its own tensor -> lay out as (w0, b0, w1, b1, ...)
   mx_net_layout(critic_in_dim(c), 1, 0, Cr);
   // mx_net_layout put wq (1 x H) and bq (1, padded to 4); extend for K heads: stride between heads = H + 4
@@ -400,6 +447,7 @@ extern "C" int mx_maddpg_param_layout(const mx_maddpg_cfg* c, int32_t which, mx_
   MxNetLayout A, Cr;
   maddpg_layouts(c, &A, &Cr);
   const MxNetLayout& L = which == 0 ? A : Cr;
+  if (which < 0 || which > 2 || (which == 2 && !c->mlp)) { mx_set_error("mx_maddpg_param_layout: which = %d", which); return -1; }
   std::vector<mx_param_entry> v;
   auto add = [&](const char* name, int off, int rows, int cols) {
     mx_param_entry e;
@@ -409,6 +457,28 @@ extern "C" int mx_maddpg_param_layout(const mx_maddpg_cfg* c, int32_t which, mx_
     v.push_back(e);
   };
   const int H = MX_H, I = L.in_dim;
+  if (c->mlp) {      // MADDPG_Actor / MADDPG_Critic: MLPBase (mlp.py:52-89) + ACTLayer (act.py) / q_outs (actor_critic.py:67)
+    if (which == 2) {
+      for (int k = 0; k < c->num_q; ++k) {
+        char nm[64];
+        snprintf(nm, sizeof(nm), "q_outs.%d.weight", k); add(nm, L.wih + k * H, 1, H);
+        snprintf(nm, sizeof(nm), "q_outs.%d.bias", k); add(nm, L.bih + k, 1, 0);
+      }
+    } else {
+      if (!c->no_feature_norm) { add("mlp.feature_norm.weight", L.fn_g, I, 0); add("mlp.feature_norm.bias", L.fn_b, I, 0); }
+      add("mlp.mlp.fc1.0.weight", L.w1, H, I); add("mlp.mlp.fc1.0.bias", L.b1, H, 0);
+      add("mlp.mlp.fc1.2.weight", L.ln1_g, H, 0); add("mlp.mlp.fc1.2.bias", L.ln1_b, H, 0);
+      add("mlp.mlp.fc_h.0.weight", L.wh, H, H); add("mlp.mlp.fc_h.0.bias", L.bh, H, 0);
+      add("mlp.mlp.fc_h.2.weight", L.lnh_g, H, 0); add("mlp.mlp.fc_h.2.bias", L.lnh_b, H, 0);
+      add("mlp.mlp.fc2.0.0.weight", L.w2, H, H); add("mlp.mlp.fc2.0.0.bias", L.b2, H, 0);
+      add("mlp.mlp.fc2.0.2.weight", L.ln2_g, H, 0); add("mlp.mlp.fc2.0.2.bias", L.ln2_b, H, 0);
+      if (which == 0) { add("act.action_out.weight", L.wih, c->act_dim, H); add("act.action_out.bias", L.bih, c->act_dim, 0); }
+    }
+    if (total_floats) *total_floats = L.size;
+    const int n = (int)v.size();
+    if (out) for (int i = 0; i < n && i < max_entries; ++i) out[i] = v[i];
+    return n;
+  }
   if (!c->no_feature_norm) { add("rnn.feature_norm.weight", L.fn_g, I, 0); add("rnn.feature_norm.bias", L.fn_b, I, 0); }
   add("rnn.mlp.fc1.0.weight", L.w1, H, I); add("rnn.mlp.fc1.0.bias", L.b1, H, 0);
   add("rnn.mlp.fc1.2.weight", L.ln1_g, H, 0); add("rnn.mlp.fc1.2.bias", L.ln1_b, H, 0);
@@ -495,6 +565,11 @@ extern "C" int mx_maddpg_create(const mx_maddpg_cfg* c, float* const actor_vecs[
   return 0;
 }
 extern "C" void mx_maddpg_destroy(mx_maddpg* h) { delete h; }
+extern "C" int mx_maddpg_set_valid(mx_maddpg* h, const float* valid_dev) {
+  if (!h) { mx_set_error("mx_maddpg_set_valid: null handle"); return 1; }
+  h->valid = valid_dev;
+  return 0;
+}
 extern "C" const float* mx_maddpg_info(mx_maddpg* h) { return h->ws + h->W.info; }
 extern "C" const float* mx_maddpg_priorities(mx_maddpg* h) { return h->ws + h->W.prio; }
 extern "C" int mx_maddpg_grad_views(mx_maddpg* h, int64_t* actor_off_bytes, int64_t* critic_off_bytes) {
@@ -533,6 +608,10 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
   o.nseg = 2;
   o.seg_begin[0] = 0; o.seg_end[0] = L.lno_g; o.seg_parts[0] = parts[0];
   o.seg_begin[1] = L.lno_g; o.seg_end[1] = (int)P; o.seg_parts[1] = head_parts;
+  if (c.mlp) {        // every gradient comes from k_front_bwd; the critic's trained range stops at its trunk (the frozen heads follow it)
+    o.nseg = 1;
+    if (!actor) { o.P = L.wih; o.gpart_ld = P; o.seg_end[0] = L.wih; }
+  }
   o.spart = ws + h->W.spart; o.spart_n = 0;
   o.info = ws + h->W.info + (actor ? 4 : 0);
   o.adam_t = reinterpret_cast<double*>(ws + (actor ? h->W.adam_ta : h->W.adam_tc));
@@ -540,10 +619,146 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
   o.lr = c.lr; o.beta1 = c.adam_beta1; o.beta2 = c.adam_beta2; o.eps = c.adam_eps; o.max_grad_norm = c.max_grad_norm; o.tau = c.tau;
   o.weight_decay = c.weight_decay;
   if (mx_launch_grad_reduce(o, s)) return 1;     // (its scalar block bumps the Adam step count; the loss scalars come from the loss kernel)
-  MX_LAUNCH(k_set_scalars, dim3(1), dim3(32), 0, s, o.grad + P, (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c)));
+  MX_LAUNCH(k_set_scalars, dim3(1), dim3(32), 0, s, o.grad + o.P, (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c)));
   MX_COUNT();
   MX_MARK("k_set_scalars", s);
   return mx_launch_adam(o, s);
+}
+
+// ---- cfg.mlp: shared_train_policy_on_batch of the transition-level trainer (maddpg.py:90-249) ---------------------------------------
+// A batch is B transitions stored as episodes of length 1: obs rows m = (b*2 + t)*N + n with t = 0 the observation and t = 1 the next
+// observation, so the recurrent path's critic-input packing serves unchanged (mode 0: (s, a), mode 1: (s', a'), mode 2: the N
+// agent-replaced copies).  No recurrence: every net is the front kernel with its head in the weight_ih slot, and k_front_bwd runs
+// with no_gru.  The critic's heads are frozen (not in the reference's parameters()): the live heads give Q(s, a) and, in the actor
+// phase, the gradient path into the actor; the target heads give Q'(s', a').
+static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor,
+                           cudaStream_t s) {
+  const mx_maddpg_cfg& c = h->cfg;
+  float* ws = h->ws;
+  const MxMaddpgWs& W = h->W;
+  const int B = b->B, N = c.n_agents, K = c.num_q, Ac = c.act_dim, S = c.state_dim;
+  const int Ma = B * 2 * N, Mc = B, Mr = N * B;
+  const int ldc = mx_round_up(critic_in_dim(&c), 4);
+  const MxNetLayout& LA = h->actor;
+  const MxNetLayout& LC = h->critic;
+  const int fnorm = c.no_feature_norm ? 0 : 1;
+
+  // ---------- A. live + target actor on obs and next_obs; target actions a' from the next_obs rows (maddpg.py:64-74) ----------
+  FrontFwdArgs ff;
+  memset(&ff, 0, sizeof(ff));
+  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
+  ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = fnorm; ff.act_tanh = c.use_tanh;
+  ff.theta[0] = h->th_a; ff.theta[1] = h->th_a_tgt; ff.L = LA;
+  ff.gi[0] = ws + W.a_gi[0]; ff.gi[1] = ws + W.a_gi[1];
+  ff.u1 = ws + W.a_u1; ff.u2 = ws + W.a_u2; ff.st0 = ws + W.a_st0; ff.st1 = ws + W.a_st1; ff.st2 = ws + W.a_st2;
+  if (mx_launch_front_fwd(ff, 2, s)) return 1;
+  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[1], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
+            ws + W.a_nact, nullptr);
+  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  if (c.discrete) {      // onehot_from_logits with the next-avail mask (MADDPG) / hard Gumbel-softmax, the draw already added (MATD3)
+    ActXformArgs ax;
+    memset(&ax, 0, sizeof(ax));
+    ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
+    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
+  }
+
+  // ---------- B. live critic on (s, a), target critic on (s', a'); TD target, loss, priorities (maddpg.py:112-151) ----------
+  PackArgs pk;
+  memset(&pk, 0, sizeof(pk));
+  pk.B = B; pk.T = 1; pk.N = N; pk.S = S; pk.Ac = Ac; pk.share = b->share; pk.share_ld = b->share_ld; pk.acts = b->acts; pk.act_ld = b->act_ld;
+  pk.ldx = ldc;
+  pk.mode = 0; pk.x = ws + W.c_x;
+  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
+  pk.mode = 1; pk.x = ws + W.t_x; pk.actor_out = ws + W.a_nact;
+  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
+  FrontFwdArgs fc;
+  memset(&fc, 0, sizeof(fc));
+  fc.tc_acc = ws + W.tc_acc; fc.tc_acc_cols = (int)W.tc_acc_cols;
+  fc.X = ws + W.c_x; fc.ldx = ldc; fc.M = Mc; fc.feature_norm = fnorm; fc.act_tanh = c.use_tanh; fc.theta[0] = h->th_c; fc.L = LC;
+  fc.gi[0] = ws + W.c_gi[0];
+  fc.u1 = ws + W.c_u1; fc.u2 = ws + W.c_u2; fc.st0 = ws + W.c_st0; fc.st1 = ws + W.c_st1; fc.st2 = ws + W.c_st2;
+  if (mx_launch_front_fwd(fc, 1, s)) return 1;
+  FrontFwdArgs ft;
+  memset(&ft, 0, sizeof(ft));
+  ft.tc_acc = ws + W.tc_acc; ft.tc_acc_cols = (int)W.tc_acc_cols;
+  ft.X = ws + W.t_x; ft.ldx = ldc; ft.M = Mc; ft.feature_norm = fnorm; ft.act_tanh = c.use_tanh; ft.theta[0] = h->th_c_tgt; ft.L = LC; ft.gi[0] = ws + W.t_gi;
+  if (mx_launch_front_fwd(ft, 1, s)) return 1;
+  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mc)), dim3(256), 0, s, (const float*)fc.gi[0], Mc, K, (const float*)nullptr, ws + W.c_q, nullptr);
+  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mc)), dim3(256), 0, s, (const float*)ft.gi[0], Mc, K, (const float*)nullptr, nullptr, ws + W.t_qmin);
+  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  CriticLossArgs cl;
+  memset(&cl, 0, sizeof(cl));
+  cl.B = B; cl.T = 1; cl.N = N; cl.K = K; cl.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : N; cl.ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : 1;
+  cl.qpred = ws + W.c_q; cl.qnext_min = ws + W.t_qmin; cl.rewards = b->rewards; cl.dones_env = b->dones_env;
+  cl.weights = c.use_per ? b->weights : nullptr; cl.gamma = c.gamma; cl.huber_delta = c.huber_delta; cl.per_eps = c.per_eps;
+  cl.use_huber = c.use_huber; cl.prio_mean_k = 1; cl.dq = ws + W.c_dq; cl.err = ws + W.c_err; cl.scal = ws + W.scal_c; cl.prio = c.use_per ? ws + W.prio : nullptr;
+  MX_LAUNCH(k_critic_loss, dim3(1), dim3(256), 0, s, cl); MX_COUNT(); MX_MARK("k_critic_loss", s);
+
+  // ---------- C. critic backward through the frozen live heads into the trunk; clip + Adam over the trunk ----------
+  MX_LAUNCH(k_mlp_dgi_cols, dim3(launch1d((long long)Mc * MX_G)), dim3(256), 0, s, (const float*)(ws + W.c_dq), K, Mc, ws + W.c_dgi);
+  MX_COUNT(); MX_MARK("k_mlp_dgi_cols", s);
+  int parts[2] = {0, 0};
+  FrontBwdArgs fb;
+  memset(&fb, 0, sizeof(fb));
+  fb.X = ws + W.c_x; fb.ldx = ldc; fb.M = Mc; fb.T = 1; fb.N = 1; fb.feature_norm = fnorm; fb.act_tanh = c.use_tanh; fb.no_gru = 1;
+  fb.theta = h->th_c; fb.L = LC; fb.u1 = fc.u1; fb.u2 = fc.u2; fb.st0 = fc.st0; fb.st1 = fc.st1; fb.st2 = fc.st2; fb.dgi = ws + W.c_dgi;
+  fb.gpart = ws + W.gpart_c; fb.P = h->Pc;
+  fb.da2_out = ws + W.tc_da2; fb.da1_out = ws + W.tc_da1; fb.tc_imgT = ws + W.tc_imgT;      // (option wgrad_tc)
+  fb.tc_acc = ws + W.tc_acc; fb.tc_acc_cols = (int)W.tc_acc_cols;
+  if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
+  if (optimise(h, false, parts, 0, s)) return 1;
+  if (!update_actor) return 0;
+
+  // ---------- D. actor loss through head 0 of the UPDATED critic on the agent-replaced copies, masked by valid_transition ----------
+  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[0], Ma, Ac, (const float*)nullptr, ws + W.a_out, nullptr);
+  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  if (c.discrete) {    // get_actions(obs, avail, use_gumbel=True): hard Gumbel-softmax, straight-through (maddpg.py:209)
+    ActXformArgs ax;
+    memset(&ax, 0, sizeof(ax));
+    ax.M = Ma; ax.Ac = Ac; ax.mode = 1; ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
+    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
+  }
+  pk.mode = 2; pk.x = ws + W.r_x; pk.actor_out = ws + (c.discrete ? W.a_act : W.a_out);
+  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mr * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
+  FrontFwdArgs fr;
+  memset(&fr, 0, sizeof(fr));
+  fr.tc_acc = ws + W.tc_acc; fr.tc_acc_cols = (int)W.tc_acc_cols;
+  fr.X = ws + W.r_x; fr.ldx = ldc; fr.M = Mr; fr.feature_norm = fnorm; fr.act_tanh = c.use_tanh; fr.theta[0] = h->th_c; fr.L = LC; fr.gi[0] = ws + W.r_gi;
+  fr.u1 = ws + W.r_u1; fr.u2 = ws + W.r_u2; fr.st0 = ws + W.r_st0; fr.st1 = ws + W.r_st1; fr.st2 = ws + W.r_st2;
+  if (mx_launch_front_fwd(fr, 1, s)) return 1;
+  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mr)), dim3(256), 0, s, (const float*)fr.gi[0], Mr, K, (const float*)nullptr, ws + W.r_q, nullptr);
+  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  ActorLossArgs al;
+  memset(&al, 0, sizeof(al));
+  al.B = B; al.T = 1; al.N = N; al.K = K; al.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : N; al.qa = ws + W.r_q; al.dones = b->dones;
+  al.valid = h->valid; al.valid_idx = b->idx; al.dout = ws + W.r_dout; al.scal = ws + W.scal_a;
+  MX_LAUNCH(k_actor_loss, dim3(1), dim3(256), 0, s, al); MX_COUNT(); MX_MARK("k_actor_loss", s);
+  // back through the frozen critic (trunk and live head 0) to its action inputs, then into the actor's head rows
+  MX_LAUNCH(k_mlp_dgi_cols, dim3(launch1d((long long)Mr * MX_G)), dim3(256), 0, s, (const float*)(ws + W.r_dout), K, Mr, ws + W.r_dgi);
+  MX_COUNT(); MX_MARK("k_mlp_dgi_cols", s);
+  FrontBwdArgs fbr;
+  memset(&fbr, 0, sizeof(fbr));
+  fbr.X = ws + W.r_x; fbr.ldx = ldc; fbr.M = Mr; fbr.T = 1; fbr.N = 1; fbr.feature_norm = fnorm; fbr.act_tanh = c.use_tanh; fbr.no_gru = 1;
+  fbr.theta = h->th_c; fbr.L = LC; fbr.u1 = fr.u1; fbr.u2 = fr.u2; fbr.st0 = fr.st0; fbr.st1 = fr.st1; fbr.st2 = fr.st2; fbr.dgi = ws + W.r_dgi;
+  fbr.gpart = ws + W.gpart_c; fbr.P = h->Pc; fbr.dX = ws + W.r_dx; fbr.skip_wgrad = 1;
+  int dummy = 0;
+  if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
+  MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, 1, N, S, Ac,
+            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, 0, (int)MX_G);
+  MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
+  FrontBwdArgs fba;
+  memset(&fba, 0, sizeof(fba));
+  fba.X = b->obs; fba.ldx = b->obs_ld; fba.M = Ma; fba.T = 1; fba.N = N; fba.feature_norm = fnorm; fba.act_tanh = c.use_tanh; fba.no_gru = 1;
+  fba.theta = h->th_a; fba.L = LA; fba.u1 = ff.u1; fba.u2 = ff.u2; fba.st0 = ff.st0; fba.st1 = ff.st1; fba.st2 = ff.st2; fba.dgi = ws + W.a_dgi;
+  fba.gpart = ws + W.gpart_a; fba.P = h->Pa;
+  fba.da2_out = ws + W.tc_da2; fba.da1_out = ws + W.tc_da1; fba.tc_imgT = ws + W.tc_imgT;
+  fba.tc_acc = ws + W.tc_acc; fba.tc_acc_cols = (int)W.tc_acc_cols;
+  int aparts[2] = {0, 0};
+  if (mx_launch_front_bwd(fba, &aparts[0], s)) return 1;
+  return optimise(h, true, aparts, 0, s);
 }
 
 extern "C" int mx_maddpg_step(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, int32_t* update_actor_out, void* stream) {
@@ -567,6 +782,12 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     if (c.discrete && upd && !actor_noise_dev) { mx_set_error("maddpg step: discrete actor update needs the Gumbel draws (actor_noise_dev)"); return 1; }
   }
   cudaStream_t s = (cudaStream_t)stream;
+  if (c.mlp) {
+    if (maddpg_step_mlp(h, b, target_noise_dev, actor_noise_dev, update_actor, s)) return 1;
+    if (update_actor_out) *update_actor_out = update_actor ? 1 : 0;
+    if (h->force_update_actor < 0) h->num_updates += 1;
+    return 0;
+  }
   float* ws = h->ws;
   const MxMaddpgWs& W = h->W;
   const int B = b->B, T = c.episode_len, N = c.n_agents, K = c.num_q, Ac = c.act_dim, S = c.state_dim;
@@ -740,7 +961,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     int dummy = 0;
     if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
     MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, T, N, S, Ac,
-              (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dout, multi ? c.act_offset : 0);
+              (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dout, multi ? c.act_offset : 0, Ac);
     MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
     // actor backward + Adam
     const int ahead_grid = mx_imin_host(mx_num_sms(), mx_ceil_div(Ma, 32));
@@ -859,12 +1080,14 @@ extern "C" int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, do
 }
 extern "C" int64_t mx_maddpg_num_updates(const mx_maddpg* h) { return h->num_updates; }
 
+// cfg.mlp: the critic's target update stops at its trunk -- the target heads stay the target critic's own initialisation
+static int64_t critic_tracked(const mx_maddpg* h) { return h->cfg.mlp ? (int64_t)h->critic.wih : h->Pc; }
 extern "C" int mx_maddpg_soft_update(mx_maddpg* h, void* stream) {
-  if (mx_launch_polyak(h->th_c_tgt, h->th_c, h->Pc, h->cfg.tau, (cudaStream_t)stream)) return 1;
+  if (mx_launch_polyak(h->th_c_tgt, h->th_c, critic_tracked(h), h->cfg.tau, (cudaStream_t)stream)) return 1;
   return mx_launch_polyak(h->th_a_tgt, h->th_a, h->Pa, h->cfg.tau, (cudaStream_t)stream);
 }
 extern "C" int mx_maddpg_hard_update(mx_maddpg* h, void* stream) {
-  cudaMemcpyAsync(h->th_c_tgt, h->th_c, (size_t)h->Pc * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+  cudaMemcpyAsync(h->th_c_tgt, h->th_c, (size_t)critic_tracked(h) * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
   cudaMemcpyAsync(h->th_a_tgt, h->th_a, (size_t)h->Pa * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
   return 0;
 }

@@ -195,7 +195,8 @@ struct OptimArgs {
   float *theta, *theta_tgt, *adam_m, *adam_v;
   const float* gpart;
   float* grad;             // [P + 8]
-  long long P;
+  long long P;             // parameters the optimiser updates: [0, P) of theta / theta_tgt / adam_m / adam_v
+  long long gpart_ld;      // floats between consecutive gradient partials (0: P); larger when the partials also hold frozen tensors past P
   int seg_begin[4], seg_end[4], seg_parts[4], nseg;   // parameter segments and how many partials each has
   const float* spart;
   int spart_n;

@@ -59,13 +59,14 @@ MX_DEVINL float4 optim_reduce_partials(const OptimArgs& a) {
     for (int s = 0; s < a.nseg; ++s)
       if (i >= a.seg_begin[s] && i < a.seg_end[s]) parts = a.seg_parts[s];     // segment bounds are multiples of 4 floats
     const float* gp = a.gpart + i;
+    const long long ld = a.gpart_ld > 0 ? a.gpart_ld : a.P;
     float4 b0 = acc, b1 = acc, b2 = acc, b3 = acc;
     int p = sl;
     for (; p + 28 < parts; p += 32) {
-      const float4 v0 = mx_ld4(gp + (size_t)p * a.P), v1 = mx_ld4(gp + (size_t)(p + 4) * a.P);
-      const float4 v2 = mx_ld4(gp + (size_t)(p + 8) * a.P), v3 = mx_ld4(gp + (size_t)(p + 12) * a.P);
-      const float4 v4 = mx_ld4(gp + (size_t)(p + 16) * a.P), v5 = mx_ld4(gp + (size_t)(p + 20) * a.P);
-      const float4 v6 = mx_ld4(gp + (size_t)(p + 24) * a.P), v7 = mx_ld4(gp + (size_t)(p + 28) * a.P);
+      const float4 v0 = mx_ld4(gp + (size_t)p * ld), v1 = mx_ld4(gp + (size_t)(p + 4) * ld);
+      const float4 v2 = mx_ld4(gp + (size_t)(p + 8) * ld), v3 = mx_ld4(gp + (size_t)(p + 12) * ld);
+      const float4 v4 = mx_ld4(gp + (size_t)(p + 16) * ld), v5 = mx_ld4(gp + (size_t)(p + 20) * ld);
+      const float4 v6 = mx_ld4(gp + (size_t)(p + 24) * ld), v7 = mx_ld4(gp + (size_t)(p + 28) * ld);
       b0.x += v0.x; b0.y += v0.y; b0.z += v0.z; b0.w += v0.w;
       b1.x += v1.x; b1.y += v1.y; b1.z += v1.z; b1.w += v1.w;
       b2.x += v2.x; b2.y += v2.y; b2.z += v2.z; b2.w += v2.w;
@@ -76,7 +77,7 @@ MX_DEVINL float4 optim_reduce_partials(const OptimArgs& a) {
       b3.x += v7.x; b3.y += v7.y; b3.z += v7.z; b3.w += v7.w;
     }
     for (; p < parts; p += 4) {
-      const float4 v = mx_ld4(gp + (size_t)p * a.P);
+      const float4 v = mx_ld4(gp + (size_t)p * ld);
       b0.x += v.x; b0.y += v.y; b0.z += v.z; b0.w += v.w;
     }
     acc.x = (b0.x + b1.x) + (b2.x + b3.x); acc.y = (b0.y + b1.y) + (b2.y + b3.y);

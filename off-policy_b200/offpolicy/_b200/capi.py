@@ -37,7 +37,7 @@ class Episodes(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("obs", "share_obs", "acts", "rewards", "dones", "dones_env", "avail")]
 
 
-ABI_VERSION = 3        # MX_ABI_VERSION of include/marl_b200.h the struct mirrors below correspond to
+ABI_VERSION = 4        # MX_ABI_VERSION of include/marl_b200.h the struct mirrors below correspond to
 
 
 class QmixCfg(C.Structure):
@@ -53,7 +53,8 @@ class MaddpgCfg(C.Structure):
                                           "actor_update_interval", "use_huber", "use_per")] +
                 [(n, C.c_float) for n in ("gamma", "huber_delta", "per_nu", "per_eps", "lr", "adam_beta1", "adam_beta2", "adam_eps",
                                           "max_grad_norm", "tau", "weight_decay", "target_noise")] +
-                [("discrete", C.c_int32), ("no_feature_norm", C.c_int32), ("use_tanh", C.c_int32), ("cent_act_dim", C.c_int32), ("act_offset", C.c_int32)])
+                [("discrete", C.c_int32), ("no_feature_norm", C.c_int32), ("use_tanh", C.c_int32), ("cent_act_dim", C.c_int32), ("act_offset", C.c_int32),
+                 ("mlp", C.c_int32)])
 
 
 class ParamEntry(C.Structure):
@@ -147,6 +148,7 @@ def _declare(lib):
         "mx_tc_linear_probe": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
         "mx_maddpg_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(vp)]),
         "mx_maddpg_num_updates": (i64, [vp]),
+        "mx_maddpg_set_valid": (C.c_int, [vp, vp]),
         "mx_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, C.POINTER(vp)]),
         "mx_graph_launch": (C.c_int, [vp, vp]),
         "mx_graph_destroy": (None, [vp]),

@@ -168,3 +168,26 @@ def build_maddpg(cfg, B, T):
     pol = Policy({"args": args, "device": capi.device()}, info)
     tr = Trainer(args, cfg.n_agents, {"policy_0": pol}, lambda a: "policy_0", device=capi.device(), episode_length=T)
     return args, pol, tr
+
+
+def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td3=False, **over):
+    """(args, policy, trainer) for the transition-level MADDPG (td3 False) / MATD3 (True), one shared policy; `over` sets args fields."""
+    from offpolicy._b200 import capi
+    if td3:
+        from offpolicy.algorithms.matd3.algorithm.MATD3Policy import MATD3Policy as Policy
+        from offpolicy.algorithms.matd3.matd3 import MATD3 as Trainer
+    else:
+        from offpolicy.algorithms.maddpg.algorithm.MADDPGPolicy import MADDPGPolicy as Policy
+        from offpolicy.algorithms.maddpg.maddpg import MADDPG as Trainer
+    args = types.SimpleNamespace(
+        hidden_size=64, layer_N=1, use_ReLU=True, use_feature_normalization=True, use_orthogonal=True, gain=0.01, use_conv1d=False,
+        stacked_frames=1, gamma=0.99, use_per=False, per_nu=0.9, per_eps=1e-6, use_huber_loss=False, huber_delta=10.0, max_grad_norm=10.0,
+        lr=7e-4, opti_eps=1e-5, weight_decay=0.0, tau=0.005, use_popart=False, use_value_active_masks=False, use_same_share_obs=True,
+        batch_size=B, epsilon_start=1.0, epsilon_finish=0.05, epsilon_anneal_time=50000, act_noise_std=0.1, target_action_noise_std=0.2)
+    for k, v in over.items():
+        setattr(args, k, v)
+    info = dict(obs_space=Box(obs_dim, -np.inf, np.inf), share_obs_space=Box(state_dim, -np.inf, np.inf),
+                act_space=Discrete(act_dim) if discrete else Box(act_dim), cent_obs_dim=state_dim, cent_act_dim=act_dim * n_agents)
+    pol = Policy({"args": args, "device": capi.device()}, info)
+    tr = Trainer(args, n_agents, {"policy_0": pol}, lambda a: "policy_0", device=capi.device())
+    return args, pol, tr

@@ -107,3 +107,33 @@ def reference_style_init(entries, cfg, gain, use_orthogonal=True, hyper_layers=2
         linear("mixer.hyper_b2.0", S, HY, 1.0)
         linear("mixer.hyper_b2.2", HY, 1, 1.0)
     return out
+
+
+def mlp_init(in_dim, hidden, heads, use_orthogonal, use_relu=True, feature_norm=True):
+    """MLPBase (mlp.py:52-89: feature LayerNorm, fc1, fc_h, fc2 = deepcopy of fc_h) then the heads [(prefix, out_dim, gain)], in the
+    reference's construction order: nn.Linear's own init, then orthogonal_ / xavier_uniform_ x gain, biases 0.  Returns {name: tensor}."""
+    import torch.nn as nn
+    init_w = nn.init.orthogonal_ if use_orthogonal else nn.init.xavier_uniform_
+    relu_gain = nn.init.calculate_gain("relu" if use_relu else "tanh")
+    sd = {}
+
+    def linear(prefix, i, o, g):
+        m = nn.Linear(i, o)
+        init_w(m.weight.data, gain=g)
+        m.bias.data.zero_()
+        sd[prefix + ".weight"], sd[prefix + ".bias"] = m.weight.data, m.bias.data
+
+    def lnorm(prefix, n):
+        sd[prefix + ".weight"], sd[prefix + ".bias"] = torch.ones(n), torch.zeros(n)
+
+    if feature_norm:
+        lnorm("mlp.feature_norm", in_dim)
+    linear("mlp.mlp.fc1.0", in_dim, hidden, relu_gain)
+    lnorm("mlp.mlp.fc1.2", hidden)
+    linear("mlp.mlp.fc_h.0", hidden, hidden, relu_gain)
+    lnorm("mlp.mlp.fc_h.2", hidden)
+    for k in ("0.weight", "0.bias", "2.weight", "2.bias"):
+        sd["mlp.mlp.fc2.0." + k] = sd["mlp.mlp.fc_h." + k].clone()
+    for prefix, o, g in heads:
+        linear(prefix, hidden, o, g)
+    return sd

@@ -1,7 +1,7 @@
 """Fall-through to the reference tree for everything OUTSIDE the accelerated hot path.
 
 The drop-in package shadows only the modules SURVEY.md section 8(b) lists; `offpolicy.runner`, `offpolicy.envs`,
-`offpolicy.config`, `offpolicy.scripts`, the MLP algorithms (maddpg, matd3, mqmix, mvdn) and the remaining
+`offpolicy.config`, `offpolicy.scripts` and the remaining
 `offpolicy.utils.*` helpers keep coming, byte-identical, from the reference checkout when one is present
 (OFFPOLICY_REFERENCE_ROOT, default /root/reference).  Without a checkout the hot-path modules still work standalone.
 """

@@ -9,38 +9,16 @@ import numpy as np
 import torch
 
 from offpolicy._b200 import capi
-from offpolicy._b200.flat import FlatModule
+from offpolicy._b200.flat import FlatModule, mlp_init
 from offpolicy._b200.host_util import LinearDecay, space_dim, is_discrete, onehot
 from offpolicy.algorithms.qmix.algorithm.QMixPolicy import qmix_cfg_struct, param_entries
 
 
 def mlp_reference_style_init(entries, in_dim, hidden, act_dim, gain, use_orthogonal=True, use_relu=True):
-    """Initial weights in the reference's construction order (MLPBase: feature LayerNorm, fc1, fc_h, fc2 = clone of fc_h, mlp.py:14-29;
-    then ACTLayer, act.py:10-20) so that a seeded run consumes torch's generator identically."""
-    import torch.nn as nn
-    init_w = nn.init.orthogonal_ if use_orthogonal else nn.init.xavier_uniform_
-    relu_gain = nn.init.calculate_gain("relu" if use_relu else "tanh")
-    out = {}
-
-    def linear(prefix, i, o, g):
-        m = nn.Linear(i, o)
-        init_w(m.weight.data, gain=g)
-        m.bias.data.zero_()
-        out[prefix + ".weight"], out[prefix + ".bias"] = m.weight.data, m.bias.data
-
-    def lnorm(prefix, n):
-        out[prefix + ".weight"], out[prefix + ".bias"] = torch.ones(n), torch.zeros(n)
-
-    if any(n.endswith("mlp.feature_norm.weight") for n, *_ in entries):      # absent with --use_feature_normalization off
-        lnorm("mlp.feature_norm", in_dim)
-    linear("mlp.mlp.fc1.0", in_dim, hidden, relu_gain)
-    lnorm("mlp.mlp.fc1.2", hidden)
-    linear("mlp.mlp.fc_h.0", hidden, hidden, relu_gain)
-    lnorm("mlp.mlp.fc_h.2", hidden)
-    for k in ("0.weight", "0.bias", "2.weight", "2.bias"):
-        out["mlp.mlp.fc2.0." + k] = out["mlp.mlp.fc_h." + k].clone()
-    linear("q.action_out", hidden, act_dim, gain)
-    return out
+    """Initial weights in the reference's construction order (MLPBase, mlp.py:14-29, then ACTLayer, act.py:10-20) so that a seeded run
+    consumes torch's generator identically; keys of the q_network views."""
+    fn = any(n.endswith("mlp.feature_norm.weight") for n, *_ in entries)      # absent with --use_feature_normalization off
+    return mlp_init(in_dim, hidden, [("q.action_out", act_dim, gain)], use_orthogonal, use_relu, fn)
 
 
 class M_QMixPolicy(object):

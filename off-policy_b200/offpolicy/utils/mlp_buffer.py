@@ -5,10 +5,12 @@ step 1 = (next_obs, next_share_obs, next_avail_acts), plus acts / rewards / done
 wrap, uniform and prioritised sampling (device-side fp64 trees), running reward statistics and the 128-bit gather kernel are the ones
 of the recurrent path; `sample()` returns the reference's 13-tuple (11 fields + importance weights + indices, the last two None for
 uniform sampling) whose entries materialise the reference's NumPy layout
-on access while the B200 trainer (algorithms/mqmix/mqmix.py) reads the device-side batch directly.  `valid_transition` is not
-consumed by any shared-policy learner kernel and is kept in a host-side array.
+on access while the B200 trainers (algorithms/mqmix/mqmix.py, algorithms/maddpg/maddpg.py) read the device-side batch directly.
+`valid_transition` is kept twice: a host array for `materialize`, and a device copy [buffer_size][N] (`valid_dev`) that the MADDPG /
+MATD3 actor loss reads through the batch's sampled indices.
 """
 import numpy as np
+import torch
 
 from offpolicy.utils.rec_buffer import RecPolicyBuffer, _LazyField
 
@@ -64,6 +66,7 @@ class MlpPolicyBuffer(object):
         self.rep = RecPolicyBuffer(buffer_size, 1, num_agents, obs_space, share_obs_space, act_space, use_same_share_obs, use_avail_acts,
                                    use_reward_normalization, use_per=use_per, per_alpha=per_alpha, max_batch=max_batch or 1024)
         self.valid_transition = np.zeros((self.buffer_size, self.num_agents, 1), dtype=np.float32)      # mlp_buffer.py:156
+        self.valid_dev = torch.zeros(self.buffer_size, self.num_agents, dtype=torch.float32, device=self.rep.dev)
 
     @property
     def filled_i(self):
@@ -86,6 +89,8 @@ class MlpPolicyBuffer(object):
         idx = self.rep.insert(n, np.stack([obs, next_obs], 0), np.stack([f32(share_obs), f32(next_share_obs)], 0), f32(acts)[None],
                               f32(rewards)[None], f32(dones)[None], f32(dones_env).reshape(1, n, 1), av)
         self.valid_transition[idx] = f32(valid_transition).reshape(n, self.num_agents, 1)
+        self.valid_dev[torch.from_numpy(np.asarray(idx, dtype=np.int64)).to(self.rep.dev)] = \
+            torch.from_numpy(self.valid_transition[idx, :, 0]).to(self.rep.dev)
         return idx
 
     # -- reference layout of one sampled field (mlp_buffer.py:203-240: `_cast` = transpose(1, 0, 2)) ----------------

@@ -1,0 +1,123 @@
+"""Grad-steps/s of the transition-level MADDPG / MATD3 learner at the shapes of scripts/train_mpe_maddpg.sh: simple_spread (3 agents,
+obs 18, Discrete(5), shared observation 54), B = 1 000 transitions drawn from a replay of 500 000.
+
+GPU arm: the whole-update CUDA graph (device uniform draw + gather -> mx_maddpg step -> soft target update), the per-update noise drawn
+on the host from torch's CPU generator exactly as the reference draws it and copied into the graph's fixed buffers before each replay;
+timed over `--steps` replays after `--warmup`, ending in a device synchronise.  CPU arm: oracle/maddpg_mlp.py (the reference's
+update restated in eager PyTorch) on the same host and shapes, with its thread count and the host's core count.
+Prints one JSON line per algorithm.  Needs a CUDA device; it never falls back to the CPU for the GPU arm.
+
+    python tools/bench_mlp_maddpg.py --steps 500 --warmup 50
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "off-policy_b200"), os.path.join(ROOT, "tests")]
+
+N, O, A, S = 3, 18, 5, 54
+
+
+def fill(buf, B, size, rng):
+    from mlp_maddpg_checks import synth_batch
+    tr = lambda x: np.asarray(x["policy_0"]).transpose(1, 0, 2)
+    for _ in range(size // B):
+        b = synth_batch(rng, N, B, O, S, A, True)
+        buf.insert(B, {"policy_0": tr(b[0])}, {"policy_0": b[1]["policy_0"]}, {"policy_0": tr(b[2])}, {"policy_0": tr(b[3])},
+                   {"policy_0": tr(b[4])}, {"policy_0": b[5]["policy_0"]}, {"policy_0": tr(b[6])}, {"policy_0": b[7]["policy_0"]},
+                   {"policy_0": tr(b[8])}, None, None)
+
+
+def gpu_arm(td3, B, size, steps, warmup):
+    from offpolicy._b200 import capi
+    from offpolicy._b200.factory import build_mlp_maddpg, Discrete, Box
+    from offpolicy.utils.mlp_buffer import MlpReplayBuffer
+    lib = capi.lib()
+    side = torch.cuda.Stream()
+    with torch.cuda.stream(side):
+        torch.manual_seed(1)
+        args, pol, tr = build_mlp_maddpg(N, O, A, S, B, discrete=True, td3=td3)
+        info = {"policy_0": dict(obs_space=Box(O), share_obs_space=Box(S), act_space=Discrete(A))}
+        buf = MlpReplayBuffer(info, {"policy_0": [0, 1, 2]}, size, True, False, max_batch=B)
+        fill(buf, B, size, np.random.default_rng(2))
+        buf.seed_device_rng(3)
+        pb = buf.policy_buffers["policy_0"]
+        capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(pb.valid_dev)))
+        tn, an = torch.zeros(B, 2, N, A, device="cuda"), torch.zeros(B, 2, N, A, device="cuda")
+        g = C.c_void_p()
+        capi.check(lib.mx_maddpg_graph_capture(pb.rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn), capi.ptr(an), 1, capi.stream_ptr(),
+                                               C.byref(g)))
+
+        def one():
+            for dst, draw, step in ((tn, tr.draw_target_noise(B), 1), (an, tr.draw_actor_noise(B), 0)):
+                if draw is not None:
+                    dst.copy_(tr._rows(draw, B, step))
+            capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
+        for _ in range(warmup):
+            one()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(steps):
+            one()
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+        loss = float(tr._info[0])
+    assert np.isfinite(loss)
+    return steps / dt, loss
+
+
+def cpu_arm(td3, B, steps):
+    from mlp_maddpg_checks import synth_batch
+    from oracle.maddpg_mlp import MlpMaddpg, draw_noise
+    from offpolicy._b200.flat import mlp_init
+    torch.manual_seed(1)
+    heads = [("q_outs.%d" % k, 1, 1.0) for k in range(2 if td3 else 1)]
+    a = mlp_init(O, 64, [("act.action_out", A, 0.01)], True)
+    c = mlp_init(S + N * A, 64, heads, True)
+    ct = mlp_init(S + N * A, 64, heads, True)
+    split = lambda d, head: {k: v for k, v in d.items() if k.startswith("q_outs") == head}
+    L = MlpMaddpg(a, split(c, False), split(c, True), a, split(c, False), split(ct, True), True, td3, lr=5e-4)
+    rng = np.random.default_rng(4)
+    batches = [synth_batch(rng, N, B, O, S, A, True) for _ in range(4)]
+    L.step(batches[0], *draw_noise(N, B, A, True, td3, 0.2))
+    t0 = time.perf_counter()
+    for i in range(steps):
+        L.step(batches[i % 4], *draw_noise(N, B, A, True, td3, 0.2))
+        L.soft_update()
+    return steps / (time.perf_counter() - t0)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=500)
+    ap.add_argument("--warmup", type=int, default=50)
+    ap.add_argument("--batch", type=int, default=1000)
+    ap.add_argument("--buffer", type=int, default=500_000)
+    ap.add_argument("--cpu-steps", type=int, default=20)
+    ap.add_argument("--algo", choices=["maddpg", "matd3", "both"], default="both")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_mlp_maddpg: needs a CUDA device")
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    for algo in (["maddpg", "matd3"] if a.algo == "both" else [a.algo]):
+        td3 = algo == "matd3"
+        rate, loss = gpu_arm(td3, a.batch, a.buffer, a.steps, a.warmup)
+        cpu = cpu_arm(td3, a.batch, a.cpu_steps)
+        print(json.dumps({"metric": "grad-steps/s", "algo": algo, "value": rate, "unit": "steps/s", "batch": a.batch, "buffer": a.buffer,
+                          "steps": a.steps, "warmup": a.warmup, "path": "CUDA graph: device draw + gather + mx_maddpg step (mlp) + soft update; "
+                          "host noise draws copied in per step", "last_critic_loss": loss, "gpu": q,
+                          "cpu_oracle": {"value": cpu, "unit": "steps/s", "torch_threads": torch.get_num_threads(), "host_cores": os.cpu_count(),
+                                         "steps": a.cpu_steps, "kind": "oracle/maddpg_mlp.py (eager PyTorch restatement of the reference update)"},
+                          "speedup_vs_cpu_oracle": rate / cpu}))
+
+
+if __name__ == "__main__":
+    main()
