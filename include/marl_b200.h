@@ -282,7 +282,8 @@ typedef struct mx_maddpg_cfg {
    * without recurrence, a batch = B transitions stored as episodes of length 1 (episode_len must be 1; step 0 = obs, step 1 = next
    * obs).  The critic's K Q heads are not trained (a plain list in the reference, SURVEY.md App. D-6): the live and the target heads
    * are two fixed initialisations kept behind the critic's trunk, outside the range Adam, clipping and the target updates touch.
-   * The actor loss is masked by valid_transition (mx_maddpg_set_valid).  One shared policy only (cent_act_dim = 0). */
+   * The actor loss is masked by valid_transition (mx_maddpg_set_valid).  Several policies work as in the recurrent learner
+   * (cent_act_dim > 0, mx_maddpg_cent_contribute before every step); mx_maddpg_graph_capture takes one shared policy only. */
   int32_t mlp;
 } mx_maddpg_cfg;
 /* which = 0: actor ("rnn.*", "act.action_out.*"), 1: critic ("rnn.*", "q_outs.k.*"); names = reference state_dict keys.
@@ -303,9 +304,10 @@ int mx_maddpg_step(mx_maddpg* h, const mx_batch* batch, const float* target_nois
  * update the actor; batch->avail (or NULL) masks unavailable actions to -1e10 like util.py:115,141. */
 int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* batch, const float* target_noise_dev, const float* actor_noise_dev,
                       int32_t* update_actor_out, void* stream);
-/* Several policies: r_maddpg.py:40-105 (get_update_info).  Runs src's TARGET actor over src_batch (noise as in mx_maddpg_step_ex) and
- * writes src's columns of the two centralised action vectors (buffer actions; target actions at t+1) into dst's workspace.  Before
- * mx_maddpg_step_ex(dst, ...) call it once per policy, dst itself included (same stream). */
+/* Several policies: r_maddpg.py:40-105 / maddpg.py:38-81 (get_update_info).  Runs src's TARGET actor over src_batch (noise as in
+ * mx_maddpg_step_ex) and writes src's columns of the two centralised action vectors (buffer actions; target actions at t+1; for
+ * cfg.mlp the next-observation step of the transition) into dst's workspace.  Before mx_maddpg_step_ex(dst, ...) call it once per
+ * policy, dst itself included (same stream). */
 int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* src_batch, const float* target_noise_dev, mx_maddpg* dst, void* stream);
 /* Whole-update CUDA graph (declared with mx_graph below): [sample ->] step [-> PER write-back] [-> soft update when the actor
  * was updated, base_runner.py:250-252]; flags as for mx_graph_capture.  One graph per variant (update_actor = 1 / 0); the two

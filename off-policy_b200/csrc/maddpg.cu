@@ -423,8 +423,8 @@ static int maddpg_check(const mx_maddpg_cfg* c) {
     mx_set_error("mx_maddpg: act_offset %d + n_agents*act_dim %d exceeds cent_act_dim %d", c->act_offset, c->n_agents * c->act_dim, c->cent_act_dim); return 1;
   }
   if (c->cent_act_dim == 0 && c->act_offset != 0) { mx_set_error("mx_maddpg: act_offset needs cent_act_dim"); return 1; }
-  if (c->mlp && (c->episode_len != 1 || c->cent_act_dim != 0)) {
-    mx_set_error("mx_maddpg: the MLP (transition-level) variant takes transitions as episodes of length 1 and one shared policy"); return 1;
+  if (c->mlp && c->episode_len != 1) {
+    mx_set_error("mx_maddpg: the MLP (transition-level) variant takes transitions as episodes of length 1"); return 1;
   }
   return 0;
 }
@@ -631,6 +631,9 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
 // agent-replaced copies).  No recurrence: every net is the front kernel with its head in the weight_ih slot, and k_front_bwd runs
 // with no_gru.  The critic's heads are frozen (not in the reference's parameters()): the live heads give Q(s, a) and, in the actor
 // phase, the gradient path into the actor; the target heads give Q'(s', a').
+// Several policies (cent_act_dim > 0): the centralised action vectors were assembled by mx_maddpg_cent_contribute, so the step runs
+// only the live actor and never reads its own target actions; the batch is this policy's (rewards, dones_env, shared observation,
+// PER weights, maddpg.py:103-107) and the valid_transition store is this policy's [rows][n_agents].
 static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor,
                            cudaStream_t s) {
   const mx_maddpg_cfg& c = h->cfg;
@@ -642,6 +645,7 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   const MxNetLayout& LA = h->actor;
   const MxNetLayout& LC = h->critic;
   const int fnorm = c.no_feature_norm ? 0 : 1;
+  const bool multi = c.cent_act_dim > 0;
 
   // ---------- A. live + target actor on obs and next_obs; target actions a' from the next_obs rows (maddpg.py:64-74) ----------
   FrontFwdArgs ff;
@@ -651,11 +655,13 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   ff.theta[0] = h->th_a; ff.theta[1] = h->th_a_tgt; ff.L = LA;
   ff.gi[0] = ws + W.a_gi[0]; ff.gi[1] = ws + W.a_gi[1];
   ff.u1 = ws + W.a_u1; ff.u2 = ws + W.a_u2; ff.st0 = ws + W.a_st0; ff.st1 = ws + W.a_st1; ff.st2 = ws + W.a_st2;
-  if (mx_launch_front_fwd(ff, 2, s)) return 1;
-  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[1], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
-            ws + W.a_nact, nullptr);
-  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  if (c.discrete) {      // onehot_from_logits with the next-avail mask (MADDPG) / hard Gumbel-softmax, the draw already added (MATD3)
+  if (mx_launch_front_fwd(ff, multi ? 1 : 2, s)) return 1;      // several policies: the target actions come from cent_nacts
+  if (!multi) {
+    MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[1], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
+              ws + W.a_nact, nullptr);
+    MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  }
+  if (c.discrete && !multi) {      // onehot_from_logits with the next-avail mask (MADDPG) / hard Gumbel-softmax, the draw already added (MATD3)
     ActXformArgs ax;
     memset(&ax, 0, sizeof(ax));
     ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
@@ -668,6 +674,7 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   memset(&pk, 0, sizeof(pk));
   pk.B = B; pk.T = 1; pk.N = N; pk.S = S; pk.Ac = Ac; pk.share = b->share; pk.share_ld = b->share_ld; pk.acts = b->acts; pk.act_ld = b->act_ld;
   pk.ldx = ldc;
+  if (multi) { pk.CA = c.cent_act_dim; pk.off = c.act_offset; pk.ca_ld = mx_round_up(c.cent_act_dim, 4); pk.cent_acts = ws + W.cent_acts; pk.cent_nacts = ws + W.cent_nacts; }
   pk.mode = 0; pk.x = ws + W.c_x;
   MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
   pk.mode = 1; pk.x = ws + W.t_x; pk.actor_out = ws + W.a_nact;
@@ -747,7 +754,7 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   int dummy = 0;
   if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
   MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, 1, N, S, Ac,
-            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, 0, (int)MX_G);
+            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, c.act_offset, (int)MX_G);
   MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
   FrontBwdArgs fba;
   memset(&fba, 0, sizeof(fba));
@@ -1018,7 +1025,9 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
   if (!src || !dst || !b) { mx_set_error("mx_maddpg_cent_contribute: null argument"); return 1; }
   const mx_maddpg_cfg& c = src->cfg;
   const mx_maddpg_cfg& d = dst->cfg;
-  if (c.cent_act_dim <= 0 || d.cent_act_dim != c.cent_act_dim || d.episode_len != c.episode_len) { mx_set_error("mx_maddpg_cent_contribute: both learners need the same cent_act_dim > 0 and episode length"); return 1; }
+  if (c.cent_act_dim <= 0 || d.cent_act_dim != c.cent_act_dim || d.episode_len != c.episode_len || d.mlp != c.mlp) {
+    mx_set_error("mx_maddpg_cent_contribute: both learners need the same cent_act_dim > 0, episode length and mlp flag"); return 1;
+  }
   if (b->B <= 0 || b->B > c.max_batch || b->B > d.max_batch) { mx_set_error("mx_maddpg_cent_contribute: batch size outside [1, max_batch]"); return 1; }
   if (!b->obs || !b->acts) { mx_set_error("mx_maddpg_cent_contribute: missing batch field"); return 1; }
   if (c.target_noise > 0.f && !target_noise_dev) { mx_set_error("mx_maddpg_cent_contribute: MATD3 target noise expected"); return 1; }
@@ -1034,16 +1043,24 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
   ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
   ff.theta[0] = src->th_a_tgt; ff.L = LA; ff.gi[0] = ws + W.a_gi[1];
   if (mx_launch_front_fwd(ff, 1, s)) return 1;
-  GruFwdArgs gf;
-  memset(&gf, 0, sizeof(gf));
-  gf.theta[0] = src->th_a_tgt; gf.whh = LA.whh; gf.bhh = LA.bhh; gf.gi[0] = ff.gi[0]; gf.hall[0] = ws + W.a_h[1]; gf.R = B * N; gf.T = T; gf.N = N;
-  if (mx_launch_gru_fwd(gf, 1, s)) return 1;
-  HeadArgs ha;
-  memset(&ha, 0, sizeof(ha));
-  ha.lno_g = LA.lno_g; ha.lno_b = LA.lno_b; ha.w = LA.wq; ha.b = LA.bq; ha.OD = Ac; ha.b_stride = 1; ha.w_stride = MX_H; ha.M = Ma;
-  ha.theta = src->th_a_tgt; ha.h = gf.hall[0]; ha.out = ws + W.a_nact; ha.noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
-  MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
-  if (c.discrete) {
+  if (c.mlp) {
+    // maddpg.py:64-74: no recurrence, the head sits in the weight_ih slot (as maddpg_step_mlp phase A).  The noise rows are the
+    // step-1 (next-observation) rows [b][2][N][Ac]; k_cent_scatter's row (b*(T+1)+t+1)*N+n with T = 1, t = 0 is that same step.
+    MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[0], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
+              ws + W.a_nact, nullptr);
+    MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
+  } else {
+    GruFwdArgs gf;
+    memset(&gf, 0, sizeof(gf));
+    gf.theta[0] = src->th_a_tgt; gf.whh = LA.whh; gf.bhh = LA.bhh; gf.gi[0] = ff.gi[0]; gf.hall[0] = ws + W.a_h[1]; gf.R = B * N; gf.T = T; gf.N = N;
+    if (mx_launch_gru_fwd(gf, 1, s)) return 1;
+    HeadArgs ha;
+    memset(&ha, 0, sizeof(ha));
+    ha.lno_g = LA.lno_g; ha.lno_b = LA.lno_b; ha.w = LA.wq; ha.b = LA.bq; ha.OD = Ac; ha.b_stride = 1; ha.w_stride = MX_H; ha.M = Ma;
+    ha.theta = src->th_a_tgt; ha.h = gf.hall[0]; ha.out = ws + W.a_nact; ha.noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
+    MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
+  }
+  if (c.discrete) {      // one-hot with the next-avail mask (MADDPG) / hard Gumbel-softmax (MATD3)
     ActXformArgs ax;
     memset(&ax, 0, sizeof(ax));
     ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
@@ -1062,6 +1079,11 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
 extern "C" int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                                        const float* actor_noise_dev, int32_t update_actor, void* stream, mx_graph** out) {
   if (!r || !h || !out) { mx_set_error("mx_maddpg_graph_capture: null argument"); return 1; }
+  if (h->cfg.mlp && h->cfg.cent_act_dim > 0) {      // the graph would replay the step without the other policies' contributions
+    mx_set_error("mx_maddpg_graph_capture: an MLP learner with several policies (cent_act_dim > 0) cannot be captured: its step needs "
+                 "mx_maddpg_cent_contribute from every policy first; run it eagerly");
+    return 1;
+  }
   if ((flags & 2u) && mx_replay_set_beta(r, beta, stream)) return 1;
   auto seq = [=](void* st) -> int {
     if (flags & 1u) { if (mx_replay_sample_uniform(r, B, st)) return 1; }

@@ -170,15 +170,18 @@ def build_maddpg(cfg, B, T):
     return args, pol, tr
 
 
-def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td3=False, **over):
-    """(args, policy, trainer) for the transition-level MADDPG (td3 False) / MATD3 (True), one shared policy; `over` sets args fields."""
-    from offpolicy._b200 import capi
+def _mlp_maddpg_classes(td3):
     if td3:
         from offpolicy.algorithms.matd3.algorithm.MATD3Policy import MATD3Policy as Policy
         from offpolicy.algorithms.matd3.matd3 import MATD3 as Trainer
     else:
         from offpolicy.algorithms.maddpg.algorithm.MADDPGPolicy import MADDPGPolicy as Policy
         from offpolicy.algorithms.maddpg.maddpg import MADDPG as Trainer
+    return Policy, Trainer
+
+
+def mlp_maddpg_args(B, **over):
+    """Namespace fields MADDPGPolicy / MADDPG / MATD3 read (config.py defaults); `over` sets args fields."""
     args = types.SimpleNamespace(
         hidden_size=64, layer_N=1, use_ReLU=True, use_feature_normalization=True, use_orthogonal=True, gain=0.01, use_conv1d=False,
         stacked_frames=1, gamma=0.99, use_per=False, per_nu=0.9, per_eps=1e-6, use_huber_loss=False, huber_delta=10.0, max_grad_norm=10.0,
@@ -186,8 +189,38 @@ def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td
         batch_size=B, epsilon_start=1.0, epsilon_finish=0.05, epsilon_anneal_time=50000, act_noise_std=0.1, target_action_noise_std=0.2)
     for k, v in over.items():
         setattr(args, k, v)
+    return args
+
+
+def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td3=False, **over):
+    """(args, policy, trainer) for the transition-level MADDPG (td3 False) / MATD3 (True), one shared policy; `over` sets args fields."""
+    from offpolicy._b200 import capi
+    Policy, Trainer = _mlp_maddpg_classes(td3)
+    args = mlp_maddpg_args(B, **over)
     info = dict(obs_space=Box(obs_dim, -np.inf, np.inf), share_obs_space=Box(state_dim, -np.inf, np.inf),
                 act_space=Discrete(act_dim) if discrete else Box(act_dim), cent_obs_dim=state_dim, cent_act_dim=act_dim * n_agents)
     pol = Policy({"args": args, "device": capi.device()}, info)
     tr = Trainer(args, n_agents, {"policy_0": pol}, lambda a: "policy_0", device=capi.device())
     return args, pol, tr
+
+
+def build_mlp_maddpg_multi(specs, state_dim, B, discrete=True, td3=False, **over):
+    """(args, {policy_id: policy}, trainer, agents) for the transition-level MADDPG / MATD3 with several policies (share_policy off).
+    specs: one (obs_dim, act_dim) or (obs_dim, act_dim, n_agents) per policy; policy_i controls the next n_agents agents (1 by default),
+    agents = {policy_id: [agent ids]}.  The policies are constructed in id order, as train_mpe.py:139-150 does."""
+    from offpolicy._b200 import capi
+    Policy, Trainer = _mlp_maddpg_classes(td3)
+    args = mlp_maddpg_args(B, **over)
+    specs = [tuple(s) + (1,) * (3 - len(s)) for s in specs]
+    total = sum(a * n for _, a, n in specs)
+    pols, agents, mapping, nxt = {}, {}, {}, 0
+    for i, (o, a, n) in enumerate(specs):
+        p = "policy_%d" % i
+        info = dict(obs_space=Box(o, -np.inf, np.inf), share_obs_space=Box(state_dim, -np.inf, np.inf),
+                    act_space=Discrete(a) if discrete else Box(a), cent_obs_dim=state_dim, cent_act_dim=total)
+        pols[p] = Policy({"args": args, "device": capi.device()}, info)
+        agents[p] = list(range(nxt, nxt + n))
+        mapping.update({k: p for k in agents[p]})
+        nxt += n
+    tr = Trainer(args, nxt, pols, lambda k: mapping[k], device=capi.device())
+    return args, pols, tr, agents

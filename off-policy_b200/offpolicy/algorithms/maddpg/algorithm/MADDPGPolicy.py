@@ -51,8 +51,10 @@ class MADDPGPolicy(object):
         self.num_q = 2 if td3 else 1
         cfg = maddpg_cfg_struct(self.args, 1, self.obs_dim, self.act_dim, self.central_obs_dim, 1, 1, td3, target_noise, 1, self.discrete,
                                 mlp=True)
-        # the critic input is [cent_obs | centralised action]: cent_act_dim = n_agents * act_dim with one shared policy
+        # the critic input is [cent_obs | centralised action]: cent_act_dim = n_agents * act_dim with one shared policy, the total action
+        # width of all agents with one policy per agent (which need not be a multiple of this policy's act_dim)
         cfg.n_agents = max(1, self.central_act_dim // self.act_dim)
+        cfg.cent_act_dim = self.central_act_dim
         self._a_entries, self.Pa = maddpg_entries(cfg, 0)
         self._c_entries, self.Pc = maddpg_entries(cfg, 1)
         self._h_entries, _ = maddpg_entries(cfg, 2)

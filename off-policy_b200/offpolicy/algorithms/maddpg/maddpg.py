@@ -8,8 +8,14 @@ N(0, target_action_noise_std) for Box actions), then the actor update's Gumbel d
 
 The reference never increments `num_updates` here (maddpg.py:33, 100; compare r_maddpg.py:330), so `update_actor` is always True and
 MATD3 updates its actor on every call despite `actor_update_interval = 2` (SURVEY.md App. D-14).  The learner is therefore
-configured with an actor update interval of 1.  Only the shared-policy, shared-observation form is built:
-`cent_train_policy_on_batch`, several policies and `--use_popart` raise."""
+configured with an actor update interval of 1.
+
+Several policies (`--share_policy` off, train_mpe.py:139-150: one policy per agent, possibly with different observation and action
+spaces) get one learner each.  Every critic sees the actions of all agents: `cent_act_dim` is the total action width and each policy's
+agents sit at `act_offset`, in sorted policy-id order (maddpg.py:55-79).  Before a policy's step, every policy q writes its buffer
+actions and its target actor's next actions into the updated policy's centralised action vectors (`mx_maddpg_cent_contribute`), q by q
+in id order, which is also the order of the reference's target-noise draws.  Only the shared-observation form is built:
+`cent_train_policy_on_batch` and `--use_popart` raise."""
 import ctypes as C
 
 import numpy as np
@@ -67,14 +73,44 @@ class _HostTransitions(object):
         return b
 
 
+class _Engine(object):
+    """One policy's learner: its mx_maddpg handle (cfg.mlp), the workspace views and the host-batch staging."""
+
+    def __init__(self, args, pol, n_agents, max_batch, cent_act_dim, act_offset):
+        lib = capi.lib()
+        self.pol, self.n_agents = pol, n_agents
+        # cfg.target_noise > 0 tells the learner that target-action noise is passed.  MATD3 always smooths (MADDPGPolicy.py:93, 111 test
+        # `target_noise is not None`): a Discrete actor takes Gumbel draws whatever the std, a Box actor N(0, std) draws, all-zero at std 0
+        tnoise = (1.0 if pol.discrete else float(pol.target_noise)) if pol.td3 else 0.0
+        self.cfg = maddpg_cfg_struct(args, n_agents, pol.obs_dim, pol.act_dim, pol.central_obs_dim, 1, max_batch, pol.td3, tnoise, 1,
+                                     pol.discrete, cent_act_dim=cent_act_dim, act_offset=act_offset, mlp=True)
+        nbytes = int(lib.mx_maddpg_workspace_bytes(C.byref(self.cfg)))
+        if nbytes < 0:
+            raise capi.MxError(lib.mx_last_error().decode())
+        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=capi.device())
+        av = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.actor_vecs])
+        cv = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.critic_vecs])
+        h = C.c_void_p()
+        capi.check(lib.mx_maddpg_create(C.byref(self.cfg), av, cv, capi.ptr(self.workspace), nbytes, C.byref(h)))
+        self.handle = h
+        ip = lib.mx_maddpg_info(h) - self.workspace.data_ptr()
+        self.info = self.workspace[ip:ip + 32].view(torch.float32)
+        pp = lib.mx_maddpg_priorities(h) - self.workspace.data_ptr()
+        self.prio = self.workspace[pp:pp + 4 * max_batch].view(torch.float32)
+        self.host_batch = None
+
+    def close(self):
+        if self.handle:
+            capi.lib().mx_maddpg_destroy(self.handle)
+            self.handle = None
+
+
 class MADDPG(object):
     def __init__(self, args, num_agents, policies, policy_mapping_fn, device=None, actor_update_interval=1):
         self.args = args
         self.use_per = args.use_per
         if getattr(args, "use_popart", False):
             raise NotImplementedError("B200 MADDPG path: --use_popart is not implemented")
-        if list(policies.keys()) != ["policy_0"]:
-            raise NotImplementedError("B200 MADDPG path: only one shared policy is implemented (the transition replay is shared-policy only)")
         self.num_agents = num_agents
         self.policies = policies
         self.policy_mapping_fn = policy_mapping_fn
@@ -85,83 +121,80 @@ class MADDPG(object):
         self.actor_update_interval = actor_update_interval
         self.max_batch = int(getattr(args, "batch_size", 32))
         self.dev = capi.device()
-        pol = self.policies["policy_0"]
-        self.pol = pol
-        N = len(self.policy_agents["policy_0"])
-        if pol.central_act_dim != N * pol.act_dim:
-            raise NotImplementedError("B200 MADDPG path: cent_act_dim %d != n_agents * act_dim %d" % (pol.central_act_dim, N * pol.act_dim))
-        lib = capi.lib()
-        # cfg.target_noise > 0 tells the learner that target-action noise is passed.  MATD3 always smooths (MADDPGPolicy.py:93, 111 test
-        # `target_noise is not None`): a Discrete actor takes Gumbel draws whatever the std, a Box actor N(0, std) draws, all-zero at std 0
-        tnoise = (1.0 if pol.discrete else float(pol.target_noise)) if pol.td3 else 0.0
-        self.cfg = maddpg_cfg_struct(args, N, pol.obs_dim, pol.act_dim, pol.central_obs_dim, 1, self.max_batch, pol.td3, tnoise, 1,
-                                     pol.discrete, mlp=True)
-        nbytes = int(lib.mx_maddpg_workspace_bytes(C.byref(self.cfg)))
-        if nbytes < 0:
-            raise capi.MxError(lib.mx_last_error().decode())
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.dev)
-        av = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.actor_vecs])
-        cv = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.critic_vecs])
-        h = C.c_void_p()
-        capi.check(lib.mx_maddpg_create(C.byref(self.cfg), av, cv, capi.ptr(self.workspace), nbytes, C.byref(h)))
-        self.handle = h
-        pol._trainer, pol._handle = self, h
-        ip = lib.mx_maddpg_info(h) - self.workspace.data_ptr()
-        self._info = self.workspace[ip:ip + 32].view(torch.float32)
-        pp = lib.mx_maddpg_priorities(h) - self.workspace.data_ptr()
-        self._prio = self.workspace[pp:pp + 4 * self.max_batch].view(torch.float32)
-        self._host_batch = None
+        self.multi = len(self.policy_ids) > 1
+        total = sum(len(self.policy_agents[p]) * self.policies[p].act_dim for p in self.policy_ids)
+        self._eng = {}
+        off = 0
+        for p in self.policy_ids:                    # the centralised action vector: sorted ids, each policy's agents in order
+            pol, n_p = self.policies[p], len(self.policy_agents[p])
+            if self.multi and pol.central_act_dim != total:
+                raise ValueError("policy %s: cent_act_dim %d != total action width %d of all agents" % (p, pol.central_act_dim, total))
+            if not self.multi and pol.central_act_dim != n_p * pol.act_dim:
+                raise NotImplementedError("B200 MADDPG path: cent_act_dim %d != n_agents * act_dim %d" % (pol.central_act_dim, n_p * pol.act_dim))
+            self._eng[p] = _Engine(args, pol, n_p, self.max_batch, total if self.multi else 0, off if self.multi else 0)
+            pol._trainer, pol._handle = self, self._eng[p].handle
+            off += n_p * pol.act_dim
+        first = self._eng[self.policy_ids[0]]
+        # the first policy's learner under the single-policy names (graph helpers, tests)
+        self.pol, self.cfg, self.workspace, self.handle, self._info, self._prio = first.pol, first.cfg, first.workspace, first.handle, first.info, first.prio
         self._noise_dev = self._actor_noise_dev = None
+        self._keep = None
 
     def __del__(self):
         try:
-            if getattr(self, "handle", None):
-                capi.lib().mx_maddpg_destroy(self.handle)
-                self.handle = None
+            for e in getattr(self, "_eng", {}).values():
+                e.close()
+            self.handle = None
         except Exception:
             pass
 
-    def grad_views(self):
-        """Numerator gradients (actor, critic) as flat views, for the parity tests."""
+    def grad_views(self, p_id=None):
+        """Numerator gradients (actor, critic) of one policy's learner as flat views, for the parity tests."""
+        e = self._eng[p_id or self.policy_ids[0]]
         a, c = C.c_int64(), C.c_int64()
-        capi.lib().mx_maddpg_grad_views(self.handle, C.byref(a), C.byref(c))
-        return (self.workspace[a.value:a.value + 4 * (self.pol.Pa + 4)].view(torch.float32),
-                self.workspace[c.value:c.value + 4 * (self.pol.Pc + 4)].view(torch.float32))
+        capi.lib().mx_maddpg_grad_views(e.handle, C.byref(a), C.byref(c))
+        return (e.workspace[a.value:a.value + 4 * (e.pol.Pa + 4)].view(torch.float32),
+                e.workspace[c.value:c.value + 4 * (e.pol.Pc + 4)].view(torch.float32))
 
-    def draw_target_noise(self, B):
-        """The draw get_update_info makes through the target policy (maddpg.py:71): (N*B, A) agent-major rows, or None."""
-        pol, N = self.pol, self.cfg.n_agents
+    def draw_target_noise(self, B, p_id=None):
+        """The draw get_update_info makes through policy p_id's target policy (maddpg.py:71): (N_p*B, A_p) agent-major rows, or None."""
+        e = self._eng[p_id or self.policy_ids[0]]
+        pol = e.pol
         if not pol.td3:
             return None
         if pol.discrete:
-            return sample_gumbel((N * B, pol.act_dim))                                             # util.py:178-181
-        return torch.empty(N * B, pol.act_dim).normal_(mean=0, std=float(pol.target_noise))       # util.py:217-218
+            return sample_gumbel((e.n_agents * B, pol.act_dim))                                     # util.py:178-181
+        return torch.empty(e.n_agents * B, pol.act_dim).normal_(mean=0, std=float(pol.target_noise))       # util.py:217-218
 
-    def draw_actor_noise(self, B):
-        """Gumbel draws of the actor update's get_actions(..., use_gumbel=True) (maddpg.py:209): (N*B, A), or None for Box actors."""
-        return sample_gumbel((self.cfg.n_agents * B, self.pol.act_dim)) if self.pol.discrete else None
+    def draw_actor_noise(self, B, p_id=None):
+        """Gumbel draws of policy p_id's actor update, get_actions(..., use_gumbel=True) (maddpg.py:209): (N_p*B, A_p), or None for Box
+        actors."""
+        e = self._eng[p_id or self.policy_ids[0]]
+        return sample_gumbel((e.n_agents * B, e.pol.act_dim)) if e.pol.discrete else None
 
-    def _rows(self, draw, B, step):
+    def _rows(self, draw, B, step, p_id=None):
         """(N*B, A) agent-major draw -> [b][step][n][A] of the learner's transition rows (the other step zero)."""
         if draw is None:
             return None
-        N, A = self.cfg.n_agents, self.pol.act_dim
+        e = self._eng[p_id or self.policy_ids[0]]
+        N, A = e.n_agents, e.pol.act_dim
         ours = torch.zeros(B, 2, N, A)
         ours[:, step] = draw.view(N, B, A).permute(1, 0, 2)
         return ours.to(self.dev, non_blocking=True)
 
-    def _device_batch(self, batch):
+    def _device_batch(self, batch, p_id):
         lib = capi.lib()
+        e = self._eng[p_id]
         if isinstance(batch, MlpSampledBatch):
-            buf = batch.buffers["policy_0"]
-            if buf.rep.sample_serial != batch.serial["policy_0"]:
+            buf = batch.buffers[p_id]
+            if buf.rep.sample_serial != batch.serial[p_id]:
                 raise RuntimeError("stale sample: the buffer has been sampled again since this batch was drawn")
-            capi.check(lib.mx_maddpg_set_valid(self.handle, capi.ptr(buf.valid_dev)))
+            capi.check(lib.mx_maddpg_set_valid(e.handle, capi.ptr(buf.valid_dev)))
             return buf.rep.batch_struct(batch.B)
-        if self._host_batch is None:
-            self._host_batch = _HostTransitions(self.cfg, self.dev)
-        b = self._host_batch.pack(batch, "policy_0", self.use_per)
-        capi.check(lib.mx_maddpg_set_valid(self.handle, capi.ptr(self._host_batch.valid)))
+        if e.host_batch is None:
+            e.host_batch = _HostTransitions(e.cfg, self.dev)
+        b = e.host_batch.pack(batch, p_id, self.use_per)
+        capi.check(lib.mx_maddpg_set_valid(e.handle, capi.ptr(e.host_batch.valid)))
         return b
 
     def train_policy_on_batch(self, update_policy_id, batch):
@@ -174,19 +207,33 @@ class MADDPG(object):
 
     def shared_train_policy_on_batch(self, update_policy_id, batch):
         """maddpg.py:90-249."""
-        if update_policy_id != "policy_0":
-            raise NotImplementedError("B200 MADDPG path: one shared policy 'policy_0'")
-        lib = capi.lib()
-        b = self._device_batch(batch)
-        self._noise_dev = self._rows(self.draw_target_noise(b.B), b.B, 1)
-        self._actor_noise_dev = self._rows(self.draw_actor_noise(b.B), b.B, 0)
+        if update_policy_id not in self._eng:
+            raise KeyError("unknown policy id %r" % (update_policy_id,))
+        lib, stream = capi.lib(), capi.stream_ptr()
+        e = self._eng[update_policy_id]
+        b = self._device_batch(batch, update_policy_id)
+        if self.multi:
+            # maddpg.py:38-81 (get_update_info): every policy's buffer actions and TARGET-actor next actions, policy by policy in id
+            # order -- the target-noise draws (MATD3) consume torch's CPU generator in that same order
+            keep = []
+            for q in self.policy_ids:
+                bq = b if q == update_policy_id else self._device_batch(batch, q)
+                nq = self._rows(self.draw_target_noise(b.B, q), b.B, 1, q)
+                keep.append((bq, nq))
+                if q == update_policy_id:
+                    self._noise_dev = nq
+                capi.check(lib.mx_maddpg_cent_contribute(self._eng[q].handle, C.byref(bq), capi.ptr(nq), e.handle, stream))
+            self._keep = keep
+        else:
+            self._noise_dev = self._rows(self.draw_target_noise(b.B, update_policy_id), b.B, 1, update_policy_id)
+        self._actor_noise_dev = self._rows(self.draw_actor_noise(b.B, update_policy_id), b.B, 0, update_policy_id)
         upd = C.c_int32()
-        capi.check(lib.mx_maddpg_step_ex(self.handle, C.byref(b), capi.ptr(self._noise_dev), capi.ptr(self._actor_noise_dev), C.byref(upd),
-                                         capi.stream_ptr()))
-        info = self._info
+        capi.check(lib.mx_maddpg_step_ex(e.handle, C.byref(b), capi.ptr(self._noise_dev), capi.ptr(self._actor_noise_dev), C.byref(upd),
+                                         stream))
+        info = e.info
         train_info = {"critic_loss": info[0], "critic_grad_norm": info[1], "actor_loss": info[4], "actor_grad_norm": info[5],
                       "update_actor": True}
-        new_priorities = DeviceArray(self._prio[:b.B]) if self.use_per else None
+        new_priorities = DeviceArray(e.prio[:b.B]) if self.use_per else None
         return train_info, new_priorities, batch[12]
 
     def prep_training(self):

@@ -8,11 +8,15 @@ uniform sampling) whose entries materialise the reference's NumPy layout
 on access while the B200 trainers (algorithms/mqmix/mqmix.py, algorithms/maddpg/maddpg.py) read the device-side batch directly.
 `valid_transition` is kept twice: a host array for `materialize`, and a device copy [buffer_size][N] (`valid_dev`) that the MADDPG /
 MATD3 actor loss reads through the batch's sampled indices.
+
+Several policies (`--share_policy` off, one policy per agent): one store per policy with its own observation / action widths, its own
+`valid_dev` and its own PER trees.  A sample draws ONE index set and applies it to every store, as the reference does
+(mlp_buffer.py:100-106 uniform, 285-296 prioritised from the updated policy's tree).
 """
 import numpy as np
 import torch
 
-from offpolicy.utils.rec_buffer import RecPolicyBuffer, _LazyField
+from offpolicy.utils.rec_buffer import RecPolicyBuffer, _LazyField, sample_shared_uniform, share_indices
 
 MLP_FIELDS = ("obs", "share_obs", "acts", "rewards", "next_obs", "next_share_obs", "dones", "dones_env", "valid_transition",
               "avail_acts", "next_avail_acts")
@@ -122,16 +126,17 @@ class MlpReplayBuffer(object):
                  rng="numpy", max_batch=None, _per_alpha=None):
         self.policy_info = policy_info
         self.rng = rng
-        if list(policy_info.keys()) != ["policy_0"]:
-            raise NotImplementedError("B200 replay: only the shared-policy layout ('policy_0') is implemented")
         self.policy_buffers = {
             p_id: MlpPolicyBuffer(buffer_size, len(policy_agents[p_id]), policy_info[p_id]["obs_space"], policy_info[p_id]["share_obs_space"],
                                   policy_info[p_id]["act_space"], use_same_share_obs, use_avail_acts, use_reward_normalization,
                                   use_per=_per_alpha is not None, per_alpha=_per_alpha or 0.0, max_batch=max_batch)
             for p_id in policy_info.keys()}
 
+    def _first(self):
+        return self.policy_buffers["policy_0"] if "policy_0" in self.policy_buffers else next(iter(self.policy_buffers.values()))
+
     def __len__(self):
-        return self.policy_buffers["policy_0"].filled_i
+        return self._first().filled_i              # mlp_buffer.py:44-45: the length of policy_0's store
 
     def insert(self, num_insert_steps, obs, share_obs, acts, rewards, next_obs, next_share_obs, dones, dones_env, valid_transition,
                avail_acts, next_avail_acts):
@@ -151,13 +156,8 @@ class MlpReplayBuffer(object):
             b.rep.seed_device_rng(seed)
 
     def sample(self, batch_size):
-        rep = self.policy_buffers["policy_0"].rep
-        inds = None
-        if self.rng == "device":
-            rep.sample_device_uniform(batch_size)
-        else:
-            inds = np.random.randint(0, self.__len__(), batch_size)                # == np.random.choice(len, B), mlp_buffer.py:100
-            rep.gather(inds)
+        inds = sample_shared_uniform([b.rep for b in self.policy_buffers.values()], self._first().rep, batch_size, self.rng,
+                                     self.__len__())                                  # np.random.choice(len, B), mlp_buffer.py:100
         return MlpSampledBatch(self.policy_buffers, batch_size, list(self.policy_info.keys()), host_inds=inds)
 
 
@@ -173,15 +173,16 @@ class PrioritizedMlpReplayBuffer(MlpReplayBuffer):
     def sample(self, batch_size, beta=0, p_id=None):
         assert len(self) > batch_size, "Not enough samples in the buffer!"                    # mlp_buffer.py:297
         assert beta > 0                                                                        # mlp_buffer.py:298
-        rep = self.policy_buffers[p_id or "policy_0"].rep
+        rep = (self.policy_buffers[p_id] if p_id else self._first()).rep
         if self.rng != "device":
             rep.adopt_numpy_rng()                 # masses come from NumPy's global stream like np.random.random (mlp_buffer.py:287)
             rep.sample_device_per(batch_size, beta)
             rep.export_rng_to_numpy()
         else:
             rep.sample_device_per(batch_size, beta)
+        share_indices([b.rep for b in self.policy_buffers.values()], rep, batch_size)      # p_id's draw selects every store's rows
         return MlpSampledBatch(self.policy_buffers, batch_size, list(self.policy_info.keys()), weights=rep.sampled_weights(batch_size),
                                idxes=rep.sampled_indices(batch_size), per=True)
 
     def update_priorities(self, idxes, priorities, p_id=None):
-        self.policy_buffers[p_id or "policy_0"].rep.update_priorities(idxes, priorities)
+        (self.policy_buffers[p_id] if p_id else self._first()).rep.update_priorities(idxes, priorities)     # p_id's tree only

@@ -428,6 +428,29 @@ class RecPolicyBuffer(object):
         self._keep = (idx_t, pr_t, lv_t)   # keep alive until the stream has consumed them
 
 
+def share_indices(stores, src, batch_size):
+    """Gather into every store but `src` the rows `src` has just drawn on the device: with several policies the reference draws ONE
+    index set and applies it to every policy's store (rec_buffer.py:76-80, 291-299; mlp_buffer.py:100-106, 288-296)."""
+    for other in stores:
+        if other is not src:
+            other.gather_device(src.sampled_indices(batch_size).tensor, batch_size)
+
+
+def sample_shared_uniform(stores, first, batch_size, rng, n):
+    """One uniform index set over [0, n) for every store: drawn on the device by `first` (rng = "device") and gathered into the
+    others, or drawn on the host from NumPy's global stream.  Returns the host indices, or None for a device draw."""
+    if rng == "device":
+        first.sample_device_uniform(batch_size)
+        share_indices(stores, first, batch_size)
+        return None
+    # rec_buffer.py:76 / mlp_buffer.py:100 draw np.random.choice(len, B); randint(0, len, B) is the same call underneath (same
+    # masked-rejection draws from the global MT19937 stream, same int64 result: tests/test_oracle_rng.py) without choice()'s checks
+    inds = np.random.randint(0, n, batch_size)
+    for b in stores:
+        b.gather(inds)
+    return inds
+
+
 class RecReplayBuffer(object):
     """Uniform episode replay (rec_buffer.py:10-82)."""
 
@@ -476,18 +499,7 @@ class RecReplayBuffer(object):
 
     def sample(self, batch_size):
         p_ids = list(self.policy_info.keys())
-        buf = self._first()
-        if self.rng == "device":
-            buf.sample_device_uniform(batch_size)
-            for other in self.policy_buffers.values():      # several policies: ONE index set for every policy's store (rec_buffer.py:76-80)
-                if other is not buf:
-                    other.gather_device(buf.sampled_indices(batch_size).tensor, batch_size)
-        else:
-            # rec_buffer.py:76 draws np.random.choice(len, B); randint(0, len, B) is the same call underneath (same masked-rejection
-            # draws from the global MT19937 stream, same int64 result: tests/test_oracle_rng.py) without choice()'s argument checks
-            inds = np.random.randint(0, self.__len__(), batch_size)
-            for b in self.policy_buffers.values():
-                b.gather(inds)
+        sample_shared_uniform(list(self.policy_buffers.values()), self._first(), batch_size, self.rng, self.__len__())
         return SampledBatch(self.policy_buffers, batch_size, None, None, p_ids)
 
 
@@ -511,9 +523,7 @@ class PrioritizedRecReplayBuffer(RecReplayBuffer):
             buf.export_rng_to_numpy()
         else:
             buf.sample_device_per(batch_size, beta)
-        for other in self.policy_buffers.values():          # the indices drawn from p_id's tree select the episodes of EVERY policy (rec_buffer.py:291-299)
-            if other is not buf:
-                other.gather_device(buf.sampled_indices(batch_size).tensor, batch_size)
+        share_indices(self.policy_buffers.values(), buf, batch_size)      # p_id's draw selects the episodes of EVERY policy (rec_buffer.py:291-299)
         return SampledBatch(self.policy_buffers, batch_size, buf.sampled_weights(batch_size), buf.sampled_indices(batch_size),
                             list(self.policy_info.keys()))
 
