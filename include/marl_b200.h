@@ -30,8 +30,9 @@
 extern "C" {
 #endif
 
-#define MX_ABI_VERSION 4
+#define MX_ABI_VERSION 5
 #define MX_MAX_NAME 64
+#define MX_MAX_ACT_SEG 4       /* mx_maddpg_cfg.act_seg: MultiDiscrete sub-spaces per agent */
 
 typedef struct mx_replay mx_replay;   /* one policy's episode store + sampler (RecPolicyBuffer + PER trees) */
 typedef struct mx_qmix mx_qmix;       /* recurrent QMIX / VDN learner (QMix trainer + QMixPolicy nets + QMixer) */
@@ -285,9 +286,16 @@ typedef struct mx_maddpg_cfg {
    * The actor loss is masked by valid_transition (mx_maddpg_set_valid).  Several policies work as in the recurrent learner
    * (cent_act_dim > 0, mx_maddpg_cent_contribute before every step); mx_maddpg_graph_capture takes one shared policy only. */
   int32_t mlp;
+  /* MultiDiscrete actions (envs/mpe/multi_discrete.py, act.py:15-17: one Linear head per sub-space): the action is n_act_seg one-hot
+   * blocks of act_seg[i] columns, act_dim = their sum.  Arg-max, hard Gumbel-softmax and its straight-through gradient work per block,
+   * and the available-action mask is ignored (MADDPGPolicy.py:73-89) -- also with n_act_seg = 1, which is a MultiDiscrete space of one
+   * sub-space.  0 = one block of act_dim (Box / Discrete, the mask applies).  Segments need discrete and mlp (the recurrent learner
+   * takes none and keeps act_dim <= 8).  The MLP learner takes act_dim <= 32 (Box, Discrete or MultiDiscrete). */
+  int32_t n_act_seg;
+  int32_t act_seg[MX_MAX_ACT_SEG];
 } mx_maddpg_cfg;
 /* which = 0: actor ("rnn.*", "act.action_out.*"), 1: critic ("rnn.*", "q_outs.k.*"); names = reference state_dict keys.
- * cfg.mlp: actor "mlp.*", "act.action_out.*"; critic "mlp.*" (the trained trunk); which = 2: the critic's frozen heads "q_outs.k.*",
+ * cfg.mlp: actor "mlp.*", "act.action_out.*" (with n_act_seg > 0: "act.action_outs.i.*", consecutive row blocks of one head); critic "mlp.*" (the trained trunk); which = 2: the critic's frozen heads "q_outs.k.*",
  * located in the live and in the target critic vector alike. */
 int mx_maddpg_param_layout(const mx_maddpg_cfg* cfg, int32_t which, mx_param_entry* out, int32_t max_entries, int64_t* total_floats);
 int64_t mx_maddpg_workspace_bytes(const mx_maddpg_cfg* cfg);

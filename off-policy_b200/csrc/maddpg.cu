@@ -291,31 +291,57 @@ __global__ void __launch_bounds__(256) k_actor_loss(ActorLossArgs a) {   // ONE 
   }
 }
 
+// The action of one agent as one-hot blocks (MultiDiscrete: one per sub-space, act.py:15-17; Box / Discrete: one block of Ac).
+#define MX_MAX_ACT 32       // widest action the kernels below hold in registers (cfg.mlp; the recurrent learner keeps Ac <= 8)
+struct ActSegs {
+  int n;                    // number of blocks, >= 1
+  int len[MX_MAX_ACT_SEG];  // their widths, summing to Ac
+};
+
 // d(actor action of agent i at (b,t)) = dX[(i,b,t)][S + i*Ac + k]   ->   dense head gradient of the actor [M_a][Ac].
 // Discrete actors (soft != null): the action is the straight-through hard Gumbel-softmax sample, so the gradient reaches the
-// logits through the soft sample y = softmax(logits + g):  dlogit_k = y_k (d_k - sum_j d_j y_j)            (util.py:160-165)
+// logits through the soft sample y = softmax(logits + g) of its block:  dlogit_k = y_k (d_k - sum_{j in block(k)} d_j y_j)   (util.py:160-165)
 // dact rows have dact_ld >= Ac columns, the ones past Ac are zero-filled (cfg.mlp: the actor's "gi" gradient rows, dact_ld = 3H).
 __global__ void __launch_bounds__(256) k_scatter_actor_grad(const float* dX, int ldx, int B, int T, int N, int S, int Ac, const float* soft, float* dact, int off,
-                                                            int dact_ld) {
+                                                            int dact_ld, ActSegs sg) {
   const long long rows = (long long)B * (T + 1) * N;
   for (long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x; m < rows; m += (long long)gridDim.x * blockDim.x) {
     const int n = (int)(m % N);
     const long long bt1 = m / N;
     const int t = (int)(bt1 % (T + 1)), b = (int)(bt1 / (T + 1));
-    float d[8];
-    for (int k = 0; k < Ac; ++k) d[k] = t < T ? dX[(((size_t)n * B + b) * T + t) * ldx + S + off + n * Ac + k] : 0.f;
+    float d[MX_MAX_ACT];      // fully unrolled below: held in registers
+#pragma unroll
+    for (int k = 0; k < MX_MAX_ACT; ++k) d[k] = (k < Ac && t < T) ? dX[(((size_t)n * B + b) * T + t) * ldx + S + off + n * Ac + k] : 0.f;
     if (soft) {
-      float dot = 0.f;
-      for (int k = 0; k < Ac; ++k) dot += d[k] * soft[m * Ac + k];
-      for (int k = 0; k < Ac; ++k) d[k] = soft[m * Ac + k] * (d[k] - dot);
+      float y[MX_MAX_ACT];
+#pragma unroll
+      for (int k = 0; k < MX_MAX_ACT; ++k) y[k] = k < Ac ? soft[m * Ac + k] : 0.f;
+      int k0 = 0;
+#pragma unroll
+      for (int s = 0; s < MX_MAX_ACT_SEG; ++s) {
+        if (s >= sg.n) break;
+        const int k1 = k0 + sg.len[s];
+        float dot = 0.f;
+#pragma unroll
+        for (int k = 0; k < MX_MAX_ACT; ++k)
+          if (k >= k0 && k < k1) dot += d[k] * y[k];
+#pragma unroll
+        for (int k = 0; k < MX_MAX_ACT; ++k)
+          if (k >= k0 && k < k1) d[k] = y[k] * (d[k] - dot);
+        k0 = k1;
+      }
     }
-    for (int k = 0; k < dact_ld; ++k) dact[m * dact_ld + k] = k < Ac ? d[k] : 0.f;
+#pragma unroll
+    for (int k = 0; k < MX_MAX_ACT; ++k)
+      if (k < Ac) dact[m * dact_ld + k] = d[k];
+    for (int k = Ac; k < dact_ld; ++k) dact[m * dact_ld + k] = 0.f;
   }
 }
 
-// Discrete action heads (Ac <= 8, one thread per row).  mode 0: `onehot_from_logits` = every maximal logit is hot
-// (util.py:106-118);  mode 1: hard Gumbel-softmax, value (y_hard - y) + y with y = softmax(logits + g) and y_hard the
-// one-hot of y's maxima (util.py:133-166, temperature 1).  Unavailable actions are forced to -1e10 first (util.py:115, 141).
+// Discrete action heads (Ac <= MX_MAX_ACT, one thread per row), each block of sg on its own.  mode 0: `onehot_from_logits` = every
+// maximal logit of the block is hot (util.py:106-118);  mode 1: hard Gumbel-softmax, value (y_hard - y) + y with y = softmax(logits + g)
+// over the block and y_hard the one-hot of the block's maxima of y (util.py:133-166, temperature 1).  Unavailable actions are forced to
+// -1e10 first (util.py:115, 141); MultiDiscrete heads ignore the mask (MADDPGPolicy.py:73-89), so the caller passes none.
 struct ActXformArgs {
   int M, Ac, mode;
   const float* logits;      // [M][Ac]  (already includes the Gumbel draw when gumbel == null)
@@ -324,30 +350,53 @@ struct ActXformArgs {
   int avail_ld;
   float* out;               // [M][Ac]
   float* soft;              // [M][Ac] soft sample (mode 1) or null
+  ActSegs sg;
 };
 __global__ void __launch_bounds__(256) k_act_transform(ActXformArgs a) {
   for (long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x; m < a.M; m += (long long)gridDim.x * blockDim.x) {
-    float v[8];
-    float mx = -INFINITY;
-    for (int k = 0; k < a.Ac; ++k) {
-      float x = a.logits[m * a.Ac + k];
-      if (a.gumbel) x += a.gumbel[m * a.Ac + k];
-      if (a.avail && a.avail[m * a.avail_ld + k] == 0.f) x = -1e10f;
+    float v[MX_MAX_ACT];      // fully unrolled below: held in registers
+#pragma unroll
+    for (int k = 0; k < MX_MAX_ACT; ++k) {
+      float x = 0.f;
+      if (k < a.Ac) {
+        x = a.logits[m * a.Ac + k];
+        if (a.gumbel) x += a.gumbel[m * a.Ac + k];
+        if (a.avail && a.avail[m * a.avail_ld + k] == 0.f) x = -1e10f;
+      }
       v[k] = x;
-      mx = fmaxf(mx, x);
     }
-    if (a.mode == 0) {
-      for (int k = 0; k < a.Ac; ++k) a.out[m * a.Ac + k] = v[k] == mx ? 1.f : 0.f;
-      continue;
-    }
-    float sum = 0.f;
-    for (int k = 0; k < a.Ac; ++k) { v[k] = expf(v[k] - mx); sum += v[k]; }
-    float ymax = 0.f;
-    for (int k = 0; k < a.Ac; ++k) { v[k] = v[k] / sum; ymax = fmaxf(ymax, v[k]); }
-    for (int k = 0; k < a.Ac; ++k) {
-      const float hard = v[k] == ymax ? 1.f : 0.f;
-      a.out[m * a.Ac + k] = (hard - v[k]) + v[k];
-      if (a.soft) a.soft[m * a.Ac + k] = v[k];
+    int k0 = 0;
+#pragma unroll
+    for (int s = 0; s < MX_MAX_ACT_SEG; ++s) {
+      if (s >= a.sg.n) break;
+      const int k1 = k0 + a.sg.len[s];
+      float mx = -INFINITY;
+#pragma unroll
+      for (int k = 0; k < MX_MAX_ACT; ++k)
+        if (k >= k0 && k < k1) mx = fmaxf(mx, v[k]);
+      if (a.mode == 0) {
+#pragma unroll
+        for (int k = 0; k < MX_MAX_ACT; ++k)
+          if (k >= k0 && k < k1) a.out[m * a.Ac + k] = v[k] == mx ? 1.f : 0.f;
+        k0 = k1;
+        continue;
+      }
+      float sum = 0.f;
+#pragma unroll
+      for (int k = 0; k < MX_MAX_ACT; ++k)
+        if (k >= k0 && k < k1) { v[k] = expf(v[k] - mx); sum += v[k]; }
+      float ymax = 0.f;
+#pragma unroll
+      for (int k = 0; k < MX_MAX_ACT; ++k)
+        if (k >= k0 && k < k1) { v[k] = v[k] / sum; ymax = fmaxf(ymax, v[k]); }
+#pragma unroll
+      for (int k = 0; k < MX_MAX_ACT; ++k)
+        if (k >= k0 && k < k1) {
+          const float hard = v[k] == ymax ? 1.f : 0.f;
+          a.out[m * a.Ac + k] = (hard - v[k]) + v[k];
+          if (a.soft) a.soft[m * a.Ac + k] = v[k];
+        }
+      k0 = k1;
     }
   }
 }
@@ -412,12 +461,47 @@ struct mx_maddpg {
 static inline int mx_imin_host(int a, int b) { return a < b ? a : b; }
 static int cent_act_width(const mx_maddpg_cfg* c) { return c->cent_act_dim > 0 ? c->cent_act_dim : c->n_agents * c->act_dim; }
 static int critic_in_dim(const mx_maddpg_cfg* c) { return c->state_dim + cent_act_width(c); }
+// the one-hot blocks of one agent's action: cfg.act_seg, or one block of act_dim when n_act_seg = 0
+static ActSegs act_segs(const mx_maddpg_cfg* c) {
+  ActSegs sg;
+  memset(&sg, 0, sizeof(sg));
+  if (c->n_act_seg <= 0) { sg.n = 1; sg.len[0] = c->act_dim; return sg; }
+  sg.n = c->n_act_seg;
+  for (int i = 0; i < c->n_act_seg; ++i) sg.len[i] = c->act_seg[i];
+  return sg;
+}
+// k_act_transform arguments for the M actor rows of cfg c.  n_act_seg > 0 is a MultiDiscrete action (one segment included), which takes
+// no available-action mask (MADDPGPolicy.py:73-89); maddpg_check allows it on the MLP learner only
+static ActXformArgs act_xform_args(const mx_maddpg_cfg* c, int M, int mode, const float* avail, int avail_ld) {
+  ActXformArgs ax;
+  memset(&ax, 0, sizeof(ax));
+  ax.M = M; ax.Ac = c->act_dim; ax.mode = mode; ax.sg = act_segs(c);
+  ax.avail = c->n_act_seg > 0 ? nullptr : avail; ax.avail_ld = avail_ld;
+  return ax;
+}
 
 static int maddpg_check(const mx_maddpg_cfg* c) {
   if (!c) { mx_set_error("null cfg"); return 1; }
   if (c->hidden != MX_H) { mx_set_error("hidden_size %d unsupported: kernels are specialised for %d", c->hidden, MX_H); return 1; }
   if (c->n_agents <= 0 || c->obs_dim <= 0 || c->act_dim <= 0 || c->state_dim <= 0 || c->episode_len <= 0 || c->max_batch <= 0) { mx_set_error("mx_maddpg: non-positive dimension"); return 1; }
-  if (c->num_q < 1 || c->num_q > 4 || c->act_dim > 8) { mx_set_error("mx_maddpg: num_q must be 1..4 and act_dim <= 8"); return 1; }
+  if (c->num_q < 1 || c->num_q > 4) { mx_set_error("mx_maddpg: num_q must be 1..4"); return 1; }
+  if (c->act_dim > (c->mlp ? MX_MAX_ACT : 8)) {
+    mx_set_error("mx_maddpg: act_dim %d > %d (the %s learner's limit)", c->act_dim, c->mlp ? MX_MAX_ACT : 8, c->mlp ? "MLP" : "recurrent"); return 1;
+  }
+  if (c->n_act_seg < 0 || c->n_act_seg > MX_MAX_ACT_SEG) { mx_set_error("mx_maddpg: n_act_seg %d outside [0, %d]", c->n_act_seg, MX_MAX_ACT_SEG); return 1; }
+  if (c->n_act_seg > 0) {
+    if (!c->discrete) { mx_set_error("mx_maddpg: action segments (MultiDiscrete) need discrete = 1"); return 1; }
+    if (!c->mlp) {      // n_act_seg > 0 means MultiDiscrete (per-block transforms, no mask): built for the MLP learner only
+      mx_set_error("mx_maddpg: the recurrent learner takes no action segments (n_act_seg = %d); MultiDiscrete is built for the MLP learner only", c->n_act_seg);
+      return 1;
+    }
+    int sum = 0;
+    for (int i = 0; i < c->n_act_seg; ++i) {
+      if (c->act_seg[i] < 1) { mx_set_error("mx_maddpg: action segment %d has width %d < 1", i, c->act_seg[i]); return 1; }
+      sum += c->act_seg[i];
+    }
+    if (sum != c->act_dim) { mx_set_error("mx_maddpg: action segments sum to %d, act_dim is %d", sum, c->act_dim); return 1; }
+  }
   if (c->max_batch * c->episode_len > 65536) { mx_set_error("mx_maddpg: B*T too large"); return 1; }
   if (c->cent_act_dim < 0 || c->act_offset < 0 || (c->cent_act_dim > 0 && c->act_offset + c->n_agents * c->act_dim > c->cent_act_dim)) {
     mx_set_error("mx_maddpg: act_offset %d + n_agents*act_dim %d exceeds cent_act_dim %d", c->act_offset, c->n_agents * c->act_dim, c->cent_act_dim); return 1;
@@ -472,7 +556,17 @@ extern "C" int mx_maddpg_param_layout(const mx_maddpg_cfg* c, int32_t which, mx_
       add("mlp.mlp.fc_h.2.weight", L.lnh_g, H, 0); add("mlp.mlp.fc_h.2.bias", L.lnh_b, H, 0);
       add("mlp.mlp.fc2.0.0.weight", L.w2, H, H); add("mlp.mlp.fc2.0.0.bias", L.b2, H, 0);
       add("mlp.mlp.fc2.0.2.weight", L.ln2_g, H, 0); add("mlp.mlp.fc2.0.2.bias", L.ln2_b, H, 0);
-      if (which == 0) { add("act.action_out.weight", L.wih, c->act_dim, H); add("act.action_out.bias", L.bih, c->act_dim, 0); }
+      if (which == 0 && c->n_act_seg > 0) {      // ACTLayer.action_outs (act.py:15-17): consecutive row blocks of the one head
+        int r = 0;
+        for (int i = 0; i < c->n_act_seg; ++i) {
+          char nm[64];
+          snprintf(nm, sizeof(nm), "act.action_outs.%d.weight", i); add(nm, L.wih + H * r, c->act_seg[i], H);
+          snprintf(nm, sizeof(nm), "act.action_outs.%d.bias", i); add(nm, L.bih + r, c->act_seg[i], 0);
+          r += c->act_seg[i];
+        }
+      } else if (which == 0) {
+        add("act.action_out.weight", L.wih, c->act_dim, H); add("act.action_out.bias", L.bih, c->act_dim, 0);
+      }
     }
     if (total_floats) *total_floats = L.size;
     const int n = (int)v.size();
@@ -662,10 +756,8 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
     MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
   }
   if (c.discrete && !multi) {      // onehot_from_logits with the next-avail mask (MADDPG) / hard Gumbel-softmax, the draw already added (MATD3)
-    ActXformArgs ax;
-    memset(&ax, 0, sizeof(ax));
-    ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
+    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
     MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
   }
 
@@ -722,10 +814,8 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[0], Ma, Ac, (const float*)nullptr, ws + W.a_out, nullptr);
   MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
   if (c.discrete) {    // get_actions(obs, avail, use_gumbel=True): hard Gumbel-softmax, straight-through (maddpg.py:209)
-    ActXformArgs ax;
-    memset(&ax, 0, sizeof(ax));
-    ax.M = Ma; ax.Ac = Ac; ax.mode = 1; ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
-    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    ActXformArgs ax = act_xform_args(&c, Ma, 1, b->avail, b->act_ld);
+    ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
     MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
   }
   pk.mode = 2; pk.x = ws + W.r_x; pk.actor_out = ws + (c.discrete ? W.a_act : W.a_out);
@@ -754,7 +844,7 @@ static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_
   int dummy = 0;
   if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
   MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, 1, N, S, Ac,
-            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, c.act_offset, (int)MX_G);
+            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, c.act_offset, (int)MX_G, act_segs(&c));
   MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
   FrontBwdArgs fba;
   memset(&fba, 0, sizeof(fba));
@@ -828,10 +918,8 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   ha.theta = h->th_a_tgt; ha.h = gf.hall[1]; ha.sto = nullptr; ha.out = ws + W.a_nact; ha.noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
   MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
   if (c.discrete) {      // target actions: arg-max one-hot (MADDPG) / hard Gumbel-softmax sample (MATD3; the head added the draw)
-    ActXformArgs ax;
-    memset(&ax, 0, sizeof(ax));
-    ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
+    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
     MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
   }
 
@@ -925,10 +1013,8 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     g2.gates = ws + W.c_gates; g2.hn = ws + W.c_hn;
     if (mx_launch_gru_fwd(g2, 1, s)) return 1;
     if (c.discrete) {    // the live actor's hard Gumbel-softmax sample (straight-through), r_maddpg.py:277
-      ActXformArgs ax;
-      memset(&ax, 0, sizeof(ax));
-      ax.M = Ma; ax.Ac = Ac; ax.mode = 1; ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
-      ax.avail = b->avail; ax.avail_ld = b->act_ld;
+      ActXformArgs ax = act_xform_args(&c, Ma, 1, b->avail, b->act_ld);
+      ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
       MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
     }
     pk.mode = 2; pk.x = ws + W.r_x; pk.actor_out = ws + (c.discrete ? W.a_act : W.a_out); pk.hseq = g2.hall[0]; pk.h0 = ws + W.r_h0;
@@ -968,7 +1054,7 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
     int dummy = 0;
     if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
     MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, T, N, S, Ac,
-              (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dout, multi ? c.act_offset : 0, Ac);
+              (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dout, multi ? c.act_offset : 0, Ac, act_segs(&c));
     MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
     // actor backward + Adam
     const int ahead_grid = mx_imin_host(mx_num_sms(), mx_ceil_div(Ma, 32));
@@ -1061,10 +1147,8 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
     MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
   }
   if (c.discrete) {      // one-hot with the next-avail mask (MADDPG) / hard Gumbel-softmax (MATD3)
-    ActXformArgs ax;
-    memset(&ax, 0, sizeof(ax));
-    ax.M = Ma; ax.Ac = Ac; ax.mode = c.target_noise > 0.f ? 1 : 0; ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    ax.avail = b->avail; ax.avail_ld = b->act_ld;
+    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
+    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
     MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
   }
   MX_LAUNCH(k_cent_scatter, dim3(launch1d((long long)B * T * N * Ac)), dim3(256), 0, s, (const float*)(ws + W.a_nact), b->acts, b->act_ld, B, T, N, Ac,

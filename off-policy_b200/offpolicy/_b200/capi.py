@@ -37,7 +37,7 @@ class Episodes(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("obs", "share_obs", "acts", "rewards", "dones", "dones_env", "avail")]
 
 
-ABI_VERSION = 4        # MX_ABI_VERSION of include/marl_b200.h the struct mirrors below correspond to
+ABI_VERSION = 5        # MX_ABI_VERSION of include/marl_b200.h the struct mirrors below correspond to
 
 
 class QmixCfg(C.Structure):
@@ -48,13 +48,16 @@ class QmixCfg(C.Structure):
                                           "max_grad_norm", "tau")] + [("prev_act_inp", C.c_int32), ("mlp", C.c_int32), ("no_feature_norm", C.c_int32), ("use_tanh", C.c_int32)])
 
 
+MAX_ACT_SEG = 4        # MX_MAX_ACT_SEG: MultiDiscrete sub-spaces per agent (mx_maddpg_cfg.act_seg)
+
+
 class MaddpgCfg(C.Structure):
     _fields_ = ([(n, C.c_int32) for n in ("n_agents", "obs_dim", "act_dim", "state_dim", "hidden", "episode_len", "max_batch", "num_q",
                                           "actor_update_interval", "use_huber", "use_per")] +
                 [(n, C.c_float) for n in ("gamma", "huber_delta", "per_nu", "per_eps", "lr", "adam_beta1", "adam_beta2", "adam_eps",
                                           "max_grad_norm", "tau", "weight_decay", "target_noise")] +
                 [("discrete", C.c_int32), ("no_feature_norm", C.c_int32), ("use_tanh", C.c_int32), ("cent_act_dim", C.c_int32), ("act_offset", C.c_int32),
-                 ("mlp", C.c_int32)])
+                 ("mlp", C.c_int32), ("n_act_seg", C.c_int32), ("act_seg", C.c_int32 * MAX_ACT_SEG)])
 
 
 class ParamEntry(C.Structure):

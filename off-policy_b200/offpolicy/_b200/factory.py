@@ -81,6 +81,26 @@ class Discrete(object):  # duck-typed gym.spaces.Discrete
         self.n = n
 
 
+class MultiDiscrete(object):     # duck-typed envs/mpe/multi_discrete.py: the policies read the class name and .low / .high
+    def __init__(self, array_of_param_array):
+        self.low = np.array([x[0] for x in array_of_param_array])
+        self.high = np.array([x[1] for x in array_of_param_array])
+        self.num_discrete_space = self.low.shape[0]
+
+
+def act_space(act, discrete=True):
+    """The action space for a width: an int -> Discrete(n) (Box(n) with discrete False); a list / tuple of sub-space widths ->
+    MultiDiscrete([[0, n_0 - 1], [0, n_1 - 1], ...])."""
+    if isinstance(act, (list, tuple, np.ndarray)):
+        return MultiDiscrete([[0, int(n) - 1] for n in act])
+    return Discrete(act) if discrete else Box(act)
+
+
+def act_width(act):
+    """Width of the action vector of an action description of act_space (the sum of the sub-space widths for MultiDiscrete)."""
+    return int(np.sum(act)) if isinstance(act, (list, tuple, np.ndarray)) else int(act)
+
+
 def pd(x, p_id="policy_0"):
     """{policy_id: array}: the per-policy dict every buffer / trainer entry point of the reference takes."""
     return {p_id: x}
@@ -193,12 +213,13 @@ def mlp_maddpg_args(B, **over):
 
 
 def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td3=False, **over):
-    """(args, policy, trainer) for the transition-level MADDPG (td3 False) / MATD3 (True), one shared policy; `over` sets args fields."""
+    """(args, policy, trainer) for the transition-level MADDPG (td3 False) / MATD3 (True), one shared policy; `over` sets args fields.
+    act_dim: an int, or a list of sub-space widths for a MultiDiscrete action space (act_space)."""
     from offpolicy._b200 import capi
     Policy, Trainer = _mlp_maddpg_classes(td3)
     args = mlp_maddpg_args(B, **over)
     info = dict(obs_space=Box(obs_dim, -np.inf, np.inf), share_obs_space=Box(state_dim, -np.inf, np.inf),
-                act_space=Discrete(act_dim) if discrete else Box(act_dim), cent_obs_dim=state_dim, cent_act_dim=act_dim * n_agents)
+                act_space=act_space(act_dim, discrete), cent_obs_dim=state_dim, cent_act_dim=act_width(act_dim) * n_agents)
     pol = Policy({"args": args, "device": capi.device()}, info)
     tr = Trainer(args, n_agents, {"policy_0": pol}, lambda a: "policy_0", device=capi.device())
     return args, pol, tr
@@ -206,18 +227,19 @@ def build_mlp_maddpg(n_agents, obs_dim, act_dim, state_dim, B, discrete=True, td
 
 def build_mlp_maddpg_multi(specs, state_dim, B, discrete=True, td3=False, **over):
     """(args, {policy_id: policy}, trainer, agents) for the transition-level MADDPG / MATD3 with several policies (share_policy off).
-    specs: one (obs_dim, act_dim) or (obs_dim, act_dim, n_agents) per policy; policy_i controls the next n_agents agents (1 by default),
+    specs: one (obs_dim, act_dim) or (obs_dim, act_dim, n_agents) per policy, act_dim as in act_space (a list of sub-space widths gives a
+    MultiDiscrete policy, whatever `discrete` says); policy_i controls the next n_agents agents (1 by default),
     agents = {policy_id: [agent ids]}.  The policies are constructed in id order, as train_mpe.py:139-150 does."""
     from offpolicy._b200 import capi
     Policy, Trainer = _mlp_maddpg_classes(td3)
     args = mlp_maddpg_args(B, **over)
     specs = [tuple(s) + (1,) * (3 - len(s)) for s in specs]
-    total = sum(a * n for _, a, n in specs)
+    total = sum(act_width(a) * n for _, a, n in specs)
     pols, agents, mapping, nxt = {}, {}, {}, 0
     for i, (o, a, n) in enumerate(specs):
         p = "policy_%d" % i
         info = dict(obs_space=Box(o, -np.inf, np.inf), share_obs_space=Box(state_dim, -np.inf, np.inf),
-                    act_space=Discrete(a) if discrete else Box(a), cent_obs_dim=state_dim, cent_act_dim=total)
+                    act_space=act_space(a, discrete), cent_obs_dim=state_dim, cent_act_dim=total)
         pols[p] = Policy({"args": args, "device": capi.device()}, info)
         agents[p] = list(range(nxt, nxt + n))
         mapping.update({k: p for k in agents[p]})

@@ -15,7 +15,11 @@ spaces) get one learner each.  Every critic sees the actions of all agents: `cen
 agents sit at `act_offset`, in sorted policy-id order (maddpg.py:55-79).  Before a policy's step, every policy q writes its buffer
 actions and its target actor's next actions into the updated policy's centralised action vectors (`mx_maddpg_cent_contribute`), q by q
 in id order, which is also the order of the reference's target-noise draws.  Only the shared-observation form is built:
-`cent_train_policy_on_batch` and `--use_popart` raise."""
+`cent_train_policy_on_batch` and `--use_popart` raise.
+
+MultiDiscrete policies (`act_dim` an ndarray of sub-space widths) occupy `output_dim` columns of every action vector; the learner gets
+the sub-space widths (cfg.act_seg) and transforms each one-hot block on its own.  Their Gumbel draws are one `sample_gumbel` call per
+sub-space, in sub-space order, as the reference's per-block `gumbel_softmax` calls make them (MADDPGPolicy.py:73-89)."""
 import ctypes as C
 
 import numpy as np
@@ -27,6 +31,14 @@ from offpolicy.utils.mlp_buffer import MlpSampledBatch
 from offpolicy.utils.rec_buffer import DeviceArray
 
 
+def _gumbel_blocks(rows, pol):
+    """Gumbel(0, 1) draws for `rows` actor rows of a Discrete policy: one sample_gumbel call per MultiDiscrete sub-space, in order (the
+    reference's per-block gumbel_softmax calls), or one call over the whole action."""
+    if pol.act_segs is None:
+        return sample_gumbel((rows, pol.act_dim))
+    return torch.cat([sample_gumbel((rows, n)) for n in pol.act_segs], -1)
+
+
 class _HostTransitions(object):
     """Device copy of a batch handed over in the reference's NumPy layout (mlp_buffer.py:203-240): compatibility path."""
 
@@ -34,7 +46,7 @@ class _HostTransitions(object):
         B, N = cfg.max_batch, cfg.n_agents
         r4 = lambda v: (v + 3) // 4 * 4
         self.cfg, self.dev = cfg, dev
-        self.obs_ld, self.share_ld, self.act_ld = r4(cfg.obs_dim), r4(cfg.state_dim), r4(cfg.act_dim)
+        self.obs_ld, self.share_ld, self.act_ld = r4(cfg.obs_dim), r4(cfg.state_dim), r4(cfg.act_dim)      # cfg.act_dim = output_dim
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.obs, self.share, self.acts, self.avail = z(B, 2, N, self.obs_ld), z(B, 2, self.share_ld), z(B, 1, N, self.act_ld), z(B, 2, N, self.act_ld)
         self.rew, self.dones, self.dones_env, self.weights, self.valid = z(B, 1, N), z(B, 1, N), z(B, 1), z(B), z(B, N)
@@ -82,8 +94,8 @@ class _Engine(object):
         # cfg.target_noise > 0 tells the learner that target-action noise is passed.  MATD3 always smooths (MADDPGPolicy.py:93, 111 test
         # `target_noise is not None`): a Discrete actor takes Gumbel draws whatever the std, a Box actor N(0, std) draws, all-zero at std 0
         tnoise = (1.0 if pol.discrete else float(pol.target_noise)) if pol.td3 else 0.0
-        self.cfg = maddpg_cfg_struct(args, n_agents, pol.obs_dim, pol.act_dim, pol.central_obs_dim, 1, max_batch, pol.td3, tnoise, 1,
-                                     pol.discrete, cent_act_dim=cent_act_dim, act_offset=act_offset, mlp=True)
+        self.cfg = maddpg_cfg_struct(args, n_agents, pol.obs_dim, pol.output_dim, pol.central_obs_dim, 1, max_batch, pol.td3, tnoise, 1,
+                                     pol.discrete, cent_act_dim=cent_act_dim, act_offset=act_offset, mlp=True, act_segs=pol.act_segs)
         nbytes = int(lib.mx_maddpg_workspace_bytes(C.byref(self.cfg)))
         if nbytes < 0:
             raise capi.MxError(lib.mx_last_error().decode())
@@ -122,18 +134,18 @@ class MADDPG(object):
         self.max_batch = int(getattr(args, "batch_size", 32))
         self.dev = capi.device()
         self.multi = len(self.policy_ids) > 1
-        total = sum(len(self.policy_agents[p]) * self.policies[p].act_dim for p in self.policy_ids)
+        total = sum(len(self.policy_agents[p]) * self.policies[p].output_dim for p in self.policy_ids)
         self._eng = {}
         off = 0
         for p in self.policy_ids:                    # the centralised action vector: sorted ids, each policy's agents in order
             pol, n_p = self.policies[p], len(self.policy_agents[p])
             if self.multi and pol.central_act_dim != total:
                 raise ValueError("policy %s: cent_act_dim %d != total action width %d of all agents" % (p, pol.central_act_dim, total))
-            if not self.multi and pol.central_act_dim != n_p * pol.act_dim:
-                raise NotImplementedError("B200 MADDPG path: cent_act_dim %d != n_agents * act_dim %d" % (pol.central_act_dim, n_p * pol.act_dim))
+            if not self.multi and pol.central_act_dim != n_p * pol.output_dim:
+                raise NotImplementedError("B200 MADDPG path: cent_act_dim %d != n_agents * output_dim %d" % (pol.central_act_dim, n_p * pol.output_dim))
             self._eng[p] = _Engine(args, pol, n_p, self.max_batch, total if self.multi else 0, off if self.multi else 0)
             pol._trainer, pol._handle = self, self._eng[p].handle
-            off += n_p * pol.act_dim
+            off += n_p * pol.output_dim
         first = self._eng[self.policy_ids[0]]
         # the first policy's learner under the single-policy names (graph helpers, tests)
         self.pol, self.cfg, self.workspace, self.handle, self._info, self._prio = first.pol, first.cfg, first.workspace, first.handle, first.info, first.prio
@@ -163,21 +175,21 @@ class MADDPG(object):
         if not pol.td3:
             return None
         if pol.discrete:
-            return sample_gumbel((e.n_agents * B, pol.act_dim))                                     # util.py:178-181
+            return _gumbel_blocks(e.n_agents * B, pol)                                              # util.py:178-181
         return torch.empty(e.n_agents * B, pol.act_dim).normal_(mean=0, std=float(pol.target_noise))       # util.py:217-218
 
     def draw_actor_noise(self, B, p_id=None):
         """Gumbel draws of policy p_id's actor update, get_actions(..., use_gumbel=True) (maddpg.py:209): (N_p*B, A_p), or None for Box
         actors."""
         e = self._eng[p_id or self.policy_ids[0]]
-        return sample_gumbel((e.n_agents * B, e.pol.act_dim)) if e.pol.discrete else None
+        return _gumbel_blocks(e.n_agents * B, e.pol) if e.pol.discrete else None
 
     def _rows(self, draw, B, step, p_id=None):
         """(N*B, A) agent-major draw -> [b][step][n][A] of the learner's transition rows (the other step zero)."""
         if draw is None:
             return None
         e = self._eng[p_id or self.policy_ids[0]]
-        N, A = e.n_agents, e.pol.act_dim
+        N, A = e.n_agents, e.pol.output_dim
         ours = torch.zeros(B, 2, N, A)
         ours[:, step] = draw.view(N, B, A).permute(1, 0, 2)
         return ours.to(self.dev, non_blocking=True)

@@ -39,7 +39,11 @@ def gumbel_softmax_hard(logits, avail=None):
 
 
 def maddpg_cfg_struct(args, n_agents, obs_dim, act_dim, state_dim, episode_len, max_batch, td3, target_noise, actor_update_interval,
-                      discrete=False, cent_act_dim=0, act_offset=0, mlp=False):
+                      discrete=False, cent_act_dim=0, act_offset=0, mlp=False, act_segs=None):
+    """act_segs: the MultiDiscrete sub-space widths (summing to act_dim), or None for one block (Box / Discrete)."""
+    segs = [int(n) for n in act_segs] if act_segs is not None else []
+    if len(segs) > capi.MAX_ACT_SEG:
+        raise NotImplementedError("B200 MADDPG path: at most %d MultiDiscrete sub-spaces, got %d" % (capi.MAX_ACT_SEG, len(segs)))
     return capi.MaddpgCfg(n_agents=n_agents, obs_dim=obs_dim, act_dim=act_dim, state_dim=state_dim, hidden=args.hidden_size,
                           episode_len=episode_len, max_batch=max_batch, num_q=2 if td3 else 1, actor_update_interval=actor_update_interval,
                           use_huber=int(args.use_huber_loss), use_per=int(args.use_per), gamma=args.gamma, huber_delta=args.huber_delta,
@@ -47,7 +51,8 @@ def maddpg_cfg_struct(args, n_agents, obs_dim, act_dim, state_dim, episode_len, 
                           max_grad_norm=args.max_grad_norm, tau=args.tau, weight_decay=float(getattr(args, "weight_decay", 0) or 0),
                           target_noise=float(target_noise or 0.0), discrete=int(bool(discrete)),
                           no_feature_norm=0 if getattr(args, "use_feature_normalization", True) else 1,
-                          use_tanh=0 if getattr(args, "use_ReLU", True) else 1, cent_act_dim=int(cent_act_dim), act_offset=int(act_offset), mlp=int(bool(mlp)))
+                          use_tanh=0 if getattr(args, "use_ReLU", True) else 1, cent_act_dim=int(cent_act_dim), act_offset=int(act_offset), mlp=int(bool(mlp)),
+                          n_act_seg=len(segs), act_seg=(C.c_int32 * capi.MAX_ACT_SEG)(*segs))
 
 
 def maddpg_entries(cfg, which):
