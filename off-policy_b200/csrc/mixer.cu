@@ -12,17 +12,20 @@
 #include "mx_kernels.h"
 #include "mx_tile.cuh"
 
+#include <string.h>
+
 struct MixSmem {
   int ldS, ldH, ldP, ldM, ldw;
   int o_s, o_h1, o_h2, o_hb, o_p1, o_b1, o_p2, o_hid, o_q, o_vec, o_wc, total;
 };
-static MixSmem mix_smem_layout(const MxMixLayout& L, int TE) {
+// wide: no state tile (the wide-state path reads the state layers' pre-activations instead)
+static MixSmem mix_smem_layout(const MxMixLayout& L, int TE, bool wide = false) {
   MixSmem m;
-  const int S64 = mx_round_up(L.S, 64), H64 = mx_round_up(L.HY, 64), P64 = mx_round_up(L.N * L.ME, 64), M64 = mx_round_up(L.ME, 64);
+  const int S64 = wide ? 0 : mx_round_up(L.S, 64), H64 = mx_round_up(L.HY, 64), P64 = mx_round_up(L.N * L.ME, 64), M64 = mx_round_up(L.ME, 64);
   m.ldS = mx_ld(S64); m.ldH = mx_ld(H64); m.ldP = mx_ld(P64); m.ldM = mx_ld(M64);
   m.ldw = mx_ld(S64 > H64 ? S64 : H64);
   int o = 0;
-  m.o_s = o; o += TE * m.ldS;
+  m.o_s = o; o += wide ? 0 : TE * m.ldS;
   m.o_h1 = o; o += TE * m.ldH;
   m.o_h2 = o; o += TE * m.ldH;
   m.o_hb = o; o += TE * m.ldH;
@@ -35,6 +38,21 @@ static MixSmem mix_smem_layout(const MxMixLayout& L, int TE) {
   m.o_wc = o; o += 64 * m.ldw;
   m.total = o;
   return m;
+}
+
+bool mx_mix_wide_state(const MxMixLayout& L) { return (size_t)mix_smem_layout(L, 32).total * sizeof(float) + 16 > 227 * 1024; }
+
+void mx_mix_wide_layout(const MxMixLayout& L, MxMixWide* w) {
+  memset(w, 0, sizeof(*w));
+  const int NM = L.N * L.ME;
+  const int rows[4] = {L.layers == 2 ? L.HY : NM, L.layers == 2 ? L.HY : L.ME, L.HY, L.ME};
+  const int wo[4] = {L.layers == 2 ? L.w1a : L.w1b, L.layers == 2 ? L.w2a : L.w2b, L.wb2a, L.wb1};
+  const int bo[4] = {L.layers == 2 ? L.b1a : L.b1b, L.layers == 2 ? L.b2a : L.b2b, L.bb2a, L.bb1};
+  int c = 0;
+  for (int j = 0; j < 4; ++j) { w->col[j] = c; w->rows[j] = rows[j]; w->w[j] = wo[j]; w->b[j] = bo[j]; c += mx_round_up(rows[j], 4); }
+  w->C = c;
+  w->Cp = mx_round_up(c, 16);
+  w->Sp = mx_round_up(L.S, 32);
 }
 
 // Y_s[r][c] = act(sum_k X_s[r][k] W[c][k] + b[c]) for c < Nout (columns up to round_up(Nout,64) are written, zeros beyond)
@@ -420,8 +438,34 @@ MX_DEVINL void mix_tile_load(float* dst_s, int lds, int width, const float* __re
   }
 }
 
+// wide-state path: block `blk` of net `net`'s state-layer pre-activations for the tile's elements (state row b (T+1) + t + net),
+// ReLU applied when `relu`, zero-filled out to `width` columns
+MX_DEVINL void mix_pre_load(float* dst_s, int lds, int width, const MixerArgs& a, int net, int blk, bool relu, int e0, int E, int TE) {
+  const float* pre = a.pre + (size_t)net * a.B * (a.T + 1) * a.wl.Cp + a.wl.col[blk];
+  const int nc4 = width >> 2, g4 = mx_round_up(a.wl.rows[blk], 4) >> 2;
+  for (int idx = threadIdx.x; idx < TE * nc4; idx += MX_TILE_THREADS) {
+    const int r = idx / nc4, c4 = idx - r * nc4, e = e0 + r;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (e < E && c4 < g4) {
+      const int b = e / a.T, t = e - b * a.T;
+      v = mx_ld4(pre + ((size_t)b * (a.T + 1) + t + net) * a.wl.Cp + 4 * c4);
+      if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+    }
+    mx_st4(dst_s + r * lds + 4 * c4, v);
+  }
+}
+// wide-state path: the tile's gradient at block `blk`'s pre-activations -> d_pre rows e0..
+MX_DEVINL void mix_dpre_store(const float* src_s, int lds, const MixerArgs& a, int blk, int e0, int E, int TE) {
+  const int nc4 = mx_round_up(a.wl.rows[blk], 4) >> 2;
+  for (int idx = threadIdx.x; idx < TE * nc4; idx += MX_TILE_THREADS) {
+    const int r = idx / nc4, c4 = idx - r * nc4;
+    if (e0 + r < E) mx_st4(a.d_pre + (size_t)(e0 + r) * a.wl.Cp + a.wl.col[blk] + 4 * c4, mx_ld4(src_s + r * lds + 4 * c4));
+  }
+}
+
 // blockIdx.y = 0: live net on s[t]; 1: target net on s[t+1] (qmix.py:155-157)
-template <int RM>
+// WIDE: the state-reading layers come from the state-layer GEMM (mixer_wide.cu); only the second layers run here
+template <int RM, bool WIDE>
 __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_fwd(MixerArgs a, MixSmem sm) {
   constexpr int TE = 16 * RM;
   MX_DYN_SMEM(smem);
@@ -437,11 +481,30 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_fwd(MixerArgs a, 
   MX_PDL_WAIT();
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int e0 = tile * TE;
-    mix_stage_states(a, sm, s_s, e0, E, TE, S64, net);
-    mx_cp_commit();
-    mx_cp_wait<0>();
-    __syncthreads();
-    mixer_hyper<RM>(th, L, sm, smem);
+    if constexpr (WIDE) {
+      const int H64 = mx_round_up(L.HY, 64), P64 = mx_round_up(L.N * L.ME, 64), M64 = mx_round_up(L.ME, 64);
+      if (L.layers == 2) {
+        mix_pre_load(h1_s, sm.ldH, H64, a, net, 0, true, e0, E, TE);
+        mix_pre_load(h2_s, sm.ldH, H64, a, net, 1, true, e0, E, TE);
+      } else {
+        mix_pre_load(p1_s, sm.ldP, P64, a, net, 0, false, e0, E, TE);
+        mix_pre_load(p2_s, sm.ldM, M64, a, net, 1, false, e0, E, TE);
+      }
+      mix_pre_load(hb_s, sm.ldH, H64, a, net, 2, true, e0, E, TE);
+      mix_pre_load(b1_s, sm.ldM, M64, a, net, 3, false, e0, E, TE);
+      __syncthreads();
+      if (L.layers == 2) {
+        float* Wc = smem + sm.o_wc;
+        tile_linear<RM>(h1_s, sm.ldH, L.HY, th + L.w1b, th + L.b1b, L.N * L.ME, p1_s, sm.ldP, false, Wc, sm.ldw);
+        tile_linear<RM>(h2_s, sm.ldH, L.HY, th + L.w2b, th + L.b2b, L.ME, p2_s, sm.ldM, false, Wc, sm.ldw);
+      }
+    } else {
+      mix_stage_states(a, sm, s_s, e0, E, TE, S64, net);
+      mx_cp_commit();
+      mx_cp_wait<0>();
+      __syncthreads();
+      mixer_hyper<RM>(th, L, sm, smem);
+    }
     // b2 = hb . Wb2b + bb2b   (one half-warp per element)
     {
       const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -562,7 +625,8 @@ __global__ void __launch_bounds__(512) k_mix_core(MixerArgs a) {
 }
 
 // parameter gradients of the live hypernetworks from core's d p1 / d p2 / d hid_pre / dQ (per-CTA partials like k_mixer)
-template <int RM>
+// WIDE: the state layers' weight gradients are left to the state-layer GEMM; this kernel writes the gradient at their pre-activations
+template <int RM, bool WIDE>
 __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_bwd(MixerArgs a, MixSmem sm) {
   constexpr int TE = 16 * RM;
   MX_DYN_SMEM(smem);
@@ -583,7 +647,7 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_bwd(MixerArgs a, 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++iter) {
     const int e0 = tile * TE;
     const bool accum = iter > 0;
-    mix_stage_states(a, sm, s_s, e0, E, TE, S64, 0);
+    if constexpr (!WIDE) mix_stage_states(a, sm, s_s, e0, E, TE, S64, 0);
     if (L.layers == 2) {
       mix_tile_load(h1_s, sm.ldH, H64, a.hyp_h1, a.gH, e0, E, TE);
       mix_tile_load(h2_s, sm.ldH, H64, a.hyp_h2, a.gH, e0, E, TE);
@@ -617,6 +681,25 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_bwd(MixerArgs a, 
       hb_s[idx] = v;
     }
     __syncthreads();
+    if constexpr (WIDE) {
+      mix_dpre_store(hb_s, sm.ldH, a, 2, e0, E, TE);
+      mix_dpre_store(hid_s, sm.ldM, a, 3, e0, E, TE);
+      if (L.layers == 2) {
+        tile_wgrad(p2_s, sm.ldM, L.ME, h2_s, sm.ldH, L.HY, TE, gp + L.w2b, gp + L.b2b, accum);
+        __syncthreads();
+        tile_dgrad_relu<RM>(p2_s, sm.ldM, L.ME, a.theta + L.w2b, L.HY, h2_s, h2_s, sm.ldH, Wc, sm.ldw);
+        mix_dpre_store(h2_s, sm.ldH, a, 1, e0, E, TE);
+        tile_wgrad(p1_s, sm.ldP, NM, h1_s, sm.ldH, L.HY, TE, gp + L.w1b, gp + L.b1b, accum);
+        __syncthreads();
+        tile_dgrad_relu<RM>(p1_s, sm.ldP, NM, a.theta + L.w1b, L.HY, h1_s, h1_s, sm.ldH, Wc, sm.ldw);
+        mix_dpre_store(h1_s, sm.ldH, a, 0, e0, E, TE);
+      } else {
+        mix_dpre_store(p2_s, sm.ldM, a, 1, e0, E, TE);
+        mix_dpre_store(p1_s, sm.ldP, a, 0, e0, E, TE);
+      }
+      __syncthreads();
+      continue;
+    }
     // -- hyper_b2 first layer, hyper_b1
     tile_wgrad(hb_s, sm.ldH, L.HY, s_s, sm.ldS, L.S, TE, gp + L.wb2a, gp + L.bb2a, accum);
     tile_wgrad(hid_s, sm.ldM, L.ME, s_s, sm.ldS, L.S, TE, gp + L.wb1, gp + L.bb1, accum);
@@ -694,13 +777,22 @@ static int mix_smem_attr(K kern, size_t smem, size_t* conf) {
 int mx_launch_mix_hyper_fwd(const MixerArgs& a, cudaStream_t s) {
   const int E = a.B * a.T;
   const int RM = mix_split_rm(E), TE = 16 * RM;
-  MixSmem sm = mix_smem_layout(a.L, TE);
+  MixSmem sm = mix_smem_layout(a.L, TE, a.wide != 0);
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   int grid = mx_ceil_div(E, TE);
   if (grid > mx_num_sms()) grid = mx_num_sms();
+  if (a.wide) {
+    if (mx_launch_mixw_state_fwd(a, s)) return 1;
+    static size_t w1 = 0, w2 = 0;
+    if (RM == 1) { if (mix_smem_attr(k_mix_hyper_fwd<1, true>, smem, &w1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<1, true>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+    else { if (mix_smem_attr(k_mix_hyper_fwd<2, true>, smem, &w2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<2, true>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+    MX_COUNT();
+    MX_MARK("k_mix_hyper_fwd_wide", s);
+    return MX_CHECK_LAUNCH("mix_hyper_fwd_wide");
+  }
   static size_t c1 = 0, c2 = 0;
-  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_fwd<1>, smem, &c1)) return 1; MX_LAUNCH_PDL(k_mix_hyper_fwd<1>, dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  else { if (mix_smem_attr(k_mix_hyper_fwd<2>, smem, &c2)) return 1; MX_LAUNCH_PDL(k_mix_hyper_fwd<2>, dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_fwd<1, false>, smem, &c1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<1, false>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+  else { if (mix_smem_attr(k_mix_hyper_fwd<2, false>, smem, &c2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<2, false>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
   MX_COUNT();
   MX_MARK("k_mix_hyper_fwd", s);
   return MX_CHECK_LAUNCH("mix_hyper_fwd");
@@ -720,13 +812,23 @@ int mx_launch_mix_core(const MixerArgs& a, int* scalar_parts_used, cudaStream_t 
 int mx_launch_mix_hyper_bwd(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
   const int E = a.B * a.T;
   const int RM = mix_split_rm(E), TE = 16 * RM;
-  MixSmem sm = mix_smem_layout(a.L, TE);
+  MixSmem sm = mix_smem_layout(a.L, TE, a.wide != 0);
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   int grid = mx_ceil_div(E, TE);
   if (grid > mx_num_sms()) grid = mx_num_sms();
+  if (a.wide) {
+    static size_t w1 = 0, w2 = 0;
+    if (RM == 1) { if (mix_smem_attr(k_mix_hyper_bwd<1, true>, smem, &w1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<1, true>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+    else { if (mix_smem_attr(k_mix_hyper_bwd<2, true>, smem, &w2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<2, true>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+    MX_COUNT();
+    MX_MARK("k_mix_hyper_bwd_wide", s);
+    *nparts_used = grid;
+    if (MX_CHECK_LAUNCH("mix_hyper_bwd_wide")) return 1;
+    return mx_launch_mixw_state_wgrad(a, s);
+  }
   static size_t c1 = 0, c2 = 0;
-  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_bwd<1>, smem, &c1)) return 1; MX_LAUNCH_PDL(k_mix_hyper_bwd<1>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  else { if (mix_smem_attr(k_mix_hyper_bwd<2>, smem, &c2)) return 1; MX_LAUNCH_PDL(k_mix_hyper_bwd<2>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_bwd<1, false>, smem, &c1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<1, false>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
+  else { if (mix_smem_attr(k_mix_hyper_bwd<2, false>, smem, &c2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<2, false>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
   MX_COUNT();
   MX_MARK("k_mix_hyper_bwd", s);
   *nparts_used = grid;

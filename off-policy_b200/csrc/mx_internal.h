@@ -81,6 +81,16 @@ struct MxMixLayout {
 };
 int mx_net_layout(int in_dim, int out_dim, int base, MxNetLayout* L);
 int mx_mix_layout(int S, int N, int ME, int HY, int layers, int base, MxMixLayout* L);
+// Wide-state path: the hypernetworks' four state-reading first layers stacked as the columns of one GEMM.  Block order: 0 = hyper_w1
+// (w1a, or w1b with 1-layer hypernets), 1 = hyper_w2 (w2a / w2b), 2 = hyper_b2's first layer (wb2a, ReLU), 3 = hyper_b1 (wb1).
+struct MxMixWide {
+  int C, Cp, Sp;              // stacked columns per net, padded to 16; state width padded to the GEMM's K chunk
+  int col[4], rows[4], w[4], b[4];   // block: first column (multiple of 4), rows, weight / bias offsets in the flat parameters
+};
+// true when the hypernet tile of the shared-memory mixer kernels does not fit in an SM at its largest tile height: such a learner takes
+// the wide-state path.  Depends on the layout only (not on the build, the batch size or the device).
+bool mx_mix_wide_state(const MxMixLayout& L);
+void mx_mix_wide_layout(const MxMixLayout& L, MxMixWide* w);
 
 // ---- QMIX learner workspace -----------------------------------------------------------------------
 struct MxQmixWs {           // offsets in floats into the workspace
@@ -112,6 +122,7 @@ struct MxQmixWs {           // offsets in floats into the workspace
   int64_t hyp_h1, hyp_h2, hyp_hb;               // live [E][gH]
   int64_t hyp_p1[2], hyp_b1[2], hyp_p2[2], hyp_b2[2];
   int64_t d_q, d_hp, d_p2, d_p1;
+  int64_t wimg, pre, d_pre;  // wide-state path only (empty otherwise): state-layer weight images, pre-activations, their gradient
   int64_t total;
 };
 
@@ -127,6 +138,8 @@ struct mx_qmix {
   int64_t ws_bytes;
   MxQmixWs W;
   int split_ok;            // the split mixer pipeline supports this configuration
+  int wide;                // wide-state path (mx_mix_wide_state): state layers on the tensor cores, always the split pipeline
+  MxMixWide wl;
   // data-parallel exchange over peer memory (p2p.cu): symmetric blocks of every rank, set by mx_qmix_set_peers
   int p2p_rank = 0, p2p_world = 0;
   float* p2p_blocks[16] = {nullptr};

@@ -80,8 +80,20 @@ struct MixerArgs {
   float *hyp_p1[2], *hyp_b1[2], *hyp_p2[2], *hyp_b2[2];   // [live|target]: raw hyper_w1 out [E][gP], hyper_b1 [E][gM], hyper_w2 [E][gM], b2 [E]
   float *d_q, *d_hp, *d_p2, *d_p1;                        // dL/dQ_tot [E], d(hidden pre-ELU) [E][gM], d(hyper_w2 out) [E][gM], d(hyper_w1 out) [E][gP]
   int gH, gP, gM;
+  // ---- wide-state path (mx_mix_wide_state): the hypernetworks' state-reading first layers run as one tensor-core GEMM (mixer_wide.cu);
+  // the hypernet kernels read its pre-activations instead of the state rows and hand back the gradient at them
+  int wide;
+  MxMixWide wl;
+  float* wimg;             // [net][hi Cp*Sp | lo Cp*Sp | bias Cp]: TF32 hi / lo split of the stacked state-layer weights, row-major
+  float* pre;              // [net][B*(T+1)][Cp]: state-layer pre-activations (bias added, no activation) of every state row
+  float* d_pre;            // [E][Cp]: live net's gradient at those pre-activations (ReLU-masked where the layer has one)
 };
 int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s);
+// wide-state path (mixer_wide.cu): weight images + state-layer GEMM (before the hypernet forward), state-layer weight gradient (after the
+// hypernet backward: writes the state layers' weights and biases as gradient partial 0)
+int mx_launch_mixw_state_fwd(const MixerArgs& a, cudaStream_t s);
+int mx_launch_mixw_state_wgrad(const MixerArgs& a, cudaStream_t s);
+size_t mx_mixw_image_floats(const MxMixWide& w);
 // split form of the same computation (k_mixer == hyper_fwd ; core ; hyper_bwd).  hyper_fwd depends only on the batch's states and
 // the parameters, hyper_bwd only on core's outputs: the learner runs them on a forked branch next to the agent-net kernels.
 int mx_mixer_split_supported(const MxMixLayout& L);
@@ -197,7 +209,7 @@ struct OptimArgs {
   float* grad;             // [P + 8]
   long long P;             // parameters the optimiser updates: [0, P) of theta / theta_tgt / adam_m / adam_v
   long long gpart_ld;      // floats between consecutive gradient partials (0: P); larger when the partials also hold frozen tensors past P
-  int seg_begin[4], seg_end[4], seg_parts[4], nseg;   // parameter segments and how many partials each has
+  int seg_begin[8], seg_end[8], seg_parts[8], nseg;   // parameter segments and how many partials each has
   const float* spart;
   int spart_n;
   float* info;             // [8]

@@ -169,6 +169,16 @@ static int64_t ws_layout(const mx_qmix_cfg* c, int64_t P, int npart, MxQmixWs* W
     for (int k = 0; k < 2; ++k) { W->hyp_p1[k] = tk(En * gP); W->hyp_b1[k] = tk(En * gM); W->hyp_p2[k] = tk(En * gM); W->hyp_b2[k] = tk(En); }
     W->d_q = tk(En); W->d_hp = tk(En * gM); W->d_p2 = tk(En * gM); W->d_p1 = tk(En * gP);
   }
+  {     // wide-state path: weight images, pre-activations of every state row for both nets, their gradient (live elements)
+    MxNetLayout Al; MxMixLayout Ml; int64_t P2;
+    layouts(c, &Al, &Ml, &P2);
+    const bool wide = !c->vdn && mx_mix_wide_state(Ml);
+    MxMixWide wl;
+    mx_mix_wide_layout(Ml, &wl);
+    W->wimg = tk(wide ? (int64_t)mx_mixw_image_floats(wl) : 0);
+    W->pre = tk(wide ? 2 * B * (T + 1) * wl.Cp : 0);
+    W->d_pre = tk(wide ? E * wl.Cp : 0);
+  }
   W->total = o;
   return o * 4;
 }
@@ -198,6 +208,9 @@ extern "C" int mx_qmix_create(const mx_qmix_cfg* c, float* theta, float* theta_t
   q->ws = (float*)workspace;
   q->ws_bytes = workspace_bytes;
   q->split_ok = !c->vdn && mx_mixer_split_supported(q->mix);
+  q->wide = !c->vdn && mx_mix_wide_state(q->mix);
+  mx_mix_wide_layout(q->mix, &q->wl);
+  if (q->wide && !q->split_ok) { mx_set_error("mx_qmix_create: state_dim %d needs the wide-state mixer, which supports mixer_hidden <= 64", c->state_dim); delete q; return 1; }
 #if !MX_EMU
   {
     // side branch priority (option side_prio, read at creation): 0 = default, 1 = LOWER than the caller's stream (the agent-net kernels are
@@ -236,6 +249,7 @@ extern "C" int mx_qmix_ws_lookup(const mx_qmix* q, const char* name, int64_t* by
       {"hn", W.hn, M * MX_H}, {"greedy", W.greedy, M}, {"q_taken", W.q_taken, E * N}, {"q_next", W.q_next, E * N}, {"qtot", W.qtot, E},
       {"qtot_next", W.qtot_next, E}, {"err", W.err, E}, {"dq_taken", W.dq_taken, E * N}, {"dh_out", W.dh_out, M * MX_H},
       {"xstat", W.xstat, 8}, {"dgi", W.dgi, M * MX_G}, {"grad", W.grad, q->P + 8}, {"info", W.info, 8}, {"adam_t", W.adam_t, 8}, {"prio", W.prio, B}, {"gpart", W.gpart, (int64_t)q->npart * q->P},
+      {"hyp_pre", W.pre, q->wide ? 2 * B * (T + 1) * q->wl.Cp : 0}, {"d_pre", W.d_pre, q->wide ? E * q->wl.Cp : 0},
   };
   for (const Ent& e : tab)
     if (!strcmp(e.n, name)) { *byte_offset = e.off * 4; *n_elems = e.cnt; return 0; }
@@ -277,6 +291,17 @@ static OptimArgs optim_args(mx_qmix* q, int B, const int parts[4], bool after_ex
   o.seg_begin[0] = 0; o.seg_end[0] = q->agent.lno_g; o.seg_parts[0] = parts[0];
   o.seg_begin[1] = q->agent.lno_g; o.seg_end[1] = q->agent.size; o.seg_parts[1] = parts[1];
   o.seg_begin[2] = q->agent.size; o.seg_end[2] = (int)q->P; o.seg_parts[2] = parts[2];
+  if (q->wide) {      // the state layers' gradients are ONE partial (k_mixw_wgrad), the rest of the mixer has the hypernet kernel's partials
+    const MxMixLayout& L = q->mix;
+    const int st = parts[2] > 0 ? 1 : 0;      // (0: the caller passes no partials at all)
+    auto seg = [&](int b, int e, int np) { o.seg_begin[o.nseg] = b; o.seg_end[o.nseg] = e; o.seg_parts[o.nseg] = np; ++o.nseg; };
+    o.nseg = 2;
+    if (L.layers == 2) {
+      seg(L.w1a, L.w1b, st); seg(L.w1b, L.w2a, parts[2]);
+      seg(L.w2a, L.w2b, st); seg(L.w2b, L.wb1, parts[2]);
+    }
+    seg(L.layers == 2 ? L.wb1 : L.w1b, L.wb2b, st); seg(L.wb2b, (int)q->P, parts[2]);
+  }
   o.spart = ws + q->W.spart; o.spart_n = parts[3];
   o.info = ws + q->W.info;
   o.adam_t = reinterpret_cast<double*>(ws + q->W.adam_t);
@@ -358,7 +383,7 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
   cudaStream_t side = s;
 #endif
   // the split mixer only pays off when its hypernet kernels run beside the agent nets (serial, the fused k_mixer moves less data)
-  const bool split = q->split_ok && (g_mx_mixer_split >= 2 || (g_mx_mixer_split == 1 && wanted));
+  const bool split = q->wide || (q->split_ok && (g_mx_mixer_split >= 2 || (g_mx_mixer_split == 1 && wanted)));
 
   MixerArgs mx;
   memset(&mx, 0, sizeof(mx));
@@ -375,6 +400,8 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
   for (int k = 0; k < 2; ++k) { mx.hyp_p1[k] = ws + W.hyp_p1[k]; mx.hyp_b1[k] = ws + W.hyp_b1[k]; mx.hyp_p2[k] = ws + W.hyp_p2[k]; mx.hyp_b2[k] = ws + W.hyp_b2[k]; }
   mx.d_q = ws + W.d_q; mx.d_hp = ws + W.d_hp; mx.d_p2 = ws + W.d_p2; mx.d_p1 = ws + W.d_p1;
   mx.gH = mx_round_up(c.hyper_hidden, 4); mx.gM = mx_round_up(c.mixer_hidden, 4); mx.gP = mx_round_up(c.n_agents * c.mixer_hidden, 4);
+  mx.wide = q->wide; mx.wl = q->wl;
+  if (q->wide) { mx.wimg = ws + W.wimg; mx.pre = ws + W.pre; mx.d_pre = ws + W.d_pre; }
 
   const float* X = b->obs;
   int ldx = b->obs_ld;
