@@ -380,7 +380,7 @@ void mx_graph_destroy(mx_graph* g);
 
 /* Tensor-core building block probe (parity tests): Y[M][N] = X[M][K] . W[N][K]^T with wgmma on TF32
  * operands; passes = 1 (plain TF32) or 3 (3xTF32 hi/lo split, fp32-level accuracy); swap_ls selects which descriptor field
- * carries the K-direction core-matrix stride.  N % 16 == 0, N <= 256, K % 8 == 0, K <= 64. */
+ * carries the K-direction core-matrix stride (the kernels use swap_ls = 0).  N % 16 == 0, N <= 256, K % 8 == 0, K <= 64. */
 int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int32_t N, int32_t K, int32_t passes, int32_t swap_ls, void* stream);
 
 /* Runtime options (process-wide tuning switches; the defaults are not yet re-measured on the H100).
@@ -403,8 +403,7 @@ int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int3
  *   p2p_ll (1)              data-parallel exchange as flag-in-data lines (0: slots + one flag per rank); p2p_timeout_ms (10000) wait for a peer
  *   gather_tma (1)          episode gather on the TMA unit (0: vectorised loads; 2: TMA at every size)
  *   pdl (-1)                programmatic dependent launch: -1 = QMIX steps of <= pdl_rows (12288) rows and the R-MADDPG update, 0 never, 1 always
- *   smem_carveout (100)     preferred shared-memory carveout (percent) of every step kernel; -1 = driver default
- *   tc_swap_ls (0)          shared-memory descriptor stride convention (see mx_tc_linear_probe) */
+ *   smem_carveout (100)     preferred shared-memory carveout (percent) of every step kernel; -1 = driver default */
 int mx_set_option(const char* name, int32_t value);
 
 /* number of kernel launches issued by this library since load (bench.py's gpu_launches counter) */

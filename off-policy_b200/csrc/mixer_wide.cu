@@ -12,7 +12,7 @@
 //                   owns a (128 columns x 64 state features) tile and reduces over all elements itself: the result is gradient
 //                   partial 0 of the state layers and the optimiser reads that one partial (no per-CTA partial rows over ~S x C floats)
 //
-// Both GEMMs are D[128][N] += A[128][32] . B[N][32]^T chunks on tc::issue_layer_acc (mx_tc.cuh) with the accumulator in shared memory;
+// Both GEMMs are D[128][N] += A[128][32] . B[N][32]^T chunks on tc::mma (mx_tc.cuh) with the accumulator in shared memory;
 // operands are split into TF32 hi / lo on the way into shared memory (state rows, d_pre) or copied pre-split (the weight images).  The next
 // chunk's weight tile is in flight (cp.async) and the next chunk's state values in registers while the tensor cores run the current one.
 #include "mx_internal.h"
@@ -22,8 +22,6 @@
 #define MXW_KC 32           // K chunk (state features in the forward, elements in the weight gradient)
 #define MXW_NB 128          // forward: output columns per CTA
 #define MXW_NS 64           // weight gradient: state features per CTA
-
-extern int g_mx_tc_swap;
 
 size_t mx_mixw_image_floats(const MxMixWide& w) { return (size_t)2 * ((size_t)2 * w.Cp * w.Sp + w.Cp); }
 
@@ -105,12 +103,11 @@ MX_DEVINL void mixw_put4(char* hi, char* lo, int r, int k, float4 x) {
 }
 
 // grid (row tiles of 128, 2 nets x column blocks of MXW_NB); thread r owns accumulator row r in the epilogue
-__global__ void __launch_bounds__(128, 1) k_mixw_fwd(MixerArgs a, MixwFwdSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 1) k_mixw_fwd(MixerArgs a, MixwFwdSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   const MxMixWide w = a.wl;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int ncb = (w.Cp + MXW_NB - 1) / MXW_NB;
   const int net = blockIdx.y / ncb, c0 = (blockIdx.y - net * ncb) * MXW_NB;
   const int nb = w.Cp - c0 < MXW_NB ? w.Cp - c0 : MXW_NB;      // multiple of 16
@@ -123,7 +120,7 @@ __global__ void __launch_bounds__(128, 1) k_mixw_fwd(MixerArgs a, MixwFwdSmem sm
   char* b_hi = reinterpret_cast<char*>(smem_raw) + sm.o_bhi;
   char* b_lo = reinterpret_cast<char*>(smem_raw) + sm.o_blo;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<MXW_NB>(&tmem_s, reinterpret_cast<float*>(smem_raw + sm.o_acc));
+  float* acc = reinterpret_cast<float*>(smem_raw + sm.o_acc);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -151,22 +148,19 @@ __global__ void __launch_bounds__(128, 1) k_mixw_fwd(MixerArgs a, MixwFwdSmem sm
       mx_cp_wait<0>();
     }
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
     if (kc + 1 < nk) mixw_load_x(xv, a.share, a.share_ld, a.L.S, R, m0, kc + 1);      // in flight during the MMAs
-    tc::issue_layer_acc(tmem_s, a_hi, a_lo, b_hi + buf * bstride, b_lo + buf * bstride, nb, MXW_KC, swap_ls, kc > 0 ? 1u : 0u, bar);
+    tc::mma(acc, 0, a_hi, a_lo, b_hi + buf * bstride, b_lo + buf * bstride, nb, MXW_KC, 3, kc > 0 ? 1u : 0u);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_before();
     __syncthreads();      // operand tiles free for the next chunk
-    tc::fence_after();
   }
   const int m = m0 + tid;
   float* out = a.pre + ((size_t)net * R + m) * w.Cp + c0;
   for (int cc = 0; cc < nb; cc += 32) {
     float v[32];
-    tc::tmem_ld32(tmem_s + ((uint32_t)(warp * 32) << 16) + (uint32_t)cc, v);
+    tc::ld_row(acc, cc, tid, v);
     if (m < R)
 #pragma unroll
       for (int c = 0; c < 32; c += 4)
@@ -174,7 +168,6 @@ __global__ void __launch_bounds__(128, 1) k_mixw_fwd(MixerArgs a, MixwFwdSmem sm
           mx_st4(out + cc + c, make_float4(v[c] + bias[c0 + cc + c], v[c + 1] + bias[c0 + cc + c + 1], v[c + 2] + bias[c0 + cc + c + 2],
                                            v[c + 3] + bias[c0 + cc + c + 3]));
   }
-  if (warp == 0) tc::tmem_dealloc<MXW_NB>(tmem_s);
 }
 
 int mx_launch_mixw_state_fwd(const MixerArgs& a, cudaStream_t s) {
@@ -199,7 +192,7 @@ int mx_launch_mixw_state_fwd(const MixerArgs& a, cudaStream_t s) {
     configured = true;
   }
 #endif
-  MX_LAUNCH_PDL(k_mixw_fwd, grid, dim3(128), (size_t)sm.total, s, a, sm, g_mx_tc_swap);
+  MX_LAUNCH_PDL(k_mixw_fwd, grid, dim3(128), (size_t)sm.total, s, a, sm);
   MX_COUNT();
   MX_MARK("k_mixw_fwd", s);
   return MX_CHECK_LAUNCH("mixw_fwd");
@@ -249,12 +242,11 @@ MX_DEVINL void mixw_load_g(float4 (&av)[8], float4 (&bv)[4], const MixerArgs& a,
 }
 
 // grid (feature tiles of MXW_NS, column tiles of 128)
-__global__ void __launch_bounds__(128, 2) k_mixw_wgrad(MixerArgs a, MixwGradSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 2) k_mixw_wgrad(MixerArgs a, MixwGradSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   const MxMixWide w = a.wl;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int S = a.L.S, E = a.B * a.T;
   const int k0 = blockIdx.x * MXW_NS, c0 = blockIdx.y * 128;
   const bool with_bias = blockIdx.x == 0;
@@ -264,7 +256,7 @@ __global__ void __launch_bounds__(128, 2) k_mixw_wgrad(MixerArgs a, MixwGradSmem
   char* b_hi = reinterpret_cast<char*>(smem_raw) + sm.o_bhi;
   char* b_lo = reinterpret_cast<char*>(smem_raw) + sm.o_blo;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<MXW_NS + 16>(&tmem_s, reinterpret_cast<float*>(smem_raw + sm.o_acc));
+  float* acc = reinterpret_cast<float*>(smem_raw + sm.o_acc);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -294,33 +286,28 @@ __global__ void __launch_bounds__(128, 2) k_mixw_wgrad(MixerArgs a, MixwGradSmem
         mixw_put4(b_hi, b_lo, MXW_NS + n, 4 * q, make_float4(x[0], x[1], x[2], x[3]));
       }
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
     if (kc + 1 < nk) mixw_load_g(av, bv, a, c0, k0, E, kc + 1);      // in flight during the MMAs
-    tc::issue_layer_acc(tmem_s, a_hi, a_lo, b_hi, b_lo, nb, MXW_KC, swap_ls, kc > 0 ? 1u : 0u, bar);
+    tc::mma(acc, 0, a_hi, a_lo, b_hi, b_lo, nb, MXW_KC, 3, kc > 0 ? 1u : 0u);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
   }
   // row c of the accumulator = stacked column c0 + tid: gradient partial 0 of its weight row (and bias)
   const MixwRow o = mixw_row(w, c0 + tid);
-  const uint32_t row = tmem_s + ((uint32_t)(warp * 32) << 16);
   float v[32];
   for (int cc = 0; cc < MXW_NS; cc += 32) {
-    tc::tmem_ld32(row + (uint32_t)cc, v);
+    tc::ld_row(acc, cc, tid, v);
     if (o.j >= 0)
 #pragma unroll
       for (int i = 0; i < 32; ++i)
         if (k0 + cc + i < S) a.gpart[o.w + (size_t)o.r * S + k0 + cc + i] = v[i];
   }
   if (with_bias) {      // accumulator column MXW_NS, read as element 16 of the 32 columns ending at nb = MXW_NS + 16
-    tc::tmem_ld32(row + (uint32_t)(MXW_NS - 16), v);
+    tc::ld_row(acc, MXW_NS - 16, tid, v);
     if (o.j >= 0) a.gpart[o.b + o.r] = v[16];
   }
-  if (warp == 0) tc::tmem_dealloc<MXW_NS + 16>(tmem_s);
 }
 
 int mx_launch_mixw_state_wgrad(const MixerArgs& a, cudaStream_t s) {
@@ -334,7 +321,7 @@ int mx_launch_mixw_state_wgrad(const MixerArgs& a, cudaStream_t s) {
     configured = true;
   }
 #endif
-  MX_LAUNCH_PDL(k_mixw_wgrad, grid, dim3(128), (size_t)sm.total, s, a, sm, g_mx_tc_swap);
+  MX_LAUNCH_PDL(k_mixw_wgrad, grid, dim3(128), (size_t)sm.total, s, a, sm);
   MX_COUNT();
   MX_MARK("k_mixw_wgrad", s);
   return MX_CHECK_LAUNCH("mixw_wgrad");

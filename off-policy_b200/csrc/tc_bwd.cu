@@ -11,7 +11,7 @@
 //   D1[128][144] = [dgi_r | dgi_z]^T     . [x2 | h_prev | 1]   -> dW_ih[0:128], dW_hh[0:128], db_ih[0:128] (= db_hh[0:128])
 //   D2[128][144] = [dgi_n | dgi_n * r]^T . [x2 | h_prev | 1]   -> dW_ih[128:192] (rows 0-63, cols 0-63), dW_hh[128:192] (rows 64-127, cols 64-127)
 //   D3[128][..]  = [da2   | da1]^T       . [x1 | x0]           -> dW2 (rows 0-63, cols 0-63), dW1 (rows 64-127, cols 64..)
-//   D4[128][16]  = [da2   | da1]^T       . [1 | 0..]           -> db2, db1 (a 16-column accumulator in D1's padding; same A tile, same commit)
+//   D4[128][16]  = [da2   | da1]^T       . [1 | 0..]           -> db2, db1 (a 16-column accumulator in D1's padding; same A tile, same arrival)
 // The off-diagonal blocks of D2 / D3 are products nobody needs (half of two of the three MMAs): the tensor core is not the limit here.
 // Each CTA writes its sums as ONE gradient partial (its row of gpart), like k_front_bwd does for the LayerNorm parameters it keeps.
 #include "mx_internal.h"
@@ -68,10 +68,9 @@ struct WgradArgs {
 };
 
 #define WG_THREADS 512        // staging is load-latency bound: 16 warps keep enough loads in flight; warps 0-3 own the accumulator rows in the epilogue
-__global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[4 * 64 + 2 * 128];  // ln2 g,b | ln1 g,b | fn g (128), fn b (128)
   __shared__ float st_s[3 * 2 * WG_ROWS];    // (mean, rstd) of the chunk's rows for LN2 | LN1 | the feature LayerNorm
   const FrontBwdArgs& a = w.f;
@@ -84,7 +83,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo, *b_hi = base + sm.o_bhi, *b_lo = base + sm.o_blo;
   char *o_hi = base + sm.o_ones, *o_lo = o_hi + 16 * WG_ROWS * 4;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<512>(&tmem_s, tc::cta_slice(a.tc_acc, 512));
+  float* acc = tc::cta_slice(a.tc_acc, 512);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -94,10 +93,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
   }
   for (int i = tid; i < 128; i += blockDim.x) { par_s[256 + i] = i < I ? th[L.fn_g + i] : 0.f; par_s[384 + i] = i < I ? th[L.fn_b + i] : 0.f; }
   MX_PDL_WAIT();
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
   uint32_t phase = 0;
   int iter = 0;
   for (int chunk = blockIdx.x; chunk < w.nchunks; chunk += gridDim.x, ++iter) {
@@ -186,13 +182,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
         }
       }
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer_acc(tmem_base + pass * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, 144, WG_ROWS, swap_ls, acc0, bar);
+      tc::mma(acc, pass * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, 144, WG_ROWS, 3, acc0);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);      // the MMAs have read the tiles: A (and after the second pass B) may be refilled
       phase ^= 1;
-      tc::fence_after();
     }
     // ---- A = [da2 | da1], B = [x1 | x0 | 1] -> D3 ----
     {
@@ -264,53 +258,48 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
       wg_put(o_hi, o_lo, n, kq, x);
     }
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
-    {
-      tc::issue_layer_acc(tmem_base + 2 * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, N3, WG_ROWS, swap_ls, acc0, bar, false);
-      tc::issue_layer_acc(tmem_base + WG_ONES_COL, a_hi, a_lo, o_hi, o_lo, 16, WG_ROWS, swap_ls, acc0, bar, true);      // one commit for both
-    }
+    tc::mma(acc, 2 * WG_DSTRIDE, a_hi, a_lo, b_hi, b_lo, N3, WG_ROWS, 3, acc0);
+    tc::mma(acc, WG_ONES_COL, a_hi, a_lo, o_hi, o_lo, 16, WG_ROWS, 3, acc0);
+    tc::arrive(bar);      // one arrival for both
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_after();
   }
   // ---- epilogue: thread r (warps 0-3) = accumulator row r -> this CTA's gradient partial ----
   float* gp = a.gpart + (size_t)blockIdx.x * a.P;
   if (warp < 4) {
-  const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
   const bool any = iter > 0;      // a CTA without rows writes zeros (its accumulator was never written)
   const int r = tid;
   float v[64];
   float t[32];
   // D1: gates r, z
-  if (any) tc::tmem_ld64(trow, v);
+  if (any) tc::ld_row(acc, 0, r, v);
 #pragma unroll
   for (int c4 = 0; c4 < 16; ++c4)
     *reinterpret_cast<float4*>(gp + L.wih + (size_t)r * MX_H + 4 * c4) = any ? make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   const bool gru = !a.no_gru;       // MLP variant: the recurrent slots of the partial are never written (they stay at their initial zeros)
-  if (any) tc::tmem_ld64(trow + 64, v);
+  if (any) tc::ld_row(acc, 64, r, v);
   if (gru) {
 #pragma unroll
     for (int c4 = 0; c4 < 16; ++c4)
       *reinterpret_cast<float4*>(gp + L.whh + (size_t)r * MX_H + 4 * c4) = any ? make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  if (any) tc::tmem_ld32(trow + 128, t);      // column 128: D1's ones column; column 144 (= t[16]): [da2 | da1]^T . 1
+  if (any) tc::ld_row(acc, 128, r, t);      // column 128: D1's ones column; column 144 (= t[16]): [da2 | da1]^T . 1
   gp[L.bih + r] = any ? t[0] : 0.f;
   if (gru) gp[L.bhh + r] = any ? t[0] : 0.f;
   gp[(r < 64 ? L.b2 : L.b1) + (r & 63)] = any ? t[16] : 0.f;
   // D2: n gate.  rows 0-63: dW_ih[128 + r] = cols 0-63, db_ih ; rows 64-127: dW_hh[128 + r - 64] = cols 64-127, db_hh
-  if (any) tc::tmem_ld64(trow + WG_DSTRIDE + (r < 64 ? 0 : 64), v);
+  if (any) tc::ld_row(acc, WG_DSTRIDE + (r < 64 ? 0 : 64), r, v);
   if (r < 64 || gru) {
     float* dst = gp + (r < 64 ? L.wih : L.whh) + (size_t)(128 + (r & 63)) * MX_H;
 #pragma unroll
     for (int c4 = 0; c4 < 16; ++c4)
       *reinterpret_cast<float4*>(dst + 4 * c4) = any ? make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  if (any) tc::tmem_ld32(trow + WG_DSTRIDE + 128, t);
+  if (any) tc::ld_row(acc, WG_DSTRIDE + 128, r, t);
   if (r < 64 || gru) gp[(r < 64 ? L.bih : L.bhh) + 128 + (r & 63)] = any ? t[0] : 0.f;
   // D3: rows 0-63: dW2[r] = cols 0-63, db2 ; rows 64-127: dW1[r - 64][0:I] = cols 64.., db1
-  if (any) tc::tmem_ld64(trow + 2 * WG_DSTRIDE + (r < 64 ? 0 : 64), v);
+  if (any) tc::ld_row(acc, 2 * WG_DSTRIDE + (r < 64 ? 0 : 64), r, v);
   if (r < 64) {
 #pragma unroll
     for (int c4 = 0; c4 < 16; ++c4)
@@ -322,7 +311,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
       if (c < I) dst[c] = any ? v[c] : 0.f;
     if (I > 64) {                                 // wide inputs: the second 64-column block of x0 (CTA-uniform branch)
       float v2[64];
-      if (any) tc::tmem_ld64(trow + 2 * WG_DSTRIDE + 128, v2);
+      if (any) tc::ld_row(acc, 2 * WG_DSTRIDE + 128, r, v2);
 #pragma unroll
       for (int c = 0; c < 64; ++c)
         if (64 + c < I) dst[64 + c] = any ? v2[c] : 0.f;
@@ -342,16 +331,12 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
     for (int c = tid; c < MX_H; c += blockDim.x) { gp[L.ln2_g + c] = 0.f; gp[L.ln2_b + c] = 0.f; gp[L.ln1_g + c] = 0.f; gp[L.ln1_b + c] = 0.f; }
     for (int c = tid; c < I; c += blockDim.x) { gp[L.fn_g + c] = 0.f; gp[L.fn_b + c] = 0.f; }
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<512>(tmem_base);
 }
 
 bool mx_wgrad_tc_usable(const FrontBwdArgs& a) {
   return wgrad_mode(a.L.in_dim) && a.da2_out && a.da1_out && !a.skip_wgrad && a.L.in_dim <= (g_mx_wgrad_tc_wide ? WG_MAX_IN : 64) && a.M >= 1;
 }
 
-extern int g_mx_tc_swap;
 static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, cudaStream_t s, int ln_parts = 0);
 int mx_launch_wgrad_tc(const FrontBwdArgs& a, int nparts, cudaStream_t s) { return launch_wgrad_tc(a, nparts, -1, s); }
 static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, cudaStream_t s, int ln_parts) {
@@ -373,7 +358,7 @@ static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, 
     configured = sm.total;
   }
 #endif
-  MX_LAUNCH_PDL(k_wgrad_tc, dim3(nparts), dim3(WG_THREADS), (size_t)sm.total, s, w, sm, g_mx_tc_swap);
+  MX_LAUNCH_PDL(k_wgrad_tc, dim3(nparts), dim3(WG_THREADS), (size_t)sm.total, s, w, sm);
   MX_COUNT();
   MX_MARK("k_wgrad_tc", s);
   return MX_CHECK_LAUNCH("wgrad_tc");
@@ -497,14 +482,13 @@ __device__ __forceinline__ void bt_ln_bwd_relu(bool act_tanh, float (&dy)[64], c
   }
 }
 
-__global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[2 * 64];            // gains: ln2 | ln1
   const MxNetLayout L = a.L;
   const float* __restrict__ th = a.theta;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int I = L.in_dim, Kp16 = (I + 15) & ~15;
   char* base = reinterpret_cast<char*>(smem_raw);
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo, *wih = base + sm.o_wih, *w2 = base + sm.o_w2, *w1 = base + sm.o_w1;
@@ -515,7 +499,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
   const bool restage = !stream && sm.o_w1 == sm.o_w2;
   const float* img_w2 = a.tc_imgT + 2 * 3 * 4096;
   const float* img_w1 = img_w2 + 2 * 4096;
-  if (warp == 0) tc::tmem_alloc<128>(&tmem_s, tc::cta_slice(a.tc_acc, 128));
+  float* acc = tc::cta_slice(a.tc_acc, 128);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -534,11 +518,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
     for (int v = tid; v < (nbytes >> 4); v += blockDim.x) mx_cp16(dst + 4 * v, src + 4 * v);
     mx_cp_commit();
   };
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  const uint32_t tmem_row = tmem_base + ((uint32_t)(warp * 32) << 16);
   uint32_t phase = 0;
   float acc2 = 0.f, acc1 = 0.f, acc0a = 0.f, acc0b = 0.f;      // running column sums: threads 0-63 gain gradients, 64-127 bias gradients
   const int ntiles = (a.M + 127) / 128;
@@ -557,20 +537,18 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
       bt_put_row64(a_hi, a_lo, tid, x);
       mx_cp_wait<0>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
       const char* wch = stream ? wih : wih + ch * 2 * 4096 * 4;
-      tc::issue_layer_acc(tmem_base, a_hi, a_lo, wch, wch + 4096 * 4, 64, 64, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::mma(acc, 0, a_hi, a_lo, wch, wch + 4096 * 4, 64, 64, 3, ch > 0 ? 1u : 0u);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
-      tc::fence_after();
       if (stream) stage_chunk(ch < 2 ? a.tc_imgT + (ch + 1) * 2 * 4096 : img_w2, 2 * 4096 * 4);      // next gate chunk, then W2^T: in flight during the loads / epilogue
     }
     // ---- LN2', ReLU' -> da2 ; then fc2 and LN1', ReLU' -> da1 ----
     for (int layer = 0; layer < 2; ++layer) {
       float v[64];
-      tc::tmem_ld64(tmem_row, v);
+      tc::ld_row(acc, 0, tid, v);
       const float* st = layer == 0 ? a.st2 : a.st1;
       const float* uu = layer == 0 ? a.u2 : a.u1;
       // (the MMAs that read the A tile have completed: its shared memory is the scratch until the next operand is written)
@@ -592,16 +570,12 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
         mx_cp_wait<0>();
       }
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      {
-        if (layer == 0) tc::issue_layer(tmem_base, a_hi, a_lo, w2, w2 + 4096 * 4, 64, 64, 3, swap_ls, bar);
-        else tc::issue_layer(tmem_base, a_hi, a_lo, w1, w1 + Kp16 * 64 * 4, Kp16, 64, 3, swap_ls, bar);
-      }
+      if (layer == 0) tc::mma(acc, 0, a_hi, a_lo, w2, w2 + 4096 * 4, 64, 64, 3, 0);
+      else tc::mma(acc, 0, a_hi, a_lo, w1, w1 + Kp16 * 64 * 4, Kp16, 64, 3, 0);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
-      tc::fence_after();
       if (stream) {
         if (layer == 0) stage_chunk(img_w1, 2 * Kp16 * 64 * 4);
         else if (tile + (int)gridDim.x < ntiles) stage_chunk(a.tc_imgT, 2 * 4096 * 4);      // the next tile's first gate chunk
@@ -612,7 +586,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
       const float mean = (ok && a.feature_norm) ? a.st0[2 * mm] : 0.f, rstd = (ok && a.feature_norm) ? a.st0[2 * mm + 1] : 0.f;
       for (int cb = 0; 64 * cb < I; ++cb) {
         float v[64];
-        tc::tmem_ld64(tmem_row + 64 * cb, v);         // columns >= Kp16 hold leftovers of the previous layer: masked below
+        tc::ld_row(acc, 64 * cb, tid, v);         // columns >= Kp16 hold leftovers of the previous layer: masked below
 #pragma unroll
         for (int c4 = 0; c4 < 16; ++c4) {
           float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -631,9 +605,7 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
         if (cb == 0) acc0a += part; else acc0b += part;
       }
     }
-    tc::fence_before();
     __syncthreads();     // accumulator reads drained before the next tile's MMAs
-    tc::fence_after();
   }
   // ---- this CTA's partial of the LayerNorm gain / bias gradients ----
   const int col = tid & 63;
@@ -656,9 +628,6 @@ __global__ void __launch_bounds__(128, 2) k_front_bwd_tc(FrontBwdArgs a, BwdTcSm
   }
   }
   mx_cp_wait<0>();
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<128>(tmem_base);
 }
 
 bool mx_front_bwd_tc_usable(const FrontBwdArgs& a) {
@@ -699,7 +668,7 @@ int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t
   b.wgrad_external = 1;
   if (!stream) b.ln_part = nullptr;
   if (ga > a.ln_part_rows && stream) ga = a.ln_part_rows;
-  MX_LAUNCH_PDL(k_front_bwd_tc, dim3(ga), dim3(128), (size_t)sm.total, s, b, sm, g_mx_tc_swap);
+  MX_LAUNCH_PDL(k_front_bwd_tc, dim3(ga), dim3(128), (size_t)sm.total, s, b, sm);
   MX_COUNT();
   MX_MARK("k_front_bwd_tc", s);
   if (MX_CHECK_LAUNCH("front_bwd_tc")) return 1;

@@ -17,7 +17,7 @@
 
 // =====================================================================================================
 // front forward on the tensor cores: LN -> fc1 -> ReLU -> LN -> fc2 -> ReLU -> LN -> W_ih for a 128-row tile per CTA.
-// Thread r owns accumulator row r: after tmem_ld64 a whole 64-wide layer output sits in that thread's
+// Thread r owns accumulator row r: after tc::ld_row a whole 64-wide layer output sits in that thread's
 // registers, so bias / ReLU / LayerNorm need no cross-thread traffic at all; the normalised row is split into TF32
 // hi/lo and written straight back into the A operand tiles for the next layer.
 // =====================================================================================================
@@ -137,12 +137,11 @@ __device__ __forceinline__ void tc_put_row64(char* hi, char* lo, int r, const fl
   }
 }
 
-__global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTcSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTcSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[6 * MX_H + MX_G + 2 * 64];      // b1,g1,be1,b2,g2,be2 | b_ih | fn_g, fn_b
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int net = blockIdx.y;
   const float* __restrict__ th = a.theta[net];
   const MxNetLayout L = a.L;
@@ -152,7 +151,6 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w1l = base + sm.o_w1l, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -163,7 +161,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
     par_s[6 * MX_H + MX_G + i] = i < I ? th[L.fn_g + i] : 0.f; par_s[6 * MX_H + MX_G + 64 + i] = i < I ? th[L.fn_b + i] : 0.f;
   }
   for (int i = tid; i < MX_G; i += blockDim.x) par_s[6 * MX_H + i] = th[L.bih + i];
-  MX_PDL_WAIT();        // the accumulator address, the mbarrier and the parameter rows are private / parameter data; the images and inputs are not
+  MX_PDL_WAIT();        // the mbarrier and the parameter rows are private / parameter data; the images and inputs are not
   if (a.tc_img[net]) {
     // the image is byte-identical to the shared-memory weight region: straight 16-byte async copies
     // two groups: fc1+fc2 first, W_ih (two thirds of the bytes) lands while the first two layers run
@@ -182,15 +180,12 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
   const float* bih_s = par_s + 6 * MX_H;
   const float* fng_s = par_s + 6 * MX_H + MX_G;
   const float* fnb_s = fng_s + 64;
-  tc::fence_before();
-  __syncthreads();        // parameters, accumulator address and the mbarrier are visible; the weight copies are still in flight
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  const uint32_t tmem_row = tmem_base + ((uint32_t)(warp * 32) << 16);
+  __syncthreads();        // parameters and the mbarrier are visible; the weight copies are still in flight
   uint32_t phase = 0;
   const int ntiles = (a.M + 127) / 128;
   const int I4 = (I + 3) >> 2;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    float* acc = tc::cta_slice(a.tc_acc, 256);      // (per tile: a pointer held across the loop costs registers)
     const int m = tile * 128 + tid;
     const bool ok = m < a.M;
     // ---- input row (thread per row, 16-byte loads): LayerNorm over I features, split, write the layer-1 A tile (K = Kp) ----
@@ -228,15 +223,13 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
     for (int layer = 0; layer < 2; ++layer) {
       mx_cp_wait<1>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
+      tc::mma(acc, 0, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, 0);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
-      tc::fence_after();
       float v[64];
-      tc::tmem_ld64(tmem_row, v);
+      tc::ld_row(acc, 0, tid, v);
       const float* bs = par_s + layer * 3 * MX_H;
 #pragma unroll
       for (int c = 0; c < 64; ++c) { const float z = v[c] + bs[c]; v[c] = a.act_tanh ? tanhf(z) : fmaxf(z, 0.f); }
@@ -256,18 +249,16 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
     // ---- gi = x2 . W_ih^T + b_ih ----
     mx_cp_wait<0>();
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
-    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::mma(acc, 0, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, 0);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_after();
     float* gi = a.gi[net];
 #pragma unroll 1
     for (int c0 = 0; c0 < MX_G; c0 += 64) {
       float t0[64];
-      tc::tmem_ld64(tmem_row + c0, t0);
+      tc::ld_row(acc, c0, tid, t0);
       if (ok) {
 #pragma unroll
         for (int c4 = 0; c4 < 16; ++c4)
@@ -276,13 +267,8 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc(FrontFwdArgs a, FrontTc
                           t0[4 * c4 + 3] + bih_s[c0 + 4 * c4 + 3]);
       }
     }
-    tc::fence_before();
     __syncthreads();     // every thread has drained its accumulator reads before the next tile's MMAs overwrite the accumulator
-    tc::fence_after();
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
 
@@ -331,13 +317,12 @@ __device__ __forceinline__ void tc_put_row32(char* hi, char* lo, int r, int c0, 
   }
 }
 
-__global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontTcSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontTcSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[6 * MX_H + MX_G + 2 * 64];      // b1,g1,be1,b2,g2,be2 | b_ih | fn_g, fn_b
   __shared__ float ex_s[2][2][128];                        // pair exchange of LayerNorm partial sums
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int r = tid & 127, half = tid >> 7, c0 = 32 * half;
   const int net = blockIdx.y;
   const float* __restrict__ th = a.theta[net];
@@ -348,7 +333,7 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w1l = base + sm.o_w1l, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
+  float* acc = tc::cta_slice(a.tc_acc, 256);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -376,11 +361,7 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
   const float* bih_s = par_s + 6 * MX_H;
   const float* fng_s = par_s + 6 * MX_H + MX_G;
   const float* fnb_s = fng_s + 64;
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  const uint32_t tmem_row = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);       // warps w and w + 4 read the same lane quadrant
   uint32_t phase = 0;
   int xb = 0;
   const int ntiles = (a.M + 127) / 128;
@@ -423,15 +404,13 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
     for (int layer = 0; layer < 2; ++layer) {
       mx_cp_wait<1>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer(tmem_base, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, swap_ls, bar);
+      tc::mma(acc, 0, a_hi, a_lo, layer == 0 ? w1h : w2h, layer == 0 ? w1l : w2l, MX_H, layer == 0 ? Kp : MX_H, 3, 0);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
-      tc::fence_after();
       float v[32];
-      tc::tmem_ld32(tmem_row + c0, v);
+      tc::ld_row(acc, c0, r, v);
       const float* bs = par_s + layer * 3 * MX_H;
 #pragma unroll
       for (int c = 0; c < 32; ++c) { const float z = v[c] + bs[c0 + c]; v[c] = a.act_tanh ? tanhf(z) : fmaxf(z, 0.f); }
@@ -451,18 +430,16 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
     // ---- gi = x2 . W_ih^T + b_ih: columns [96 half, 96 half + 96) ----
     mx_cp_wait<0>();
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
-    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::mma(acc, 0, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, 0);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_after();
     float* gi = a.gi[net];
 #pragma unroll 1
     for (int g0 = 96 * half; g0 < 96 * half + 96; g0 += 32) {
       float t0[32];
-      tc::tmem_ld32(tmem_row + g0, t0);
+      tc::ld_row(acc, g0, r, t0);
       if (ok) {
 #pragma unroll
         for (int c4 = 0; c4 < 8; ++c4)
@@ -471,13 +448,8 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
                           t0[4 * c4 + 3] + bih_s[g0 + 4 * c4 + 3]);
       }
     }
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
 
@@ -486,13 +458,12 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
 // columns that accumulate in the accumulator -- the A tile stays [128][64] and only one fc1 weight chunk is resident (restaged per tile from
 // the L2-resident image), so that fc2 and W_ih (96 KB as hi / lo) still fit beside them: 224 KB of dynamic shared memory.
 // =====================================================================================================
-__global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, FrontTcSmem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, FrontTcSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[6 * MX_H];             // b1,g1,be1,b2,g2,be2   (b_ih and the feature-norm rows are read through L1: the dynamic
                                                 // 224 KB leave ~3 KB of static shared memory under the 227 KB per-CTA limit)
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int net = blockIdx.y;
   const float* __restrict__ th = a.theta[net];
   const MxNetLayout L = a.L;
@@ -502,7 +473,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
   char *w1h = base + sm.o_w1h, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
+  float* acc = tc::cta_slice(a.tc_acc, 256);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -523,11 +494,7 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
   const float* bih_s = th + L.bih;
   const float* fng = th + L.fn_g;
   const float* fnb = th + L.fn_b;
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  const uint32_t tmem_row = tmem_base + ((uint32_t)(warp * 32) << 16);
   uint32_t phase = 0;
   const int ntiles = (a.M + 127) / 128;
   const int I4 = (I + 3) >> 2;
@@ -606,28 +573,24 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
       }
       mx_cp_wait<0>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer_acc(tmem_base, a_hi, a_lo, w1h, w1h + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::mma(acc, 0, a_hi, a_lo, w1h, w1h + 64 * Kc * 4, MX_H, Kc, 3, ch > 0 ? 1u : 0u);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);        // the MMAs have read the A tile and the weight chunk: both may be refilled
       phase ^= 1;
-      tc::fence_after();
     }
     // ---- fc1 epilogue, then fc2 (weights resident) ----
     for (int layer = 0; layer < 2; ++layer) {
       if (layer == 1) {
         tc::fence_async_smem();
-        tc::fence_before();
         __syncthreads();
-        tc::fence_after();
-        tc::issue_layer(tmem_base, a_hi, a_lo, w2h, w2l, MX_H, MX_H, 3, swap_ls, bar);
+        tc::mma(acc, 0, a_hi, a_lo, w2h, w2l, MX_H, MX_H, 3, 0);
+        tc::arrive(bar);
         tc::mbar_wait(bar, phase);
         phase ^= 1;
-        tc::fence_after();
       }
       float v[64];
-      tc::tmem_ld64(tmem_row, v);
+      tc::ld_row(acc, 0, tid, v);
       const float* bs = par_s + layer * 3 * MX_H;
 #pragma unroll
       for (int c = 0; c < 64; ++c) { const float z = v[c] + bs[c]; v[c] = a.act_tanh ? tanhf(z) : fmaxf(z, 0.f); }
@@ -642,25 +605,21 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
       }
 #pragma unroll
       for (int c = 0; c < 64; ++c) v[c] = (v[c] - mu) * rs * bs[MX_H + c] + bs[2 * MX_H + c];
-      tc::fence_before();
       __syncthreads();          // every thread has drained its accumulator reads before the next layer's MMAs overwrite the accumulator
-      tc::fence_after();
       tc_put_row64(a_hi, a_lo, tid, v);
     }
     // ---- gi = x2 . W_ih^T + b_ih ----
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
-    tc::issue_layer(tmem_base, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, swap_ls, bar);
+    tc::mma(acc, 0, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, 0);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_after();
     float* gi = a.gi[net];
 #pragma unroll 1
     for (int c0 = 0; c0 < MX_G; c0 += 64) {
       float t0[64];
-      tc::tmem_ld64(tmem_row + c0, t0);
+      tc::ld_row(acc, c0, tid, t0);
       if (ok) {
 #pragma unroll
         for (int c4 = 0; c4 < 16; ++c4)
@@ -669,13 +628,8 @@ __global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, Fr
                           t0[4 * c4 + 3] + bih_s[c0 + 4 * c4 + 3]);
       }
     }
-    tc::fence_before();
     __syncthreads();     // accumulator reads drained; the A tile and the fc1 chunk buffer are free for the next tile
-    tc::fence_after();
   }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
 // =====================================================================================================
@@ -696,12 +650,11 @@ __device__ __forceinline__ void tcw_stage(char* dst, const float* __restrict__ s
   float* d = reinterpret_cast<float*>(dst);
   for (int v = threadIdx.x; v < (nbytes >> 4); v += blockDim.x) mx_cp16(d + 4 * v, src + 4 * v);
 }
-__global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, FrontTcWide2Smem sm, int swap_ls) {
+__global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, FrontTcWide2Smem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   __shared__ float par_s[6 * MX_H + MX_G + 2 * 128];      // b1,g1,be1,b2,g2,be2 | b_ih | feature-norm gain, bias
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int net = blockIdx.y;
   const float* __restrict__ th = a.theta[net];
   const MxNetLayout L = a.L;
@@ -710,7 +663,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
   char* base = reinterpret_cast<char*>(smem_raw);
   char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo, *wc = base + sm.o_wc;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<256>(&tmem_s, tc::cta_slice(a.tc_acc, 256));
+  float* acc = tc::cta_slice(a.tc_acc, 256);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -730,11 +683,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
   const float* img_c1 = img + 2 * 64 * 64;
   const float* img_w2 = img + 2 * 64 * Kp;
   const float* img_wih = img_w2 + 2 * 4096;
-  tc::fence_before();
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_base = tmem_s;
-  const uint32_t tmem_row = tmem_base + ((uint32_t)(warp * 32) << 16);
   uint32_t phase = 0;
   const int ntiles = (a.M + 127) / 128;
   const int I4 = (I + 3) >> 2;
@@ -805,13 +754,11 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       }
       mx_cp_wait<0>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer_acc(tmem_base, a_hi, a_lo, wc, wc + 64 * Kc * 4, MX_H, Kc, swap_ls, ch > 0 ? 1u : 0u, bar);
+      tc::mma(acc, 0, a_hi, a_lo, wc, wc + 64 * Kc * 4, MX_H, Kc, 3, ch > 0 ? 1u : 0u);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);        // the MMAs have read the A tile and the chunk buffer: both may be refilled
       phase ^= 1;
-      tc::fence_after();
       if (ch == 0) tcw_stage(wc, img_c1, 2 * 64 * Kc1 * 4); else tcw_stage(wc, img_w2, 2 * 4096 * 4);
       mx_cp_commit();
     }
@@ -820,18 +767,16 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       if (layer == 1) {
         mx_cp_wait<0>();
         tc::fence_async_smem();
-        tc::fence_before();
         __syncthreads();
-        tc::fence_after();
-        tc::issue_layer(tmem_base, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
+        tc::mma(acc, 0, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, 0);
+        tc::arrive(bar);
         tc::mbar_wait(bar, phase);
         phase ^= 1;
-        tc::fence_after();
         tcw_stage(wc, img_wih, 4096 * 4); tcw_stage(wc + 4096 * 4, img_wih + 3 * 4096, 4096 * 4);      // gate r: hi | lo
         mx_cp_commit();
       }
       float v[64];
-      tc::tmem_ld64(tmem_row, v);
+      tc::ld_row(acc, 0, tid, v);
       const float* bs = par_s + layer * 3 * MX_H;
 #pragma unroll
       for (int c = 0; c < 64; ++c) { const float z = v[c] + bs[c]; v[c] = a.act_tanh ? tanhf(z) : fmaxf(z, 0.f); }
@@ -846,9 +791,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
       }
 #pragma unroll
       for (int c = 0; c < 64; ++c) v[c] = (v[c] - mu) * rs * bs[MX_H + c] + bs[2 * MX_H + c];
-      tc::fence_before();
       __syncthreads();          // every thread has drained its accumulator reads before the next layer's MMAs overwrite the accumulator
-      tc::fence_after();
       tc_put_row64(a_hi, a_lo, tid, v);
     }
     // ---- gi = x2 . W_ih^T + b_ih, one gate block (64 columns) at a time into accumulator columns 64 + 64 g ----
@@ -857,13 +800,11 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
     for (int g = 0; g < 3; ++g) {
       mx_cp_wait<0>();
       tc::fence_async_smem();
-      tc::fence_before();
       __syncthreads();
-      tc::fence_after();
-      tc::issue_layer(tmem_base + 64 + 64 * g, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, swap_ls, bar);
+      tc::mma(acc, 64 + 64 * g, a_hi, a_lo, wc, wc + 4096 * 4, MX_H, MX_H, 3, 0);
+      tc::arrive(bar);
       tc::mbar_wait(bar, phase);
       phase ^= 1;
-      tc::fence_after();
       if (g < 2) {
         tcw_stage(wc, img_wih + (g + 1) * 4096, 4096 * 4); tcw_stage(wc + 4096 * 4, img_wih + (3 + g + 1) * 4096, 4096 * 4);
         mx_cp_commit();
@@ -872,7 +813,7 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
         mx_cp_commit();
       }
       float t0[64];
-      tc::tmem_ld64(tmem_row + 64 + 64 * g, t0);
+      tc::ld_row(acc, 64 + 64 * g, tid, t0);
       if (ok) {
         const int c0 = 64 * g;
 #pragma unroll
@@ -882,14 +823,9 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
                           t0[4 * c4 + 3] + bih_s[c0 + 4 * c4 + 3]);
       }
     }
-    tc::fence_before();
     __syncthreads();     // accumulator reads drained; the A tile is free for the next tile
-    tc::fence_after();
   }
   mx_cp_wait<0>();
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<256>(tmem_base);
 }
 
 int g_mx_front_tc = 1;        // 1: tensor-core 3xTF32 kernels (default), 0: FFMA kernel (mx_set_option("front_tc", 0))
@@ -897,7 +833,6 @@ int g_mx_front_tc_threads = 256;   // inputs <= 64: 256 = two threads per accumu
 int g_mx_front_tc_wide = 1;   // 1 (default): 64 < in_dim <= 128 also runs on the tensor cores (k_front_fwd_tc_wide[2])
 int g_mx_front_tc_wide2 = 1;  // wide inputs: 1 (default) = k_front_fwd_tc_wide2 (weights streamed, two CTAs per SM), 0 = k_front_fwd_tc_wide (weights resident, one CTA per SM)
                               // (these defaults are not yet measured on the H100)
-int g_mx_tc_swap = 0;
 extern int g_mx_wgrad_tc, g_mx_wgrad_tc_wide, g_mx_front_bwd_tc_stream;      // tc_bwd.cu
 int g_mx_mixer_rm = 0;        // tuning overrides (0 = automatic): rows per thread of the mixer / backward front tiles
 int g_mx_front_bwd_rm = 0;
@@ -933,7 +868,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
         configured_w2 = true;
       }
 #endif
-      MX_LAUNCH_PDL(k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, a, s2, g_mx_tc_swap);
+      MX_LAUNCH_PDL(k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, a, s2);
       MX_COUNT();
       MX_MARK("k_front_fwd_tc_wide", s);
       return MX_CHECK_LAUNCH("front_fwd_tc_wide2");
@@ -945,7 +880,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
       configured_w = true;
     }
 #endif
-    MX_LAUNCH_PDL(k_front_fwd_tc_wide, dim3(gx, nets), dim3(128), smem, s, a, sm, g_mx_tc_swap);
+    MX_LAUNCH_PDL(k_front_fwd_tc_wide, dim3(gx, nets), dim3(128), smem, s, a, sm);
     MX_COUNT();
     MX_MARK("k_front_fwd_tc_wide", s);
     return MX_CHECK_LAUNCH("front_fwd_tc_wide");
@@ -966,12 +901,12 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
       configured2 = smem;
     }
 #endif
-    MX_LAUNCH_PDL(k_front_fwd_tc2, dim3(gx, nets), dim3(256), smem, s, a, sm, g_mx_tc_swap);
+    MX_LAUNCH_PDL(k_front_fwd_tc2, dim3(gx, nets), dim3(256), smem, s, a, sm);
     MX_COUNT();
     MX_MARK("k_front_fwd_tc", s);
     return MX_CHECK_LAUNCH("front_fwd_tc2");
   }
-  MX_LAUNCH_PDL(k_front_fwd_tc, dim3(gx, nets), dim3(128), smem, s, a, sm, g_mx_tc_swap);
+  MX_LAUNCH_PDL(k_front_fwd_tc, dim3(gx, nets), dim3(128), smem, s, a, sm);
   MX_COUNT();
   MX_MARK("k_front_fwd_tc", s);
   return MX_CHECK_LAUNCH("front_fwd_tc");
@@ -986,7 +921,6 @@ extern "C" int mx_set_option(const char* name, int32_t value) {
   if (!strcmp(name, "wgrad_tc")) { g_mx_wgrad_tc = value; return 0; }
   if (!strcmp(name, "wgrad_tc_wide")) { g_mx_wgrad_tc_wide = value; return 0; }
   if (!strcmp(name, "front_bwd_tc_stream")) { g_mx_front_bwd_tc_stream = value; return 0; }
-  if (!strcmp(name, "tc_swap_ls")) { g_mx_tc_swap = value; return 0; }
   if (!strcmp(name, "mixer_rm")) { g_mx_mixer_rm = value; return 0; }
   if (!strcmp(name, "front_bwd_rm")) { g_mx_front_bwd_rm = value; return 0; }
 #if !MX_EMU
@@ -1007,7 +941,6 @@ struct TcProbeArgs {
 __global__ void __launch_bounds__(128) k_tc_linear_probe(TcProbeArgs a) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ uint32_t tmem_s;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = a.K, N = a.N;
   char* a_hi = reinterpret_cast<char*>(smem_raw);
@@ -1017,7 +950,6 @@ __global__ void __launch_bounds__(128) k_tc_linear_probe(TcProbeArgs a) {
   float* acc = reinterpret_cast<float*>(b_lo + 64 * K * 4);      // [64 columns][128 rows]
   const int m0 = blockIdx.x * 128;
   const uint32_t bar = tc::bar_addr(&bar_s);
-  if (warp == 0) tc::tmem_alloc<64>(&tmem_s, acc);
   if (tid == 0) {
     tc::mbar_init(bar, blockDim.x);
     tc::mbar_init_fence();
@@ -1037,25 +969,19 @@ __global__ void __launch_bounds__(128) k_tc_linear_probe(TcProbeArgs a) {
       tc::put_split(b_hi, b_lo, r, k, K, a.W[(size_t)(n0 + r) * K + k]);
     }
     tc::fence_async_smem();
-    tc::fence_before();
     __syncthreads();
-    tc::fence_after();
-    const uint32_t tmem_base = tmem_s;
-    tc::issue_layer(tmem_base, a_hi, a_lo, b_hi, b_lo, nc, K, a.passes, a.swap_ls, bar);
+    tc::mma(acc, 0, a_hi, a_lo, b_hi, b_lo, nc, K, a.passes, 0, a.swap_ls);
+    tc::arrive(bar);
     tc::mbar_wait(bar, phase);
     phase ^= 1;
-    tc::fence_after();
     for (int c0 = 0; c0 < nc; c0 += 32) {
       float v[32];
-      tc::tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
+      tc::ld_row(acc, c0, tid, v);
       if (row < a.M)
         for (int c = 0; c < 32 && c0 + c < nc; ++c) a.Y[(size_t)row * N + n0 + c0 + c] = v[c];
     }
-    tc::fence_before();
     __syncthreads();      // accumulator reads done before the next block's MMAs overwrite it; B block free
-    tc::fence_after();
   }
-  if (warp == 0) tc::tmem_dealloc<64>(tmem_s);
 }
 
 extern "C" int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int32_t N, int32_t K, int32_t passes, int32_t swap_ls,

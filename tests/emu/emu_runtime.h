@@ -9,7 +9,7 @@
 // Model: blocks run one after another; the threads of a block are fibers (own stacks, cooperative switch) scheduled round-robin
 // (or in reverse / pseudo-random order, EMU_ORDER=reverse|random, to shake out missing barriers);
 // __syncthreads / warp collectives are cooperative barriers.  `__shared__` becomes `static` (valid
-// because blocks are sequential).  tcgen05 / TMEM / mbarrier are restated in csrc/mx_tc.cuh's MX_EMU half; TMA and clusters are not emulated.
+// because blocks are sequential).  wgmma and mbarrier are restated in csrc/mx_tc.cuh's MX_EMU half; TMA and clusters are not emulated.
 #pragma once
 #include <ucontext.h>
 

@@ -1,4 +1,4 @@
-"""Seeded random shapes x options: the QMIX step (all kernel variants: FFMA / tcgen05 forward incl. wide inputs, FFMA / tensor-core
+"""Seeded random shapes x options: the QMIX step (all kernel variants: FFMA / tensor-core forward incl. wide inputs, FFMA / tensor-core
 backward modes, PER, Huber, no double-Q, previous-action input) in lock-step with the oracle on the CPU emulator.  A wider sweep of the same
 generator (150 configurations over four seeds) was run once when the tensor-core backward was written; this keeps a slice of it in the suite."""
 import random

@@ -211,7 +211,7 @@ def test_recurrence_kernel_128_threads_maddpg(emu_engine, name):
 
 @pytest.mark.parametrize("threads", [128, 256])
 @pytest.mark.parametrize("name", ["qmix_small", "qmix_small_prev_act", "qmix_small_tanh"])
-def test_front_tcgen05_kernel_variants_match_reference_golden(emu_engine, name, threads):
+def test_front_tensor_core_kernel_variants_match_reference_golden(emu_engine, name, threads):
     """k_front_fwd_tc (one thread per accumulator row) and k_front_fwd_tc2 (two threads per row, pair-wise LayerNorm statistics): option
     front_tc_threads, default 256."""
     lib = emu_engine.lib()

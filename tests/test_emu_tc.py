@@ -1,6 +1,7 @@
-"""tcgen05 kernels on the CPU emulator (tests/emu + csrc/mx_tc.cuh's restated primitives): the emulation decodes shared-memory descriptors
-with the convention the B200 runs validated (tests/test_gpu_tc.py), so these tests check the kernels' INDEXING -- operand tiles, descriptor
-strides, TMEM lanes / columns, barrier phases -- without a GPU.  Async-proxy ordering is outside what an emulator can see."""
+"""Tensor-core (wgmma) kernels on the CPU emulator (tests/emu + csrc/mx_tc.cuh's restated instructions): the emulated wgmma decodes
+shared-memory descriptors with the convention the GPU runs validated (tests/test_gpu_tc.py) and fills each thread's own fragment registers,
+so these tests run the kernels' INDEXING -- operand tiles, descriptor strides, the warpgroups' tile dealing, fragment placement in the
+per-CTA accumulator slices, mbarrier arrivals -- without a GPU.  Async-proxy ordering is outside what an emulator can see."""
 import numpy as np
 import pytest
 import torch
@@ -41,7 +42,7 @@ def test_qmix_step_front_paths_match_reference_golden(emu_engine, front_tc):
 @pytest.mark.parametrize("obs_dim", [65, 80, 100, 128])
 def test_wide_input_front_kernel_vs_oracle(emu_engine, obs_dim):
     """64 < obs_dim <= 128 (SMAC 8m / 2s3z observations are 80 wide): fc1's K dimension fed to the tensor core in two chunks that
-    accumulate in TMEM (k_front_fwd_tc_wide, option front_tc_wide).  More than 128 rows so a CTA runs several tiles."""
+    accumulate in the accumulator (k_front_fwd_tc_wide, option front_tc_wide).  More than 128 rows so a CTA runs several tiles."""
     from oracle.qmix import QmixConfig, synth_batch
     lib = emu_engine.lib()
     cfg = QmixConfig(n_agents=5, obs_dim=obs_dim, act_dim=6, state_dim=20, gain=1.0)
@@ -83,7 +84,7 @@ def test_wide_input_kernel_is_what_runs(emu_engine):
 @pytest.mark.parametrize("name", ["qmix_small", "qmix_5ag", "qmix_small_prev_act", "qmix_small_per", "qmix_small_huber_nodq", "qmix_small_hyper1"])
 def test_tensor_core_weight_gradients_match_reference_golden(emu_engine, name, mode):
     """Option wgrad_tc.  1: k_wgrad_tc produces every dW / db of the front layers and the GRU matrices, the LayerNorm gradients and the
-    data-gradient chain still come from k_front_bwd.  2: k_front_bwd_tc (data-gradient chain + LayerNorm gradients on tcgen05) replaces
+    data-gradient chain still come from k_front_bwd.  2: k_front_bwd_tc (data-gradient chain + LayerNorm gradients on the tensor cores) replaces
     k_front_bwd altogether.  All gradient tensors against the reference's."""
     lib = emu_engine.lib()
     lib.mx_set_option(b"wgrad_tc", mode)
@@ -129,7 +130,7 @@ def test_tensor_core_backward_mlp_variant_matches_reference_golden(emu_engine, n
 @pytest.mark.parametrize("obs_dim", [65, 80, 96, 112, 128])
 def test_tensor_core_backward_wide_inputs_vs_oracle(emu_engine, obs_dim, mode):
     """64 < obs_dim <= 128 through the tensor-core backward (fc1's transposed weight image takes turns with fc2's in shared memory, the
-    feature LayerNorm's gradients are summed in two 64-column rounds, dW1 is read from two 64-column blocks of TMEM), together with the
+    feature LayerNorm's gradients are summed in two 64-column rounds, dW1 is read from two 64-column blocks of the accumulator), together with the
     wide forward kernel."""
     from oracle.qmix import QmixConfig, synth_batch
     lib = emu_engine.lib()

@@ -1,4 +1,4 @@
-"""tcgen05 (5th-gen tensor core) path: the 3xTF32 building block against fp64, then the whole QMIX step with the
+"""Tensor-core (wgmma) path: the 3xTF32 building block against fp64, then the whole QMIX step with the
 time-batched front layers routed through k_front_fwd_tc, against the reference goldens and the oracle."""
 import numpy as np
 import pytest
@@ -40,7 +40,7 @@ def test_3xtf32_building_block_matches_fp64(gpu_engine):
 @pytest.mark.parametrize("front_tc", [1, 0])
 @pytest.mark.parametrize("name", ["qmix_small", "qmix_5ag"])
 def test_qmix_step_front_paths_match_reference_golden(gpu_engine, name, front_tc):
-    """The tcgen05 front kernel is the default; the FFMA kernel stays selectable and both must hold parity."""
+    """The tensor-core front kernel is the default; the FFMA kernel stays selectable and both must hold parity."""
     lib = gpu_engine.lib()
     assert detect_swap(gpu_engine) == 0          # the convention compiled in as the default
     lib.mx_set_option(b"front_tc", front_tc)
@@ -50,7 +50,7 @@ def test_qmix_step_front_paths_match_reference_golden(gpu_engine, name, front_tc
         lib.mx_set_option(b"front_tc", 1)
 
 
-def test_config2_full_size_with_tcgen05_front_vs_oracle(gpu_engine):
+def test_config2_full_size_with_tensor_core_front_vs_oracle(gpu_engine):
     from test_gpu_qmix import _oracle_and_trainer, _compare_step
     from oracle.qmix import QmixConfig, synth_batch
     lib = gpu_engine.lib()

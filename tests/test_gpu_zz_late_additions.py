@@ -9,7 +9,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("debug", [True, False])
 def test_prev_act_inp_matches_reference_golden(gpu_engine, debug):
-    """--prev_act_inp: input width 30 + 9 = 39 (tcgen05 front kernel with K padded to 40)."""
+    """--prev_act_inp: input width 30 + 9 = 39 (tensor-core front kernel with K padded to 40)."""
     qc.check_step_against(None, "qmix_small_prev_act", intermediates=False, debug=debug)
 
 
@@ -31,7 +31,7 @@ def test_mlp_buffer_sample_layout(gpu_engine):
                          ids=["mpe_b1000", "avail_per_huber", "avail_nodq", "vdn", "hyper1_2s3z_shapes"])
 def test_mlp_learner_vs_oracle(gpu_engine, kw):
     """scripts/train_mpe_mqmix.sh sizes (batch 1000 transitions) in lock-step with the pinned oracle (oracle/mqmix.py); obs 80 takes the
-    FFMA front kernel (obs_dim > 64), obs 18 the tcgen05 one."""
+    FFMA front kernel (obs_dim > 64), obs 18 the tensor-core one."""
     import mqmix_checks as mc
     mc.check_vs_oracle(steps=2, **kw)
 
@@ -61,7 +61,7 @@ def test_c_host_example_runs(gpu_engine, tmp_path):
 @pytest.mark.parametrize("front_tc", [1, 0])
 @pytest.mark.parametrize("name", ["qmix_small_nofn", "qmix_small_tanh"])
 def test_network_structure_flags_match_reference_golden(gpu_engine, name, front_tc):
-    """--use_feature_normalization / --use_ReLU switched off (store_false flags): no input LayerNorm, tanh blocks -- tcgen05 and FFMA front."""
+    """--use_feature_normalization / --use_ReLU switched off (store_false flags): no input LayerNorm, tanh blocks -- tensor-core and FFMA front."""
     lib = gpu_engine.lib()
     lib.mx_set_option(b"front_tc", front_tc)
     try:
@@ -87,7 +87,7 @@ def test_network_structure_flags_maddpg(gpu_engine, name):
 # ---- option-gated tensor-core kernels written without a GPU (off by default): last, so that a failure here hides nothing else ----
 
 @pytest.mark.parametrize("obs_dim,n_agents,B,T", [(80, 8, 8, 20), (128, 3, 16, 12), (72, 5, 32, 10)])
-def test_wide_input_tcgen05_front_kernel_vs_oracle(gpu_engine, obs_dim, n_agents, B, T):
+def test_wide_input_tensor_core_front_kernel_vs_oracle(gpu_engine, obs_dim, n_agents, B, T):
     """k_front_fwd_tc_wide (64 < obs_dim <= 128, option front_tc_wide, off by default until timed): emulator-verified indexing; this is its
     first run on real tensor cores.  Runs under a launch-count check that the wide kernel, not the FFMA one, executed."""
     import ctypes as C
@@ -114,7 +114,7 @@ def test_wide_input_tcgen05_front_kernel_vs_oracle(gpu_engine, obs_dim, n_agents
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("name", ["qmix_small", "qmix_5ag", "qmix_small_per"])
 def test_tensor_core_weight_gradients_match_reference_golden(gpu_engine, name, mode):
-    """Option wgrad_tc (off by default until timed).  1: k_wgrad_tc -- dW / db of the front layers and the GRU matrices on tcgen05 with
+    """Option wgrad_tc (off by default until timed).  1: k_wgrad_tc -- dW / db of the front layers and the GRU matrices on the tensor cores with
     transposed operand staging, beside k_front_bwd's data-gradient chain.  2: k_front_bwd_tc replaces k_front_bwd as well.
     Emulator-verified indexing; first run on real tensor cores here."""
     lib = gpu_engine.lib()
