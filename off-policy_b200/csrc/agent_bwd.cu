@@ -15,24 +15,26 @@
 // =====================================================================================================
 // Q head backward (one warp per row-step)
 // =====================================================================================================
-// Shared memory: wq[A][64] | per-warp private accumulators dW[8][A][64], db[8][32], dgamma[8][64], dbeta[8][64].  Only the owning
-// warp touches its slice while rows are processed (no atomics); the CTA's partial is the sum over the 8 warps in fixed order,
-// so the step is run-to-run deterministic.
-static inline size_t qhead_bwd_smem(int A) { return (size_t)(A * MX_H * 9 + 8 * 32 + 2 * 8 * MX_H + 2 * MX_H) * sizeof(float); }
+// Shared memory: wq[A][64] | per-warp private accumulators dW[8][A][64], db[8][32 APL], dgamma[8][64], dbeta[8][64] (APL: 1 for
+// A <= 32, 2 for A <= 64).  Only the owning warp touches its slice while rows are processed (no atomics); the CTA's partial is the
+// sum over the 8 warps in fixed order, so the step is run-to-run deterministic.
+static inline size_t qhead_bwd_smem(int A, int APL) { return (size_t)(A * MX_H * 9 + 8 * 32 * APL + 2 * 8 * MX_H + 2 * MX_H) * sizeof(float); }
 
+template <int APL>
 __global__ void __launch_bounds__(256) k_qhead_bwd(QHeadBwdArgs a) {
+  constexpr int AR = 32 * APL;
   MX_DYN_SMEM(smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int A = a.A, AW = A * MX_H;
   float* wq_s = smem;
   float* dw_w = wq_s + AW;               // [8][A*64]
-  float* db_w = dw_w + 8 * AW;           // [8][32]
-  float* dg_w = db_w + 8 * 32;           // [8][64]
+  float* db_w = dw_w + 8 * AW;           // [8][32 APL]
+  float* dg_w = db_w + 8 * AR;           // [8][64]
   float* dbt_w = dg_w + 8 * MX_H;        // [8][64]
   float* lg_s = dbt_w + 8 * MX_H;
   float* lb_s = lg_s + MX_H;
   for (int i = tid; i < AW; i += blockDim.x) wq_s[i] = a.theta[a.wq + i];
-  for (int i = tid; i < 8 * AW + 8 * 32; i += blockDim.x) dw_w[i] = 0.f;      // dw_w and db_w are contiguous
+  for (int i = tid; i < 8 * AW + 8 * AR; i += blockDim.x) dw_w[i] = 0.f;      // dw_w and db_w are contiguous
   for (int i = tid; i < MX_H; i += blockDim.x) { lg_s[i] = a.theta[a.lno_g + i]; lb_s[i] = a.theta[a.lno_b + i]; }
   MX_PDL_WAIT();
   __syncthreads();
@@ -60,7 +62,7 @@ __global__ void __launch_bounds__(256) k_qhead_bwd(QHeadBwdArgs a) {
     const float dy0 = dqv * wq_s[act * MX_H + lane], dy1 = dqv * wq_s[act * MX_H + lane + 32];
     my_dw[act * MX_H + lane] += dqv * y0;
     my_dw[act * MX_H + lane + 32] += dqv * y1;
-    if (lane == 0) db_w[warp * 32 + act] += dqv;
+    if (lane == 0) db_w[warp * AR + act] += dqv;
     dg0 += dy0 * xh0; dg1 += dy1 * xh1; db0 += dy0; db1 += dy1;
     // LayerNorm backward
     const float dx0 = dy0 * lg_s[lane], dx1 = dy1 * lg_s[lane + 32];
@@ -82,7 +84,7 @@ __global__ void __launch_bounds__(256) k_qhead_bwd(QHeadBwdArgs a) {
   for (int i = tid; i < A; i += blockDim.x) {
     float v = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) v += db_w[w * 32 + i];
+    for (int w = 0; w < 8; ++w) v += db_w[w * AR + i];
     gp[a.bq + i] = v;
   }
   for (int i = tid; i < MX_H; i += blockDim.x) {
@@ -840,20 +842,27 @@ __global__ void __launch_bounds__(MX_TILE_THREADS, 2) k_gru_wgrad(FrontBwdArgs a
 // =====================================================================================================
 // launchers
 // =====================================================================================================
+template <int APL>
+static int qhead_bwd_launch(const QHeadBwdArgs& a, int grid, cudaStream_t s) {
+  const size_t smem = qhead_bwd_smem(a.A, APL);
+#if !MX_EMU
+  static size_t configured = 0;
+  if (smem > 48 * 1024 && smem > configured) {
+    if (cudaFuncSetAttribute(k_qhead_bwd<APL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("qhead_bwd: smem %zu too large", smem); return 1; }
+    configured = smem;
+  }
+#endif
+  MX_LAUNCH_PDL(k_qhead_bwd<APL>, dim3(grid), dim3(256), smem, s, a);
+  return 0;
+}
+
 int mx_launch_qhead_bwd(const QHeadBwdArgs& a, int* nparts_used, cudaStream_t s) {
+  if (a.A > 64) { mx_set_error("qhead_bwd: act_dim %d > 64 unsupported", a.A); return 1; }
   int grid = mx_ceil_div(a.M, 8 * 4);   // ~4 rows per warp
   const int cap = mx_num_sms();
   if (grid > cap) grid = cap;
   if (grid < 1) grid = 1;
-  const size_t smem = qhead_bwd_smem(a.A);
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > 48 * 1024 && smem > configured) {
-    if (cudaFuncSetAttribute(k_qhead_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("qhead_bwd: smem %zu too large", smem); return 1; }
-    configured = smem;
-  }
-#endif
-  MX_LAUNCH_PDL(k_qhead_bwd, dim3(grid), dim3(256), smem, s, a);
+  if (a.A > 32 ? qhead_bwd_launch<2>(a, grid, s) : qhead_bwd_launch<1>(a, grid, s)) return 1;
   MX_COUNT();
   MX_MARK("k_qhead_bwd", s);
   *nparts_used = grid;

@@ -391,11 +391,13 @@ __global__ void __launch_bounds__(GRU2_THREADS, 2) k_gru_fwd2(GruFwdArgs a) {
 }
 
 // =====================================================================================================
-// Q head + action selection (one warp per row-step)
+// Q head + action selection (one warp per row-step).  APL: availability bits per lane (1: A <= 32, 2: A <= 64, lane l holds
+// actions l and l + 32)
 // =====================================================================================================
+template <int APL>
 __global__ void __launch_bounds__(256) k_qhead(QHeadArgs a) {
-  __shared__ float wq_s[2][32 * MX_H];   // A <= 32
-  __shared__ float bq_s[2][32];
+  __shared__ float wq_s[2][32 * APL * MX_H];   // A <= 32 * APL
+  __shared__ float bq_s[2][32 * APL];
   __shared__ float lg_s[2][MX_H], lb_s[2][MX_H];
   const int tid = threadIdx.x, lane = tid & 31;
   const int A = a.A;
@@ -424,6 +426,12 @@ __global__ void __launch_bounds__(256) k_qhead(QHeadArgs a) {
     float av = 1.f;
     if (a.avail && lane < A) av = a.avail[(size_t)m * a.act_ld + lane];
     const unsigned avail_mask = __ballot_sync(0xffffffffu, av != 0.f);
+    unsigned avail_hi = 0u;                                                      // actions 32..63
+    if constexpr (APL == 2) {
+      float av2 = 1.f;
+      if (a.avail && lane + 32 < A) av2 = a.avail[(size_t)m * a.act_ld + lane + 32];
+      avail_hi = __ballot_sync(0xffffffffu, av2 != 0.f);
+    }
     // ---------------- live ----------------
     {
       const float mean = mx_warp_sum(hl0 + hl1) * (1.f / MX_H);
@@ -437,7 +445,10 @@ __global__ void __launch_bounds__(256) k_qhead(QHeadArgs a) {
         float q = mx_warp_sum(y0 * wq_s[0][k * MX_H + lane] + y1 * wq_s[0][k * MX_H + lane + 32]) + bq_s[0][k];
         if (a.qall0 && lane == 0) a.qall0[(size_t)m * A + k] = q;
         if (k == act) q_live_at_act = q;
-        const float qm = ((avail_mask >> k) & 1u) ? q : -1e10f;                 // util.py:297-302
+        unsigned on;
+        if constexpr (APL == 1) on = (avail_mask >> k) & 1u;
+        else on = ((k < 32 ? avail_mask : avail_hi) >> (k & 31)) & 1u;
+        const float qm = on ? q : -1e10f;                                        // util.py:297-302
         if (k == 0 || qm > best) { best = qm; greedy = k; }                     // first maximum wins
       }
     }
@@ -599,11 +610,12 @@ int mx_launch_gru_fwd(const GruFwdArgs& a, int nets, cudaStream_t s) {
 }
 
 int mx_launch_qhead(const QHeadArgs& a, cudaStream_t s) {
-  if (a.A > 32) { mx_set_error("qhead: act_dim %d > 32 unsupported", a.A); return 1; }
+  if (a.A > 64) { mx_set_error("qhead: act_dim %d > 64 unsupported", a.A); return 1; }
   int grid = mx_ceil_div(a.M, 8);
   const int cap = mx_num_sms() * 4;
   if (grid > cap) grid = cap;
-  MX_LAUNCH_PDL(k_qhead, dim3(grid), dim3(256), 0, s, a);
+  if (a.A > 32) MX_LAUNCH_PDL(k_qhead<2>, dim3(grid), dim3(256), 0, s, a);
+  else MX_LAUNCH_PDL(k_qhead<1>, dim3(grid), dim3(256), 0, s, a);
   MX_COUNT();
   MX_MARK("k_qhead", s);
   return MX_CHECK_LAUNCH("qhead");

@@ -6,7 +6,8 @@
 //
 // One warp per (b, t) element: the N agents of an element are N consecutive rows m = (b (T+1) + t) N + n, so everything the
 // element needs (q_taken[n], q_next[n], dq_taken[n]) stays in the warp's registers.  The head is evaluated with one lane per
-// action (two half-dot-products per action when A <= 16) on the LayerNorm output parked in a per-warp shared-memory row, so a
+// action (two half-dot-products per action when A <= 16; two actions per lane, k = lane and lane + 32, when 32 < A <= 64: the
+// APL = 2 instantiation) on the LayerNorm output parked in a per-warp shared-memory row, so a
 // 9-action head costs ~35 FMAs + 1 shuffle per lane instead of 9 five-step warp reductions.  The live head is evaluated twice per
 // row (as "t" for the taken action, as "t+1" for the double-Q arg-max): 64 x A MACs, cheaper than a round trip through memory.
 // Head-weight gradients accumulate in per-warp private shared-memory slices and are summed over the warps in fixed order
@@ -23,19 +24,21 @@
 MX_DEVINL int mid_col(int j) { return j + (j >> 5); }
 
 struct MidSmem { int o_wq, o_bq, o_ln, o_y, o_dw, o_db, o_dg, o_stage, stage_ld, total; };
-static MidSmem mid_smem(int A, int N, int gP, int gM, int MID_WARPS) {
+// APL: actions per lane (1: A <= 32, 2: A <= 64); the head, bias, availability and bias-gradient tiles have 32 * APL rows
+static MidSmem mid_smem(int A, int N, int gP, int gM, int MID_WARPS, int APL) {
   MidSmem s;
+  const int AR = 32 * APL;
   int o = 0;
-  s.o_wq = o; o += 2 * 32 * MID_WLD;            // [net][32][65]
-  s.o_bq = o; o += 2 * 32;
+  s.o_wq = o; o += 2 * AR * MID_WLD;            // [net][32 APL][65]
+  s.o_bq = o; o += 2 * AR;
   s.o_ln = o; o += 4 * MX_H;                    // live gamma, beta, target gamma, beta
   s.o_y = o; o += MID_WARPS * MID_YLD;          // per-warp LayerNorm output row (gapped)
   s.o_dw = o; o += MID_WARPS * A * MX_H;        // per-warp private dWq
-  s.o_db = o; o += MID_WARPS * 32;              // per-warp private dbq
+  s.o_db = o; o += MID_WARPS * AR;              // per-warp private dbq
   s.o_dg = o; o += 2 * MID_WARPS * MX_H;        // per-warp d gamma, d beta
   // per-warp operand staging (cp.async at the top of an element, ONE exposed L2 latency instead of one per agent and per mixer term):
-  // h rows [live t | live t+1 | target t+1][N][64], mixer hypernet outputs p1[2][gP], b1[2][gM], p2[2][gM], availability [N][32]
-  s.stage_ld = (3 * N * MX_H + 2 * gP + 4 * gM + N * 32 + 3) & ~3;
+  // h rows [live t | live t+1 | target t+1][N][64], mixer hypernet outputs p1[2][gP], b1[2][gM], p2[2][gM], availability [N][32 APL]
+  s.stage_ld = (3 * N * MX_H + 2 * gP + 4 * gM + N * AR + 3) & ~3;
   s.o_stage = o; o += MID_WARPS * s.stage_ld;
   s.total = o;
   return s;
@@ -73,6 +76,29 @@ MX_DEVINL float mid_head(const float* ys, const float* wq, const float* bq, int 
   return q;
 }
 
+// 32 < A <= 64: q_k for k = lane (qa) and k = lane + 32 (qb, 0 when k >= A), same summation order as the one-action path
+MX_DEVINL void mid_head2(const float* ys, const float* wq, const float* bq, int A, int lane, float& qa, float& qb) {
+  const int kb = lane + 32;
+  const float* wa = wq + lane * MID_WLD;
+  const float* wb = wq + (kb < A ? kb : 0) * MID_WLD;
+  float s0 = 0.f, s1 = 0.f, t0 = 0.f, t1 = 0.f;
+#pragma unroll
+  for (int j = 0; j < MX_H; j += 2) {
+    const float y0 = ys[mid_col(j)], y1 = ys[mid_col(j + 1)];
+    s0 = fmaf(y0, wa[mid_col(j)], s0); s1 = fmaf(y1, wa[mid_col(j + 1)], s1);
+    t0 = fmaf(y0, wb[mid_col(j)], t0); t1 = fmaf(y1, wb[mid_col(j + 1)], t1);
+  }
+  qa = (s0 + s1) + bq[lane];
+  qb = kb < A ? (t0 + t1) + bq[kb] : 0.f;
+}
+
+// the value of action k, held by lane k & 31 as lo (k < 32) or hi (k >= 32); every lane returns it
+template <int APL>
+MX_DEVINL float mid_pick(float lo, float hi, int k) {
+  if constexpr (APL == 1) return __shfl_sync(0xffffffffu, lo, k);
+  else return __shfl_sync(0xffffffffu, k < 32 ? lo : hi, k & 31);
+}
+
 // arg-max with "first maximum wins" over lanes k < A (value v in lane k); every lane returns the winner
 MX_DEVINL void mid_argmax(float v, int A, int lane, float& best, int& idx) {
   float bv = lane < A ? v : -3.0e38f;
@@ -86,9 +112,25 @@ MX_DEVINL void mid_argmax(float v, int A, int lane, float& best, int& idx) {
   best = bv; idx = bi;
 }
 
-template <int MID_WARPS>
+// the same over 32 < A <= 64 actions, va for k = lane and vb for k = lane + 32: the lane keeps its lower action on a tie, then the
+// warp reduction prefers the lower index, so the first maximum still wins
+MX_DEVINL void mid_argmax2(float va, float vb, int A, int lane, float& best, int& idx) {
+  float bv = va;
+  int bi = lane;
+  if (lane + 32 < A && vb > bv) { bv = vb; bi = lane + 32; }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  best = bv; idx = bi;
+}
+
+template <int MID_WARPS, int APL>
 __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
   constexpr int MID_THREADS = 32 * MID_WARPS;
+  constexpr int AR = 32 * APL;                       // rows of the head / bias / availability tiles
   MX_DYN_SMEM(smem);
   const MxMixLayout L = a.mix.L;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -97,20 +139,20 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
   float* wq_s = smem + sm.o_wq; float* bq_s = smem + sm.o_bq; float* ln_s = smem + sm.o_ln;
   float* ys = smem + sm.o_y + warp * MID_YLD;
   float* my_dw = smem + sm.o_dw + warp * A * MX_H;
-  float* my_db = smem + sm.o_db + warp * 32;
+  float* my_db = smem + sm.o_db + warp * AR;
   float* stg = smem + sm.o_stage + warp * sm.stage_ld;
   for (int net = 0; net < 2; ++net) {
     const float* th = net ? a.mix.theta_tgt : a.mix.theta;
-    for (int i = tid; i < A * MX_H; i += MID_THREADS) wq_s[net * 32 * MID_WLD + (i / MX_H) * MID_WLD + mid_col(i % MX_H)] = th[a.wq + i];
-    for (int i = tid; i < 32; i += MID_THREADS) bq_s[net * 32 + i] = i < A ? th[a.bq + i] : 0.f;
+    for (int i = tid; i < A * MX_H; i += MID_THREADS) wq_s[net * AR * MID_WLD + (i / MX_H) * MID_WLD + mid_col(i % MX_H)] = th[a.wq + i];
+    for (int i = tid; i < AR; i += MID_THREADS) bq_s[net * AR + i] = i < A ? th[a.bq + i] : 0.f;
     for (int i = tid; i < MX_H; i += MID_THREADS) { ln_s[net * 2 * MX_H + i] = th[a.lno_g + i]; ln_s[net * 2 * MX_H + MX_H + i] = th[a.lno_b + i]; }
   }
   for (int i = tid; i < MID_WARPS * A * MX_H; i += MID_THREADS) smem[sm.o_dw + i] = 0.f;
-  for (int i = tid; i < MID_WARPS * 32; i += MID_THREADS) smem[sm.o_db + i] = 0.f;
+  for (int i = tid; i < MID_WARPS * AR; i += MID_THREADS) smem[sm.o_db + i] = 0.f;
   MX_PDL_WAIT();
   __syncthreads();
   const float* lg = ln_s; const float* lb = ln_s + MX_H; const float* tg = ln_s + 2 * MX_H; const float* tb = ln_s + 3 * MX_H;
-  const float* wq0 = wq_s; const float* wq1 = wq_s + 32 * MID_WLD;
+  const float* wq0 = wq_s; const float* wq1 = wq_s + AR * MID_WLD;
   float den = 0.f, lsum = 0.f, qsum = 0.f;           // lane 0
   float dg0 = 0.f, dg1 = 0.f, db0 = 0.f, db1 = 0.f;   // LayerNorm gamma / beta gradients of this warp's rows
 
@@ -129,7 +171,7 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
     float* st_p1 = st_h + 3 * N * MX_H;                   // [2][gP]
     float* st_b1 = st_p1 + 2 * a.mix.gP;                  // [2][gM]
     float* st_p2 = st_b1 + 2 * a.mix.gM;                  // [2][gM]
-    float* st_av = st_p2 + 2 * a.mix.gM;                  // [N][32]
+    float* st_av = st_p2 + 2 * a.mix.gM;                  // [N][32 APL]
     {
       const int hv = N * (MX_H / 4);                      // 16-byte pieces per block of N rows (rows of a step are contiguous)
       const float* s0 = a.hall[0] + m0 * MX_H;
@@ -144,7 +186,9 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
         for (int i = lane; i < a.mix.gM / 4; i += 32) { mx_cp16(st_b1 + net * a.mix.gM + 4 * i, b1 + 4 * i); mx_cp16(st_p2 + net * a.mix.gM + 4 * i, p2 + 4 * i); }
       }
       if (a.avail && lane < A)
-        for (int n = 0; n < N; ++n) mx_cp4(st_av + n * 32 + lane, a.avail + (m0 + N + n) * a.act_ld + lane);
+        for (int n = 0; n < N; ++n) mx_cp4(st_av + n * AR + lane, a.avail + (m0 + N + n) * a.act_ld + lane);
+      if (APL == 2 && a.avail && lane + 32 < A)
+        for (int n = 0; n < N; ++n) mx_cp4(st_av + n * AR + lane + 32, a.avail + (m0 + N + n) * a.act_ld + lane + 32);
       mx_cp_commit();
     }
     const int act_l = lane < N ? a.act_idx[(size_t)b * a.ld_tn + (size_t)t * N + lane] : 0;       // lane n: taken action of agent n
@@ -157,29 +201,40 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
       const float* ht1 = st_h + (2 * N + n) * MX_H;
       const float h0a = hl[lane], h0b = hl[lane + 32], h1a = hl1[lane], h1b = hl1[lane + 32], g1a = ht1[lane], g1b = ht1[lane + 32];
       const int act = __shfl_sync(0xffffffffu, act_l, n);
-      float av = 1.f;
-      if (a.avail && lane < A) av = st_av[n * 32 + lane];
+      float av = 1.f, av2 = 1.f;                         // availability of actions lane and lane + 32
+      if (a.avail && lane < A) av = st_av[n * AR + lane];
+      if (APL == 2 && a.avail && lane + 32 < A) av2 = st_av[n * AR + lane + 32];
       float xh0, xh1, y0, y1, rstd;
+      // Q of actions lane (q) and lane + 32 (q_hi, APL = 2 only)
+      auto head = [&](const float* wq, const float* bq, float& q, float& q_hi) {
+        if constexpr (APL == 1) q = mid_head(ys, wq, bq, A, lane);
+        else mid_head2(ys, wq, bq, A, lane, q, q_hi);
+      };
       mid_ln(h0a, h0b, lg, lb, lane, xh0, xh1, y0, y1, rstd);
       ys[lane] = y0; ys[lane + 33] = y1;
       __syncwarp();
-      const float q_t = mid_head(ys, wq0, bq_s, A, lane);
-      const float q_taken = __shfl_sync(0xffffffffu, q_t, act);
+      float q_t, q_t_hi = 0.f;
+      head(wq0, bq_s, q_t, q_t_hi);
+      const float q_taken = mid_pick<APL>(q_t, q_t_hi, act);
       __syncwarp();
       mid_ln(h1a, h1b, lg, lb, lane, xh0, xh1, y0, y1, rstd);
       ys[lane] = y0; ys[lane + 33] = y1;
       __syncwarp();
-      const float q_t1 = mid_head(ys, wq0, bq_s, A, lane);
+      float q_t1, q_t1_hi = 0.f;
+      head(wq0, bq_s, q_t1, q_t1_hi);
       float gbest; int greedy;
-      mid_argmax(av != 0.f ? q_t1 : -1e10f, A, lane, gbest, greedy);          // util.py:297-302, first maximum wins
+      if constexpr (APL == 1) mid_argmax(av != 0.f ? q_t1 : -1e10f, A, lane, gbest, greedy);          // util.py:297-302, first maximum wins
+      else mid_argmax2(av != 0.f ? q_t1 : -1e10f, av2 != 0.f ? q_t1_hi : -1e10f, A, lane, gbest, greedy);
       __syncwarp();
       mid_ln(g1a, g1b, tg, tb, lane, xh0, xh1, y0, y1, rstd);
       ys[lane] = y0; ys[lane + 33] = y1;
       __syncwarp();
-      const float tq = mid_head(ys, wq1, bq_s + 32, A, lane);
+      float tq, tq_hi = 0.f;
+      head(wq1, bq_s + AR, tq, tq_hi);
       float q_next;
-      if (a.double_q) q_next = __shfl_sync(0xffffffffu, tq, greedy);
-      else { int dummy; mid_argmax(tq, A, lane, q_next, dummy); }              // plain max, no avail mask (qmix.py:144)
+      if (a.double_q) q_next = mid_pick<APL>(tq, tq_hi, greedy);
+      else if constexpr (APL == 1) { int dummy; mid_argmax(tq, A, lane, q_next, dummy); }              // plain max, no avail mask (qmix.py:144)
+      else { int dummy; mid_argmax2(tq, tq_hi, A, lane, q_next, dummy); }
       __syncwarp();
       if (lane == n) { qt_reg = q_taken; qn_reg = q_next; }
     }
@@ -301,7 +356,7 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
   for (int i = tid; i < A; i += MID_THREADS) {
     float v = 0.f;
 #pragma unroll
-    for (int wv = 0; wv < MID_WARPS; ++wv) v += db_all[wv * 32 + i];
+    for (int wv = 0; wv < MID_WARPS; ++wv) v += db_all[wv * AR + i];
     gp[a.bq + i] = v;
   }
   for (int i = tid; i < MX_H; i += MID_THREADS) {
@@ -312,33 +367,35 @@ __global__ void __launch_bounds__(32 * MID_WARPS) k_mid(MidArgs a, MidSmem sm) {
   }
 }
 
+static int mid_apl(const MidArgs& a) { return a.A > 32 ? 2 : 1; }
 static int mid_pick_warps(const MidArgs& a) {      // 0: does not fit even with 8 warps
   for (int w = MID_WARPS_MAX; w >= 8; w >>= 1) {
-    const MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, w);
+    const MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, w, mid_apl(a));
     if ((size_t)sm.total * sizeof(float) + 16 <= 220 * 1024) return w;
   }
   return 0;
 }
 int mx_mid_supported(const MidArgs& a) {
-  if (!(mx_mixer_split_supported(a.mix.L) && a.A <= 32 && a.N <= 32)) return 0;
+  if (!(mx_mixer_split_supported(a.mix.L) && a.A <= 64 && a.N <= 32)) return 0;
   return mid_pick_warps(a) != 0;          // the per-warp operand staging must fit
 }
 
-template <int W>
+template <int W, int APL>
 static int mid_launch(const MidArgs& a, int* parts_used, cudaStream_t s) {
   const int E = a.mix.B * a.T;
   int grid = mx_ceil_div(E, W);
   if (grid > mx_num_sms()) grid = mx_num_sms();
-  MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, W);
+  MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, W, APL);
   const size_t bytes = (size_t)sm.total * sizeof(float) + 16;
+  auto kern = k_mid<W, APL>;
 #if !MX_EMU
   static size_t configured = 0;
   if (bytes > 48 * 1024 && bytes > configured) {
-    if (cudaFuncSetAttribute(k_mid<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) { mx_set_error("mid: smem %zu too large", bytes); return 1; }
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) { mx_set_error("mid: smem %zu too large", bytes); return 1; }
     configured = bytes;
   }
 #endif
-  MX_LAUNCH_PDL(k_mid<W>, dim3(grid), dim3(32 * W), bytes, s, a, sm);
+  MX_LAUNCH_PDL(kern, dim3(grid), dim3(32 * W), bytes, s, a, sm);
   MX_COUNT();
   MX_MARK("k_mid", s);
   *parts_used = grid;
@@ -346,8 +403,13 @@ static int mid_launch(const MidArgs& a, int* parts_used, cudaStream_t s) {
 }
 int mx_launch_mid(const MidArgs& a, int* parts_used, cudaStream_t s) {
   const int w = mid_pick_warps(a);
-  if (w == 16) return mid_launch<16>(a, parts_used, s);
-  if (w == 8) return mid_launch<8>(a, parts_used, s);
+  if (a.A <= 32) {
+    if (w == 16) return mid_launch<16, 1>(a, parts_used, s);
+    if (w == 8) return mid_launch<8, 1>(a, parts_used, s);
+  } else if (a.A <= 64) {
+    if (w == 16) return mid_launch<16, 2>(a, parts_used, s);
+    if (w == 8) return mid_launch<8, 2>(a, parts_used, s);
+  }
   mx_set_error("mid: configuration does not fit (N %d, A %d)", a.N, a.A);
   return 1;
 }

@@ -55,7 +55,7 @@ static int check_cfg(const mx_qmix_cfg* c) {
   if (c->n_agents <= 0 || c->obs_dim <= 0 || c->act_dim <= 0 || c->state_dim <= 0 || c->episode_len <= 0 || c->max_batch <= 0) {
     mx_set_error("mx_qmix: non-positive dimension"); return 1;
   }
-  if (c->act_dim > 32 || c->n_agents > 32) { mx_set_error("mx_qmix: act_dim and n_agents must be <= 32"); return 1; }
+  if (c->act_dim > 64 || c->n_agents > 32) { mx_set_error("mx_qmix: act_dim must be <= 64 and n_agents <= 32"); return 1; }
   if (!c->vdn && c->hyper_layers != 1 && c->hyper_layers != 2) { mx_set_error("hypernet_layers must be 1 or 2"); return 1; }
   if (c->mlp && c->episode_len != 1) { mx_set_error("mx_qmix: the MLP (transition-level) variant stores transitions as episodes of length 1"); return 1; }
   if (c->mlp && c->prev_act_inp) { mx_set_error("mx_qmix: prev_act_inp is a recurrent-policy option"); return 1; }
