@@ -383,22 +383,13 @@ void mx_graph_destroy(mx_graph* g);
  * carries the K-direction core-matrix stride (the kernels use swap_ls = 0).  N % 16 == 0, N <= 256, K % 8 == 0, K <= 64. */
 int mx_tc_linear_probe(const float* X, const float* W, float* Y, int32_t M, int32_t N, int32_t K, int32_t passes, int32_t swap_ls, void* stream);
 
-/* Runtime options (process-wide tuning switches; the defaults are not yet re-measured on the H100).
+/* Runtime options (process-wide switches between paths that are each the default for some input or build).
  * Returns 1 for an unknown name.  (default)
- *   front_tc (1)            time-batched front layers on the wgmma 3xTF32 kernels; 0 = the FFMA kernel
- *   front_tc_threads (256)  inputs <= 56: two threads per accumulator row (k_front_fwd_tc2); 128 = one (k_front_fwd_tc)
- *   front_tc_wide (1)       64 < input width <= 128 on the tensor cores too; front_tc_wide2 (1): weights streamed, two CTAs per SM (0: resident weights)
+ *   front_tc (1)            time-batched front layers on the wgmma 3xTF32 kernels (inputs <= 128); 0 = the FFMA kernel
  *   wgrad_tc (-1)           backward of the front layers on the tensor cores: -1 = by input width (inputs > 64: mode 2), 0 = FFMA k_front_bwd,
- *                           1 = k_wgrad_tc beside k_front_bwd, 2 = k_front_bwd_tc + k_wgrad_tc; wgrad_tc_wide (1) = allow 64 < width <= 128;
- *                           front_bwd_tc_stream (1) = streamed transposed weights, two CTAs per SM
- *   front_bwd_mma (0)       mma.sync m16n8k8 3xTF32 inside k_front_bwd
- *   gru_wgrad_split (1)     GRU weight gradients as k_gru_wgrad on the forked branch beside k_front_bwd (QMIX step)
- *   gru_threads (0)         0 = 128-thread recurrences for sequences of >= 8 steps, 128 / 256 force a kernel family; gru_rows (1) rows per
- *                           128-thread CTA (2; 0 = by grid size); gru_fwd_rpc / gru_bwd_rpc (0 = automatic) rows per 256-thread CTA
- *   overlap (1) / overlap_rows (2^20)   state-only kernels on a forked stream / graph branch: 0 off, 1 when B*(T+1)*N <= overlap_rows, 2 always;
- *                           side_prio (0) stream priority of that branch; hyper_late (0)
+ *                           1 = k_wgrad_tc beside k_front_bwd, 2 = k_front_bwd_tc + k_wgrad_tc
+ *   overlap (1) / overlap_rows (2^20)   state-only kernels on a forked stream / graph branch: 0 off, 1 when B*(T+1)*N <= overlap_rows, 2 always
  *   mixer_split (1), mid_fused (1)      split hypernet / core mixer kernels; k_mid between the recurrences (0 = separate kernels)
- *   mixer_rm, mixer_split_rm, front_bwd_rm (0 = automatic)   tile heights
  *   optim_fused (1)         one-launch reduce + [exchange] + clip + Adam + Polyak (0: k_grad_reduce + k_adam)
  *   p2p_ll (1)              data-parallel exchange as flag-in-data lines (0: slots + one flag per rank); p2p_timeout_ms (10000) wait for a peer
  *   gather_tma (1)          episode gather on the TMA unit (0: vectorised loads; 2: TMA at every size)

@@ -10,7 +10,6 @@
 #include "mx_internal.h"
 #include "mx_kernels.h"
 #include "mx_tile.cuh"
-#include "mx_mma.cuh"
 
 // =====================================================================================================
 // Q head backward (one warp per row-step)
@@ -255,8 +254,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_gru_bwd(GruBwdArgs a) {
 // 48 packed FFMA2 per thread in four 12-deep chains, two xor-shuffle levels for the two column sums.  Lanes s = 0, 1 (and their
 // duplicates 2, 3) own unit 2kp + (s & 1) for the gate derivatives; the stores of a unit are split between the two duplicates.
 #define BWD2_THREADS 128
-// ROWS = 2: two sequence rows per CTA through the same register-resident W_hh slice (see k_gru_fwd2), for shapes with more rows than
-// two CTAs per SM hold at once
+// Only ROWS = 1 is launched (see k_gru_fwd2).
 template <int ROWS>
 __global__ void __launch_bounds__(BWD2_THREADS, 2) k_gru_bwd2(GruBwdArgs a) {
   constexpr int RING = 8, PF = 6;
@@ -431,7 +429,7 @@ MX_DEVINL void ln64_bwd_relu(bool act_tanh, float (&v)[RM][4], const float* u_s,
   }
 }
 
-template <int RM, bool MMA>
+template <int RM>
 __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, FrontBwdSmem sm) {
   constexpr int TM = 16 * RM;
   MX_DYN_SMEM(smem);
@@ -498,13 +496,11 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
     // ---- GRU weight gradients: dW_ih = dgi^T x2 ; dW_hh = [dgi_r, dgi_z, dgi_n*r]^T h_{t-1} ----
     if (wgemm && gru_here) {
       for (int nb = 0; nb < 3; ++nb) {
-        if (MMA) mx_mma_wgrad_block(dgi_s + nb * 64, sm.ldg, x_s, sm.ld64, TM, gp + L.wih, MX_G, MX_H, nb * 64, 0, accum);
-        else mx_wgrad_block(dgi_s + nb * 64, sm.ldg, x_s, sm.ld64, TM, gp + L.wih, MX_G, MX_H, nb * 64, 0, accum);
+        mx_wgrad_block(dgi_s + nb * 64, sm.ldg, x_s, sm.ld64, TM, gp + L.wih, MX_G, MX_H, nb * 64, 0, accum);
         if (a.no_gru) continue;
         const float* dgh = nb < 2 ? dgi_s + nb * 64 : dgn_s;
         const int ldd = nb < 2 ? sm.ldg : sm.ld64;
-        if (MMA) mx_mma_wgrad_block(dgh, ldd, hp_s, sm.ld64, TM, gp + L.whh + nb * 64 * MX_H, 64, MX_H, 0, 0, accum);
-        else mx_wgrad_block(dgh, ldd, hp_s, sm.ld64, TM, gp + L.whh + nb * 64 * MX_H, 64, MX_H, 0, 0, accum);
+        mx_wgrad_block(dgh, ldd, hp_s, sm.ld64, TM, gp + L.whh + nb * 64 * MX_H, 64, MX_H, 0, 0, accum);
       }
       mx_colsum(dgi_s, sm.ldg, TM, MX_G, gp + L.bih, accum);
       if (!a.no_gru) {
@@ -518,26 +514,6 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
     for (int i = 0; i < RM; ++i)
 #pragma unroll
       for (int jx = 0; jx < 4; ++jx) v[i][jx] = 0.f;
-    if (MMA) {       // tensor-core tiles (mx_mma.cuh): warp w owns 8 output columns; the result goes through da_s back to the (ty, tx) row layout
-      float cfr[RM][4];
-#pragma unroll
-      for (int i = 0; i < RM; ++i)
-#pragma unroll
-        for (int jx = 0; jx < 4; ++jx) cfr[i][jx] = 0.f;
-      for (int nc = 0; nc < 3; ++nc) {
-        __syncthreads();
-        mx_stage_weight(Wc, sm.ld64, th + L.wih, MX_G, MX_H, MX_H, nc * 64, 0, 64);
-        __syncthreads();
-        mx_mma_dgrad_acc<RM>(cfr, dgi_s + nc * 64, sm.ldg, Wc, sm.ld64);
-      }
-      mx_mma_store<RM>(cfr, da_s, sm.ld64);
-      __syncthreads();
-#pragma unroll
-      for (int i = 0; i < RM; ++i) {
-        const float4 q = mx_ld4(da_s + (ty * RM + i) * sm.ld64 + 4 * tx);
-        v[i][0] = q.x; v[i][1] = q.y; v[i][2] = q.z; v[i][3] = q.w;
-      }
-    } else
     for (int nc = 0; nc < 3; ++nc) {
       __syncthreads();
       mx_stage_weight(Wc, sm.ld64, th + L.wih, MX_G, MX_H, MX_H, nc * 64, 0, 64);
@@ -568,8 +544,7 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
     __syncthreads();
     // ---- fc2: dW2 = da2^T x1, db2 ; dx1 = da2 . W2 ----
     if (wgemm) {
-      if (MMA) mx_mma_wgrad_block(da_s, sm.ld64, x_s, sm.ld64, TM, gp + L.w2, MX_H, MX_H, 0, 0, accum);
-      else mx_wgrad_block(da_s, sm.ld64, x_s, sm.ld64, TM, gp + L.w2, MX_H, MX_H, 0, 0, accum);
+      mx_wgrad_block(da_s, sm.ld64, x_s, sm.ld64, TM, gp + L.w2, MX_H, MX_H, 0, 0, accum);
       mx_colsum(da_s, sm.ld64, TM, MX_H, gp + L.b2, accum);
     }
     mx_stage_weight(Wc, sm.ld64, th + L.w2, MX_H, MX_H, MX_H, 0, 0, 64);
@@ -578,21 +553,6 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
     for (int i = 0; i < RM; ++i)
 #pragma unroll
       for (int jx = 0; jx < 4; ++jx) v[i][jx] = 0.f;
-    if (MMA) {
-      float cfr[RM][4];
-#pragma unroll
-      for (int i = 0; i < RM; ++i)
-#pragma unroll
-        for (int jx = 0; jx < 4; ++jx) cfr[i][jx] = 0.f;
-      mx_mma_dgrad_acc<RM>(cfr, da_s, sm.ld64, Wc, sm.ld64);
-      mx_mma_store<RM>(cfr, x_s, sm.ld64);          // x1 is dead: its buffer carries dx1 back to the row layout
-      __syncthreads();
-#pragma unroll
-      for (int i = 0; i < RM; ++i) {
-        const float4 q = mx_ld4(x_s + (ty * RM + i) * sm.ld64 + 4 * tx);
-        v[i][0] = q.x; v[i][1] = q.y; v[i][2] = q.z; v[i][3] = q.w;
-      }
-    } else
     mx_mm_nn<RM>(da_s, sm.ld64, Wc, sm.ld64, v);
     ln64_bwd_relu<RM>(a.act_tanh != 0, v, u_s, sm.ld64, st1_s, ln1g_s, dg1, db1);
     __syncthreads();     // da_s (da2) consumed by everyone
@@ -622,8 +582,7 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
     // ---- fc1: dW1 = da1^T x0, db1 ; dx0 = da1 . W1 (only for the LN0 gain/bias) ----
     if (wgemm) {
       for (int kb = 0; kb * 64 < I; ++kb) {
-        if (MMA) mx_mma_wgrad_block(da_s, sm.ld64, x0_s + kb * 64, sm.ldi, TM, gp + L.w1, MX_H, I, 0, kb * 64, accum);
-        else mx_wgrad_block(da_s, sm.ld64, x0_s + kb * 64, sm.ldi, TM, gp + L.w1, MX_H, I, 0, kb * 64, accum);
+        mx_wgrad_block(da_s, sm.ld64, x0_s + kb * 64, sm.ldi, TM, gp + L.w1, MX_H, I, 0, kb * 64, accum);
       }
       mx_colsum(da_s, sm.ld64, TM, MX_H, gp + L.b1, accum);
     }
@@ -636,21 +595,6 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
         for (int i = 0; i < RM; ++i)
 #pragma unroll
           for (int jx = 0; jx < 4; ++jx) v[i][jx] = 0.f;
-        if (MMA) {
-          float cfr[RM][4];
-#pragma unroll
-          for (int i = 0; i < RM; ++i)
-#pragma unroll
-            for (int jx = 0; jx < 4; ++jx) cfr[i][jx] = 0.f;
-          mx_mma_dgrad_acc<RM>(cfr, da_s, sm.ld64, Wc, sm.ld64);
-          mx_mma_store<RM>(cfr, dx0_s + kb * 64, sm.ldi);
-          __syncthreads();
-#pragma unroll
-          for (int i = 0; i < RM; ++i) {
-            const float4 q = mx_ld4(dx0_s + (ty * RM + i) * sm.ldi + kb * 64 + 4 * tx);
-            v[i][0] = q.x; v[i][1] = q.y; v[i][2] = q.z; v[i][3] = q.w;
-          }
-        } else
         mx_mm_nn<RM>(da_s, sm.ld64, Wc, sm.ld64, v);
         float cg[4] = {0.f, 0.f, 0.f, 0.f}, cb[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -727,7 +671,7 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_front_bwd(FrontBwdArgs a, F
 // k_gru_wgrad: the GRU weight gradients of the time-batched backward as their own kernel,
 //   dW_ih = dgi^T x2, db_ih ;  dW_hh = [dgi_r, dgi_z, dgi_n * r]^T h_{t-1}, db_hh
 // They depend only on what k_gru_bwd left (dgi) and on saved forward rows, not on k_front_bwd's data-gradient chain, so the QMIX
-// step launches this on the forked branch BESIDE k_front_bwd (option gru_wgrad_split): same tiles, same grid, CTA b of both kernels
+// step launches this on the forked branch BESIDE k_front_bwd: same tiles, same grid, CTA b of both kernels
 // fills disjoint columns of gradient partial b; the two CTAs fit one SM together (shared memory ~77 + ~134 KB at 3m).
 // 256 threads at <= 128 registers so that a CTA of each kernel is resident together.  Two passes per tile (W_ih, then W_hh); thread
 // (tn, tk) owns rows {64 g + 2 tn, + 1 : g = 0..2} x columns 8 tk .. + 7 of the pass's matrix: per tile row 3 LDS.64 + 2 LDS.128 feed
@@ -901,11 +845,9 @@ int mx_launch_gru_bwd(const GruBwdArgs& a, cudaStream_t s) {
   const int sms = mx_num_sms();
   int rpc = 1;
   while (rpc < 4 && mx_ceil_div(a.R, rpc) > 2 * sms) rpc *= 2;
-  if (g_mx_gru_bwd_rpc == 1 || g_mx_gru_bwd_rpc == 2 || g_mx_gru_bwd_rpc == 4) rpc = g_mx_gru_bwd_rpc;
-  if (g_mx_gru_threads == 128 || (g_mx_gru_threads == 0 && g_mx_gru_bwd_rpc == 0 && a.T >= 8)) {      // default at every size (r02 sweeps)
-    const bool two = g_mx_gru_rows == 2 || (g_mx_gru_rows == 0 && a.R > 2 * mx_num_sms());      // more row-CTAs than fit at once
-    if (two) MX_LAUNCH_PDL(k_gru_bwd2<2>, dim3((a.R + 1) / 2), dim3(BWD2_THREADS), 0, s, a);
-    else MX_LAUNCH_PDL(k_gru_bwd2<1>, dim3(a.R), dim3(BWD2_THREADS), 0, s, a);
+  // sequences: the 128-thread kernel, one row per CTA (r02 sweeps)
+  if (a.T >= 8) {
+    MX_LAUNCH_PDL(k_gru_bwd2<1>, dim3(a.R), dim3(BWD2_THREADS), 0, s, a);
     MX_COUNT();
     MX_MARK("k_gru_bwd", s);
     return MX_CHECK_LAUNCH("gru_bwd2");
@@ -934,7 +876,7 @@ static int front_bwd_pick_rm(int M, int in_dim, int sms, bool gru_ext) {
   return best;
 }
 
-template <int RM, bool MMA>
+template <int RM>
 static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s) {
   const int TM = 16 * RM;
   FrontBwdSmem sm = front_bwd_smem(a.L.in_dim, TM, a.gru_wgrad_ext != 0);
@@ -942,7 +884,7 @@ static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_
   const int ntiles = mx_ceil_div(a.M, TM);
   int grid = mx_num_sms();
   if (grid > ntiles) grid = ntiles;
-  auto kern = k_front_bwd<RM, MMA>;
+  auto kern = k_front_bwd<RM>;
 #if !MX_EMU
   if (smem > 227 * 1024) { mx_set_error("front_bwd: %zu bytes of shared memory needed (obs_dim too large)", smem); return 1; }
   static size_t configured = 0;
@@ -955,26 +897,17 @@ static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_
   return MX_CHECK_LAUNCH("front_bwd");
 }
 
-extern int g_mx_front_bwd_rm;
-int g_mx_gru_wgrad_split = 1;    // 1 (default): the QMIX step runs the GRU weight gradients as k_gru_wgrad on the forked branch beside k_front_bwd
-int g_mx_front_bwd_mma = 0;      // 1: the GEMMs of k_front_bwd on mma.sync 3xTF32 tiles (mx_mma.cuh); 0 (default): FFMA micro-kernels
-                                 // (default not yet measured on the H100)
 bool mx_front_bwd_tc_usable(const FrontBwdArgs& a);
 int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s);
 int mx_launch_front_bwd(const FrontBwdArgs& a_in, int* nparts_used, cudaStream_t s) {
   if (mx_front_bwd_tc_usable(a_in)) return mx_launch_front_bwd_tc(a_in, nparts_used, s);
   FrontBwdArgs a = a_in;
   a.wgrad_external = mx_wgrad_tc_usable(a) ? 1 : 0;
-  a.use_mma = g_mx_front_bwd_mma ? 1 : 0;
-  const int rm = g_mx_front_bwd_rm ? g_mx_front_bwd_rm : front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), a.gru_wgrad_ext != 0);
+  const int rm = front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), a.gru_wgrad_ext != 0);
   int rc;
-  if (a.use_mma) {        // separate instantiations: the FFMA kernel's register allocation must not pay for the mma path
-    if (rm == 3) rc = front_bwd_launch<3, true>(a, nparts_used, s);
-    else if (rm == 4) rc = front_bwd_launch<4, true>(a, nparts_used, s);
-    else rc = front_bwd_launch<2, true>(a, nparts_used, s);
-  } else if (rm == 3) rc = front_bwd_launch<3, false>(a, nparts_used, s);
-  else if (rm == 4) rc = front_bwd_launch<4, false>(a, nparts_used, s);
-  else rc = front_bwd_launch<2, false>(a, nparts_used, s);
+  if (rm == 3) rc = front_bwd_launch<3>(a, nparts_used, s);
+  else if (rm == 4) rc = front_bwd_launch<4>(a, nparts_used, s);
+  else rc = front_bwd_launch<2>(a, nparts_used, s);
   if (rc || !a.wgrad_external) return rc;
   return mx_launch_wgrad_tc(a, *nparts_used, s);      // one gradient partial per k_front_bwd CTA: the same rows of gpart
 }
@@ -982,7 +915,7 @@ int mx_launch_front_bwd(const FrontBwdArgs& a_in, int* nparts_used, cudaStream_t
 // ---- k_gru_wgrad beside k_front_bwd ----
 bool mx_wgrad_tc_usable(const FrontBwdArgs& a);
 bool mx_gru_wgrad_split_usable(const FrontBwdArgs& a) {
-  if (!g_mx_gru_wgrad_split || g_mx_front_bwd_mma || a.no_gru || a.skip_wgrad) return false;
+  if (a.no_gru || a.skip_wgrad) return false;
   return !mx_front_bwd_tc_usable(a) && !mx_wgrad_tc_usable(a);
 }
 template <int RM>
@@ -1005,7 +938,7 @@ static int gru_wgrad_launch(const FrontBwdArgs& a, cudaStream_t s) {
 // `a` must be the arguments the following mx_launch_front_bwd call gets (gru_wgrad_ext = 1): same tile height, same grid, so CTA b
 // of both kernels writes gradient partial b
 int mx_launch_gru_wgrad(const FrontBwdArgs& a, cudaStream_t s) {
-  const int rm = g_mx_front_bwd_rm ? g_mx_front_bwd_rm : front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), true);
+  const int rm = front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), true);
   if (rm == 3) return gru_wgrad_launch<3>(a, s);
   if (rm == 4) return gru_wgrad_launch<4>(a, s);
   return gru_wgrad_launch<2>(a, s);

@@ -284,8 +284,8 @@ __global__ void __launch_bounds__(GRU_THREADS, 1) k_gru_fwd(GruFwdArgs a) {
 // every scheduler sees two warps instead of four, and on the others one -- the step is a dependent chain, fewer co-resident warps means
 // less issue and LSU contention; one xor-shuffle level instead of two.
 #define GRU2_THREADS 128
-// ROWS = 2: the CTA carries two sequence rows through the same register-resident weights (their two dependent chains interleave), for
-// shapes with more row-CTAs than two per SM can hold at once (SMAC 8m: 1 024 row-CTAs = 3.5 waves of 296; option gru_rows)
+// Only ROWS = 1 is launched.  The parameter stays because the single-row rewrite of this source compiles to a different register
+// allocation and schedule that measured up to 0.3 % slower at SMAC 8m (H100 80GB HBM3, 700 W power limit).
 template <int ROWS>
 __global__ void __launch_bounds__(GRU2_THREADS, 2) k_gru_fwd2(GruFwdArgs a) {
   __shared__ __align__(16) float h_s[2][ROWS][MX_H];
@@ -590,12 +590,10 @@ int mx_launch_gru_fwd(const GruFwdArgs& a, int nets, cudaStream_t s) {
   const int sms = mx_num_sms();
   int rpc = 1;     // one resident CTA per SM (the kernel is register heavy): grow rows-per-CTA until the grid fits one wave
   while (rpc < 4 && mx_ceil_div(a.R, rpc) * nets > 2 * sms) rpc *= 2;   // two CTAs fit per SM (<= 128 registers): co-resident CTAs hide each other's latencies
-  if (g_mx_gru_fwd_rpc == 1 || g_mx_gru_fwd_rpc == 2 || g_mx_gru_fwd_rpc == 4) rpc = g_mx_gru_fwd_rpc;
-  // the 128-thread kernel (one row per CTA); the 256-thread kernels stay behind gru_threads=256 / gru_*_rpc
-  if (g_mx_gru_threads == 128 || (g_mx_gru_threads == 0 && g_mx_gru_fwd_rpc == 0 && a.T + 1 >= 8)) {      // (one-step "branch" calls of R-MADDPG keep the multi-row CTAs: a CTA per row would spend its time loading W_hh)      // default at every size (r02 sweeps: 3m 174 vs 188 us, 2s3z 555 vs 619, 8m 1408 vs 1494)
-    const bool two = g_mx_gru_rows == 2 || (g_mx_gru_rows == 0 && (long long)a.R * nets > 2LL * mx_num_sms());      // more row-CTAs than fit at once
-    if (two) MX_LAUNCH_PDL(k_gru_fwd2<2>, dim3((a.R + 1) / 2, nets), dim3(GRU2_THREADS), 0, s, a);
-    else MX_LAUNCH_PDL(k_gru_fwd2<1>, dim3(a.R, nets), dim3(GRU2_THREADS), 0, s, a);
+  // sequences: the 128-thread kernel, one row per CTA (r02 sweeps: 3m 174 vs 188 us, 2s3z 555 vs 619, 8m 1408 vs 1494).  The one-step
+  // "branch" calls of R-MADDPG keep the multi-row CTAs: a CTA per row would spend its time loading W_hh
+  if (a.T + 1 >= 8) {
+    MX_LAUNCH_PDL(k_gru_fwd2<1>, dim3(a.R, nets), dim3(GRU2_THREADS), 0, s, a);
     MX_COUNT();
     MX_MARK("k_gru_fwd", s);
     return MX_CHECK_LAUNCH("gru_fwd2");

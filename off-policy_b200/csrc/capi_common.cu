@@ -18,35 +18,21 @@ int g_mx_pdl_skip_next = 0;
 
 // runtime options shared by the product and the emulated build (mx_set_option)
 int g_mx_p2p_timeout_ms = 10000;      // how long a rank waits for a peer's gradient before it sets the sticky abort word (tests shorten it)
-int g_mx_gru_rows = 1;        // rows per CTA of the 128-thread recurrences: 1 (default), 2, 0 = 2 when there are more row-CTAs than two per SM hold at once.
 int g_mx_p2p_ll = 1;          // data-parallel exchange inside k_optim_fused: 1 = flag-in-data lines (no fence / counter / flag hop), 0 = slots + per-rank flags
 int g_mx_mixer_split = 1;      // 1: split mixer (hypernet-forward / core / hypernet-backward kernels) whenever the forked branch is
                                //    in use; 2: always; 0: always the single fused k_mixer
-int g_mx_mixer_split_rm = 0;   // rows per thread of the split mixer's tiles (0 = automatic)
 int g_mx_overlap = 1;          // state-only kernels (weight-image prep, mixer hypernets) on a forked branch beside the agent-net
                                // kernels: 1 = when the step is latency-bound (rows <= g_mx_overlap_rows), 2 = always, 0 = never
-int g_mx_gru_threads = 0;
-int g_mx_side_prio = 0;         // priority of a learner's forked branch (read when the learner is created): 0 default, 1 lower, -1 higher
-int g_mx_hyper_late = 0;        // 0 (default): the hypernet branch forks before the front kernel; 1: after it, beside the recurrence
-                                // (the recurrence is the kernel that suffers most from co-resident CTAs)
 int g_mx_mid_fused = 1;        // 1: k_qhead + k_mix_core + k_qhead_bwd as ONE kernel (k_mid) when the split mixer is in use and no debug
                                //    outputs are requested; 0: three launches
-int g_mx_gru_fwd_rpc = 0;      // tuning overrides: sequence rows per CTA of the recurrence kernels (0 = automatic; 1, 2 or 4)
-int g_mx_gru_bwd_rpc = 0;
 int g_mx_overlap_rows = 1 << 20; // forked branch up to this many rows, serial beyond (not yet measured on the H100)
 int mx_set_option_common(const char* name, int value) {
   if (!strcmp(name, "mixer_split")) { g_mx_mixer_split = value; return 0; }
-  if (!strcmp(name, "mixer_split_rm")) { g_mx_mixer_split_rm = value; return 0; }
   if (!strcmp(name, "overlap")) { g_mx_overlap = value; return 0; }
   if (!strcmp(name, "overlap_rows")) { g_mx_overlap_rows = value; return 0; }
   if (!strcmp(name, "mid_fused")) { g_mx_mid_fused = value; return 0; }
   if (!strcmp(name, "optim_fused")) { g_mx_optim_fused = value; return 0; }
-  if (!strcmp(name, "side_prio")) { g_mx_side_prio = value; return 0; }
-  if (!strcmp(name, "hyper_late")) { g_mx_hyper_late = value; return 0; }
-  if (!strcmp(name, "front_bwd_mma")) { g_mx_front_bwd_mma = value; return 0; }
-  if (!strcmp(name, "gru_wgrad_split")) { g_mx_gru_wgrad_split = value; return 0; }
   if (!strcmp(name, "p2p_ll")) { g_mx_p2p_ll = value; return 0; }
-  if (!strcmp(name, "gru_rows")) { g_mx_gru_rows = value; return 0; }
   if (!strcmp(name, "p2p_timeout_ms")) { g_mx_p2p_timeout_ms = value; return 0; }
 #if !MX_EMU
   if (!strcmp(name, "smem_carveout")) { g_mx_smem_carveout = value; return 0; }
@@ -54,9 +40,6 @@ int mx_set_option_common(const char* name, int value) {
   if (!strcmp(name, "smem_carveout")) return 0;
 #endif
   if (!strcmp(name, "gather_tma")) { g_mx_gather_tma = value; return 0; }      // 1: episode gather on the TMA unit (default), 0: vectorised loads
-  if (!strcmp(name, "gru_threads")) { g_mx_gru_threads = value; return 0; }      // 0: by size, 128 / 256: force the recurrence kernels' CTA width
-  if (!strcmp(name, "gru_fwd_rpc")) { g_mx_gru_fwd_rpc = value; return 0; }
-  if (!strcmp(name, "gru_bwd_rpc")) { g_mx_gru_bwd_rpc = value; return 0; }
   return -1;
 }
 

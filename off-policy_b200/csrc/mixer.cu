@@ -722,7 +722,6 @@ __global__ void __launch_bounds__(MX_TILE_THREADS) k_mix_hyper_bwd(MixerArgs a, 
   }
 }
 
-extern int g_mx_mixer_rm;
 int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
   const int E = a.B * a.T;
   const int sms = mx_num_sms();
@@ -736,7 +735,7 @@ int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
     return MX_CHECK_LAUNCH("vdn_mix");
   }
   if (a.L.N > 32) { mx_set_error("mixer: n_agents > 32 unsupported"); return 1; }
-  const int RM = g_mx_mixer_rm ? g_mx_mixer_rm : ((E > 16 * sms) ? 2 : 1);
+  const int RM = (E > 16 * sms) ? 2 : 1;
   const int TE = 16 * RM;
   MixSmem sm = mix_smem_layout(a.L, TE);
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
@@ -756,11 +755,9 @@ int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
   return MX_CHECK_LAUNCH("mixer");
 }
 
-extern int g_mx_mixer_split_rm;
 int mx_mixer_split_supported(const MxMixLayout& L) { return L.ME <= 32 * MX_MIX_MAXK && L.N <= 32; }
 
 static int mix_split_rm(int E) {
-  if (g_mx_mixer_split_rm) return g_mx_mixer_split_rm;
   return (E > 16 * mx_num_sms()) ? 2 : 1;
 }
 template <class K>

@@ -10,7 +10,7 @@ void mx_set_error(const char* fmt, ...);
 extern long long g_mx_launches;
 extern int g_mx_prof_on;
 void mx_prof_mark(const char* name, cudaStream_t s);
-extern int g_mx_mixer_split, g_mx_mixer_split_rm, g_mx_overlap, g_mx_overlap_rows, g_mx_mid_fused, g_mx_gru_fwd_rpc, g_mx_gru_bwd_rpc, g_mx_optim_fused, g_mx_gru_threads, g_mx_front_bwd_mma, g_mx_hyper_late, g_mx_side_prio, g_mx_gru_wgrad_split, g_mx_p2p_ll, g_mx_p2p_timeout_ms, g_mx_gru_rows;
+extern int g_mx_mixer_split, g_mx_overlap, g_mx_overlap_rows, g_mx_mid_fused, g_mx_optim_fused, g_mx_p2p_ll, g_mx_p2p_timeout_ms;
 int mx_set_option_common(const char* name, int value);   // 0 when `name` was one of the build-independent options
 #define MX_COUNT() (++g_mx_launches)
 #define MX_MARK(name, s) do { if (g_mx_prof_on) mx_prof_mark((name), (s)); } while (0)

@@ -184,7 +184,6 @@ struct FrontBwdArgs {
   // k_wgrad_tc produces every dW / db of the front layers and the GRU input / recurrent matrices from them
   float *da2_out, *da1_out;   // [M][H] each: gradient at the fc2 / fc1 pre-activation outputs (after the ReLU mask)
   int wgrad_external;      // set by the launcher, not by callers
-  int use_mma;             // set by the launcher: GEMMs of k_front_bwd on mma.sync 3xTF32 tiles (mx_mma.cuh) instead of the FFMA micro-kernels
   float* tc_imgT;          // scratch for the transposed TF32 weight images of the all-tensor-core backward (option wgrad_tc = 2)
   int tc_imgT_ready;       // 1: the caller already built them for the current parameters (mx_launch_tc_prep_weights_T)
   float* tc_acc;           // with tc_imgT or the tensor-core weight gradients: accumulators, as FrontFwdArgs::tc_acc

@@ -212,14 +212,7 @@ extern "C" int mx_qmix_create(const mx_qmix_cfg* c, float* theta, float* theta_t
   mx_mix_wide_layout(q->mix, &q->wl);
   if (q->wide && !q->split_ok) { mx_set_error("mx_qmix_create: state_dim %d needs the wide-state mixer, which supports mixer_hidden <= 64", c->state_dim); delete q; return 1; }
 #if !MX_EMU
-  {
-    // side branch priority (option side_prio, read at creation): 0 = default, 1 = LOWER than the caller's stream (the agent-net kernels are
-    // scheduled first when both branches have CTAs pending), -1 = higher
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);            // lo = numerically largest = least priority
-    const int prio = g_mx_side_prio > 0 ? lo : (g_mx_side_prio < 0 ? hi : 0);
-    if (cudaStreamCreateWithPriority(&q->side, cudaStreamNonBlocking, prio) != cudaSuccess) { mx_set_error("mx_qmix_create: cudaStreamCreate failed"); delete q; return 1; }
-  }
+  if (cudaStreamCreateWithFlags(&q->side, cudaStreamNonBlocking) != cudaSuccess) { mx_set_error("mx_qmix_create: cudaStreamCreate failed"); delete q; return 1; }
   cudaEvent_t* evs[7] = {&q->ev_fork, &q->ev_prep, &q->ev_batch, &q->ev_hyper, &q->ev_core, &q->ev_hbwd, &q->ev_gbwd};
   for (cudaEvent_t* e : evs) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
 #endif
@@ -427,19 +420,13 @@ static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs*
     ff.tc_img[0] = ws + W.tcimg[0]; ff.tc_img[1] = ws + W.tcimg[1];
     ff.tc_acc = ws + W.tcacc; ff.tc_acc_cols = (int)W.tcacc_cols;
   }
-  // the mixer's hypernetworks depend on the sampled states and the parameters only: forked branch beside the agent nets.
-  // Default: fork before the front kernel.  hyper_late = 1 moves the fork AFTER the tensor-core front kernel (which fills an SM's shared
-  // memory, so hypernet CTAs and front CTAs cannot share an SM) -- measured slower: beside the recurrence the hypernet CTAs cost more.
-  const bool late = g_mx_hyper_late != 0;
+  // the mixer's hypernetworks depend on the sampled states and the parameters only: forked branch beside the agent nets, before the
+  // front kernel (forked after it, beside the recurrence, the hypernet CTAs cost more)
 #if !MX_EMU
-  if (split && overlap && !late) fork_to_side(q, q->ev_batch, s);
+  if (split && overlap) fork_to_side(q, q->ev_batch, s);
 #endif
-  if (split && overlap && !late) { if (mx_launch_mix_hyper_fwd(mx, side)) return 1; }
+  if (split && overlap) { if (mx_launch_mix_hyper_fwd(mx, side)) return 1; }
   if (mx_launch_front_fwd(ff, 2, s)) return 1;
-#if !MX_EMU
-  if (split && overlap && late) fork_to_side(q, q->ev_batch, s);
-#endif
-  if (split && overlap && late) { if (mx_launch_mix_hyper_fwd(mx, side)) return 1; }
 
   if (c.mlp) {      // ---- transition-level variant (M_QMix / M_VDN): no recurrence, Q = columns [0, A) of the "gi" rows ----
     int parts[4] = {0, 0, 0, 0};

@@ -23,7 +23,6 @@
 int g_mx_wgrad_tc = -1;       // -1 (default): by input width -- inputs <= 64 (3m, MPE) on the FFMA backward, wider inputs (8m / 2s3z, obs 80) on
                               // k_front_bwd_tc + k_wgrad_tc (split not yet measured on the H100); 0 / 1 / 2 force a mode
 static inline int wgrad_mode(int in_dim) { return g_mx_wgrad_tc >= 0 ? g_mx_wgrad_tc : (in_dim > 64 ? 2 : 0); }
-int g_mx_wgrad_tc_wide = 1;   // with wgrad_tc: input widths 65 .. 112 too (SMAC 8m / 2s3z observations are 80 wide)
 
 #define WG_ROWS 64            // rows per MMA group (the K extent of one staged tile)
 #define WG_DSTRIDE 160        // accumulator column stride between the three accumulators
@@ -334,7 +333,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(WgradArgs w, WgradSm
 }
 
 bool mx_wgrad_tc_usable(const FrontBwdArgs& a) {
-  return wgrad_mode(a.L.in_dim) && a.da2_out && a.da1_out && !a.skip_wgrad && a.L.in_dim <= (g_mx_wgrad_tc_wide ? WG_MAX_IN : 64) && a.M >= 1;
+  return wgrad_mode(a.L.in_dim) && a.da2_out && a.da1_out && !a.skip_wgrad && a.L.in_dim <= WG_MAX_IN && a.M >= 1;
 }
 
 static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, cudaStream_t s, int ln_parts = 0);
@@ -376,7 +375,6 @@ static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, 
 // tile's shared memory, free between MMAs) and threads 0-63 / 64-127 keep running sums of one column each.
 // =====================================================================================================
 struct BwdTcSmem { int o_ahi, o_alo, o_wih, o_w2, o_w1, total; };
-int g_mx_front_bwd_tc_stream = 1;      // 1 (default): every weight operand of k_front_bwd_tc goes through ONE chunk buffer, two CTAs per SM (inputs <= 96)
 static BwdTcSmem bwd_tc_smem(int Kp16, bool stream = false) {
   BwdTcSmem s;
   int o = 0;
@@ -635,7 +633,7 @@ bool mx_front_bwd_tc_usable(const FrontBwdArgs& a) {
 }
 
 // k_tc_prep_weights_T -> k_front_bwd_tc -> k_wgrad_tc ; *nparts_used = the number of gradient partials written
-bool mx_tc_prep_T_wanted(int in_dim) { return wgrad_mode(in_dim) >= 2 && in_dim <= (g_mx_wgrad_tc_wide ? WG_MAX_IN : 64); }
+bool mx_tc_prep_T_wanted(int in_dim) { return wgrad_mode(in_dim) >= 2 && in_dim <= WG_MAX_IN; }
 int mx_launch_tc_prep_weights_T(const float* theta, const MxNetLayout& L, float* imgT, cudaStream_t s) {
   const int n = 3 * 4096 + 4096 + mx_round_up(L.in_dim, 16) * 64;
   MX_LAUNCH_PDL(k_tc_prep_weights_T, dim3((n + 255) / 256), dim3(256), 0, s, theta, L, imgT);
@@ -647,7 +645,8 @@ int mx_launch_tc_prep_weights_T(const float* theta, const MxNetLayout& L, float*
 int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s) {
   const int Kp16 = mx_round_up(a.L.in_dim, 16);
   if (!a.tc_imgT_ready && mx_launch_tc_prep_weights_T(a.theta, a.L, a.tc_imgT, s)) return 1;
-  const bool stream = g_mx_front_bwd_tc_stream != 0 && a.ln_part != nullptr;      // needs the side array for the LayerNorm sums
+  // streamed (every weight operand through ONE chunk buffer, two CTAs per SM) when the caller gives the side array for the LayerNorm sums
+  const bool stream = a.ln_part != nullptr;
   BwdTcSmem sm = bwd_tc_smem(Kp16, stream);
 #if !MX_EMU
   static int configured = 0;
@@ -666,7 +665,6 @@ int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t
   if (gb * 512 > a.tc_acc_cols) gb = a.tc_acc_cols / 512;
   FrontBwdArgs b = a;
   b.wgrad_external = 1;
-  if (!stream) b.ln_part = nullptr;
   if (ga > a.ln_part_rows && stream) ga = a.ln_part_rows;
   MX_LAUNCH_PDL(k_front_bwd_tc, dim3(ga), dim3(128), (size_t)sm.total, s, b, sm);
   MX_COUNT();

@@ -454,195 +454,17 @@ __global__ void __launch_bounds__(256, 1) k_front_fwd_tc2(FrontFwdArgs a, FrontT
 
 
 // =====================================================================================================
-// Wide inputs (64 < in_dim <= 128: SMAC 8m / 2s3z observations): same pipeline, but fc1's K dimension is fed in chunks of 64
-// columns that accumulate in the accumulator -- the A tile stays [128][64] and only one fc1 weight chunk is resident (restaged per tile from
-// the L2-resident image), so that fc2 and W_ih (96 KB as hi / lo) still fit beside them: 224 KB of dynamic shared memory.
-// =====================================================================================================
-__global__ void __launch_bounds__(128, 1) k_front_fwd_tc_wide(FrontFwdArgs a, FrontTcSmem sm) {
-  MX_DYN_SMEM_RAW(smem_raw);
-  __shared__ __align__(8) tc::Bar bar_s;
-  __shared__ float par_s[6 * MX_H];             // b1,g1,be1,b2,g2,be2   (b_ih and the feature-norm rows are read through L1: the dynamic
-                                                // 224 KB leave ~3 KB of static shared memory under the 227 KB per-CTA limit)
-  const int tid = threadIdx.x;
-  const int net = blockIdx.y;
-  const float* __restrict__ th = a.theta[net];
-  const MxNetLayout L = a.L;
-  const bool live = (net == 0);
-  const int I = L.in_dim, Kp = (I + 7) & ~7, Kc1 = Kp - 64;
-  char* base = reinterpret_cast<char*>(smem_raw);
-  char *a_hi = base + sm.o_ahi, *a_lo = base + sm.o_alo;
-  char *w1h = base + sm.o_w1h, *w2h = base + sm.o_w2h, *w2l = base + sm.o_w2l, *wih = base + sm.o_wih, *wil = base + sm.o_wil;
-  const uint32_t bar = tc::bar_addr(&bar_s);
-  float* acc = tc::cta_slice(a.tc_acc, 256);
-  if (tid == 0) {
-    tc::mbar_init(bar, blockDim.x);
-    tc::mbar_init_fence();
-  }
-  for (int i = tid; i < MX_H; i += blockDim.x) {
-    par_s[i] = th[L.b1 + i]; par_s[MX_H + i] = th[L.ln1_g + i]; par_s[2 * MX_H + i] = th[L.ln1_b + i];
-    par_s[3 * MX_H + i] = th[L.b2 + i]; par_s[4 * MX_H + i] = th[L.ln2_g + i]; par_s[5 * MX_H + i] = th[L.ln2_b + i];
-  }
-  MX_PDL_WAIT();
-  const float* img = a.tc_img[net];
-  {   // resident layers: fc2 and W_ih (contiguous in the image after the two fc1 chunks, contiguous in shared memory from o_w2h)
-    const float* src = img + 2 * 64 * Kp;
-    float* dst = reinterpret_cast<float*>(w2h);
-    const int nvec = (sm.total - sm.o_w2h) >> 4;
-    for (int v = tid; v < nvec; v += blockDim.x) mx_cp16(dst + 4 * v, src + 4 * v);
-    mx_cp_commit();
-  }
-  const float* bih_s = th + L.bih;
-  const float* fng = th + L.fn_g;
-  const float* fnb = th + L.fn_b;
-  __syncthreads();
-  uint32_t phase = 0;
-  const int ntiles = (a.M + 127) / 128;
-  const int I4 = (I + 3) >> 2;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int m = tile * 128 + tid;
-    const bool ok = m < a.M;
-    const float* xrow = a.X + (size_t)(ok ? m : 0) * a.ldx;
-    // ---- row statistics over all I features (two reads of the row; loads issued eight float4 at a time so that a thread has 128 bytes
-    //      of its row in flight instead of one dependent load per iteration) ----
-    float mean = 0.f, rstd = 1.f;
-    {
-      float p[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int cb = 0; cb < I4; cb += 8) {
-        float4 q8[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) q8[i] = (ok && cb + i < I4) ? *reinterpret_cast<const float4*>(xrow + 4 * (cb + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int c = 4 * (cb + i);
-          p[0] += (c < I) ? q8[i].x : 0.f; p[1] += (c + 1 < I) ? q8[i].y : 0.f; p[2] += (c + 2 < I) ? q8[i].z : 0.f; p[3] += (c + 3 < I) ? q8[i].w : 0.f;
-        }
-      }
-      mean = ((p[0] + p[1]) + (p[2] + p[3])) / (float)I;
-      float q[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int cb = 0; cb < I4; cb += 8) {
-        float4 q8[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) q8[i] = (ok && cb + i < I4) ? *reinterpret_cast<const float4*>(xrow + 4 * (cb + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int c = 4 * (cb + i);
-          const float d0 = (c < I) ? q8[i].x - mean : 0.f, d1 = (c + 1 < I) ? q8[i].y - mean : 0.f, d2 = (c + 2 < I) ? q8[i].z - mean : 0.f,
-                      d3 = (c + 3 < I) ? q8[i].w - mean : 0.f;
-          q[0] = fmaf(d0, d0, q[0]); q[1] = fmaf(d1, d1, q[1]); q[2] = fmaf(d2, d2, q[2]); q[3] = fmaf(d3, d3, q[3]);
-        }
-      }
-      rstd = rsqrtf(((q[0] + q[1]) + (q[2] + q[3])) / (float)I + MX_LN_EPS);
-      if (live && ok && a.st0) { a.st0[2 * (size_t)m] = mean; a.st0[2 * (size_t)m + 1] = rstd; }
-    }
-    // ---- fc1 in two K chunks: stage the weight chunk, write the normalised input chunk as the A tile, accumulate ----
-    for (int ch = 0; ch < 2; ++ch) {
-      const int Kc = ch == 0 ? 64 : Kc1;
-      {
-        const float* src = ch == 0 ? img : img + 2 * 64 * 64;
-        float* dst = reinterpret_cast<float*>(w1h);
-        const int nvec = (2 * 64 * Kc * 4) >> 4;          // hi tile then lo tile, contiguous in the image
-        for (int v = tid; v < nvec; v += blockDim.x) mx_cp16(dst + 4 * v, src + 4 * v);
-        mx_cp_commit();
-      }
-      for (int cb = 0; 4 * cb < Kc; cb += 8) {
-        float4 q8[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int c0 = 64 * ch + 4 * (cb + i);
-          q8[i] = (ok && 4 * (cb + i) < Kc && c0 < I) ? *reinterpret_cast<const float4*>(xrow + c0) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int c4 = cb + i;
-        if (4 * c4 >= Kc) continue;
-        const int c0 = 64 * ch + 4 * c4;
-        const float4 v = q8[i];
-        float x[4] = {v.x, v.y, v.z, v.w};
-        float4 h, l;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int c = c0 + j;
-          x[j] = (ok && c < I) ? (a.feature_norm ? ((x[j] - mean) * rstd * fng[c] + fnb[c]) : x[j]) : 0.f;
-        }
-        h.x = tc::to_tf32(x[0]); h.y = tc::to_tf32(x[1]); h.z = tc::to_tf32(x[2]); h.w = tc::to_tf32(x[3]);
-        l.x = x[0] - h.x; l.y = x[1] - h.y; l.z = x[2] - h.z; l.w = x[3] - h.w;
-        const uint32_t o = tc::core_off_bytes(tid, 4 * c4, Kc);
-        *reinterpret_cast<float4*>(a_hi + o) = h;
-        *reinterpret_cast<float4*>(a_lo + o) = l;
-      }
-      }
-      mx_cp_wait<0>();
-      tc::fence_async_smem();
-      __syncthreads();
-      tc::mma(acc, 0, a_hi, a_lo, w1h, w1h + 64 * Kc * 4, MX_H, Kc, 3, ch > 0 ? 1u : 0u);
-      tc::arrive(bar);
-      tc::mbar_wait(bar, phase);        // the MMAs have read the A tile and the weight chunk: both may be refilled
-      phase ^= 1;
-    }
-    // ---- fc1 epilogue, then fc2 (weights resident) ----
-    for (int layer = 0; layer < 2; ++layer) {
-      if (layer == 1) {
-        tc::fence_async_smem();
-        __syncthreads();
-        tc::mma(acc, 0, a_hi, a_lo, w2h, w2l, MX_H, MX_H, 3, 0);
-        tc::arrive(bar);
-        tc::mbar_wait(bar, phase);
-        phase ^= 1;
-      }
-      float v[64];
-      tc::ld_row(acc, 0, tid, v);
-      const float* bs = par_s + layer * 3 * MX_H;
-#pragma unroll
-      for (int c = 0; c < 64; ++c) { const float z = v[c] + bs[c]; v[c] = a.act_tanh ? tanhf(z) : fmaxf(z, 0.f); }
-      const float mu = tc_sum64(v) * (1.f / 64.f);
-      const float rs = rsqrtf(tc_sumsq64(v, mu, 64) * (1.f / 64.f) + MX_LN_EPS);
-      float* u_out = layer == 0 ? a.u1 : a.u2;
-      float* st_out = layer == 0 ? a.st1 : a.st2;
-      if (live && ok && u_out) {
-#pragma unroll
-        for (int c4 = 0; c4 < 16; ++c4) *reinterpret_cast<float4*>(u_out + (size_t)m * MX_H + 4 * c4) = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-        if (st_out) { st_out[2 * (size_t)m] = mu; st_out[2 * (size_t)m + 1] = rs; }
-      }
-#pragma unroll
-      for (int c = 0; c < 64; ++c) v[c] = (v[c] - mu) * rs * bs[MX_H + c] + bs[2 * MX_H + c];
-      __syncthreads();          // every thread has drained its accumulator reads before the next layer's MMAs overwrite the accumulator
-      tc_put_row64(a_hi, a_lo, tid, v);
-    }
-    // ---- gi = x2 . W_ih^T + b_ih ----
-    tc::fence_async_smem();
-    __syncthreads();
-    tc::mma(acc, 0, a_hi, a_lo, wih, wil, MX_G, MX_H, 3, 0);
-    tc::arrive(bar);
-    tc::mbar_wait(bar, phase);
-    phase ^= 1;
-    float* gi = a.gi[net];
-#pragma unroll 1
-    for (int c0 = 0; c0 < MX_G; c0 += 64) {
-      float t0[64];
-      tc::ld_row(acc, c0, tid, t0);
-      if (ok) {
-#pragma unroll
-        for (int c4 = 0; c4 < 16; ++c4)
-          *reinterpret_cast<float4*>(gi + (size_t)m * MX_G + c0 + 4 * c4) =
-              make_float4(t0[4 * c4] + bih_s[c0 + 4 * c4], t0[4 * c4 + 1] + bih_s[c0 + 4 * c4 + 1], t0[4 * c4 + 2] + bih_s[c0 + 4 * c4 + 2],
-                          t0[4 * c4 + 3] + bih_s[c0 + 4 * c4 + 3]);
-      }
-    }
-    __syncthreads();     // accumulator reads drained; the A tile and the fc1 chunk buffer are free for the next tile
-  }
-}
-
-// =====================================================================================================
-// k_front_fwd_tc_wide2: the wide-input pipeline with EVERY weight operand streamed through one 32 KB chunk buffer (fc1 chunk 0, fc1
-// chunk 1, fc2, W_ih gate r, z, n -- six [64][K] hi | lo pairs per tile, copied from the L2-resident image with cp.async), so a CTA needs
-// 96 KB of shared memory and 256 accumulator columns and TWO CTAs share an SM: while one waits for an MMA, a copy or its row loads, the other
-// runs its epilogue (ncu on k_front_fwd_tc_wide at 8m: 4 warps per SM, issue-active 11 %, long-scoreboard 5 warps per issue).  The copy
+// Wide inputs (64 < in_dim <= 128: SMAC 8m / 2s3z observations): fc1's K dimension is fed in chunks of 64 columns that accumulate in the
+// accumulator, and EVERY weight operand is streamed through one 32 KB chunk buffer (fc1 chunk 0, fc1 chunk 1, fc2, W_ih gate r, z, n -- six
+// [64][K] hi | lo pairs per tile, copied from the L2-resident image with cp.async), so a CTA needs 96 KB of shared memory and 256
+// accumulator columns and TWO CTAs share an SM: while one waits for an MMA, a copy or its row loads, the other runs its epilogue (with
+// fc2 and W_ih resident, 224 KB and one CTA per SM, ncu at 8m showed 4 warps per SM, issue-active 11 %, long-scoreboard 5 warps per issue).  The copy
 // of chunk i + 1 is issued as soon as the MMAs of chunk i have completed, i.e. it flies during the epilogue between them; the three gate
 // blocks of gi accumulate in their own accumulator columns, so the epilogue of gate g overlaps the copy of gate g + 1.
 // =====================================================================================================
-struct FrontTcWide2Smem { int o_ahi, o_alo, o_wc, total; };
-static FrontTcWide2Smem front_tc_wide2_smem() {
-  FrontTcWide2Smem s;
+struct WideTcSmem { int o_ahi, o_alo, o_wc, total; };
+static WideTcSmem wide_tc_smem() {
+  WideTcSmem s;
   s.o_ahi = 0; s.o_alo = 128 * 64 * 4; s.o_wc = 2 * 128 * 64 * 4; s.total = s.o_wc + 2 * 64 * 64 * 4;
   return s;
 }
@@ -650,7 +472,7 @@ __device__ __forceinline__ void tcw_stage(char* dst, const float* __restrict__ s
   float* d = reinterpret_cast<float*>(dst);
   for (int v = threadIdx.x; v < (nbytes >> 4); v += blockDim.x) mx_cp16(d + 4 * v, src + 4 * v);
 }
-__global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, FrontTcWide2Smem sm) {
+__global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, WideTcSmem sm) {
   MX_DYN_SMEM_RAW(smem_raw);
   __shared__ __align__(8) tc::Bar bar_s;
   __shared__ float par_s[6 * MX_H + MX_G + 2 * 128];      // b1,g1,be1,b2,g2,be2 | b_ih | feature-norm gain, bias
@@ -829,62 +651,41 @@ __global__ void __launch_bounds__(128, 2) k_front_fwd_tc_wide2(FrontFwdArgs a, F
 }
 
 int g_mx_front_tc = 1;        // 1: tensor-core 3xTF32 kernels (default), 0: FFMA kernel (mx_set_option("front_tc", 0))
-int g_mx_front_tc_threads = 256;   // inputs <= 64: 256 = two threads per accumulator row (k_front_fwd_tc2), 128 = one (k_front_fwd_tc)
-int g_mx_front_tc_wide = 1;   // 1 (default): 64 < in_dim <= 128 also runs on the tensor cores (k_front_fwd_tc_wide[2])
-int g_mx_front_tc_wide2 = 1;  // wide inputs: 1 (default) = k_front_fwd_tc_wide2 (weights streamed, two CTAs per SM), 0 = k_front_fwd_tc_wide (weights resident, one CTA per SM)
-                              // (these defaults are not yet measured on the H100)
-extern int g_mx_wgrad_tc, g_mx_wgrad_tc_wide, g_mx_front_bwd_tc_stream;      // tc_bwd.cu
-int g_mx_mixer_rm = 0;        // tuning overrides (0 = automatic): rows per thread of the mixer / backward front tiles
-int g_mx_front_bwd_rm = 0;
+extern int g_mx_wgrad_tc;      // tc_bwd.cu
 
 bool mx_front_tc_usable(int in_dim, bool have_image) {
   if (!g_mx_front_tc) return false;
-  return in_dim <= 64 || (g_mx_front_tc_wide && in_dim <= 128 && have_image);
+  return in_dim <= 64 || (in_dim <= 128 && have_image);
 }
 
 int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
-  const bool wide = a.L.in_dim > 64;
-  const int Kp = mx_round_up(a.L.in_dim, 8);
-  FrontTcSmem sm = front_tc_smem(wide ? 64 : Kp);
-  const size_t smem = (size_t)sm.total;
   const int ntiles = mx_ceil_div(a.M, 128);
-  int gx = mx_num_sms() / nets;
-  if (gx > ntiles) gx = ntiles;
   if (!a.tc_acc || a.tc_acc_cols < 256 * nets) { mx_set_error("front_fwd_tc: accumulator region missing or too small"); return 1; }
-  if (gx * nets * 256 > a.tc_acc_cols) gx = a.tc_acc_cols / (256 * nets);      // 256 accumulator columns per CTA
-  if (gx < 1) gx = 1;
-  if (wide) {
+  if (a.L.in_dim > 64) {
     if (!a.tc_img[0] || (nets > 1 && !a.tc_img[1])) { mx_set_error("front_fwd_tc_wide: weight images missing"); return 1; }
-    if (g_mx_front_tc_wide2) {
-      FrontTcWide2Smem s2 = front_tc_wide2_smem();
-      int g2 = 2 * mx_num_sms() / nets;
-      if (g2 > ntiles) g2 = ntiles;
-      if (g2 * nets * 256 > a.tc_acc_cols) g2 = a.tc_acc_cols / (256 * nets);
-      if (g2 < 1) g2 = 1;
+    WideTcSmem s2 = wide_tc_smem();
+    int g2 = 2 * mx_num_sms() / nets;
+    if (g2 > ntiles) g2 = ntiles;
+    if (g2 * nets * 256 > a.tc_acc_cols) g2 = a.tc_acc_cols / (256 * nets);
+    if (g2 < 1) g2 = 1;
 #if !MX_EMU
-      static bool configured_w2 = false;
-      if (!configured_w2) {
-        if (cudaFuncSetAttribute(k_front_fwd_tc_wide2, cudaFuncAttributeMaxDynamicSharedMemorySize, s2.total) != cudaSuccess) { mx_set_error("front_fwd_tc_wide2: smem %d too large", s2.total); return 1; }
-        configured_w2 = true;
-      }
-#endif
-      MX_LAUNCH_PDL(k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, a, s2);
-      MX_COUNT();
-      MX_MARK("k_front_fwd_tc_wide", s);
-      return MX_CHECK_LAUNCH("front_fwd_tc_wide2");
-    }
-#if !MX_EMU
-    static bool configured_w = false;
-    if (!configured_w) {
-      if (cudaFuncSetAttribute(k_front_fwd_tc_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("front_fwd_tc_wide: smem %zu too large", smem); return 1; }
-      configured_w = true;
+    static bool configured_w2 = false;
+    if (!configured_w2) {
+      if (cudaFuncSetAttribute(k_front_fwd_tc_wide2, cudaFuncAttributeMaxDynamicSharedMemorySize, s2.total) != cudaSuccess) { mx_set_error("front_fwd_tc_wide2: smem %d too large", s2.total); return 1; }
+      configured_w2 = true;
     }
 #endif
-    MX_LAUNCH_PDL(k_front_fwd_tc_wide, dim3(gx, nets), dim3(128), smem, s, a, sm);
+    MX_LAUNCH_PDL(k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, a, s2);
     MX_COUNT();
     MX_MARK("k_front_fwd_tc_wide", s);
-    return MX_CHECK_LAUNCH("front_fwd_tc_wide");
+    return MX_CHECK_LAUNCH("front_fwd_tc_wide2");
   }
+  FrontTcSmem sm = front_tc_smem(mx_round_up(a.L.in_dim, 8));
+  const size_t smem = (size_t)sm.total;
+  int gx = mx_num_sms() / nets;
+  if (gx > ntiles) gx = ntiles;
+  if (gx * nets * 256 > a.tc_acc_cols) gx = a.tc_acc_cols / (256 * nets);      // 256 accumulator columns per CTA
+  if (gx < 1) gx = 1;
 #if !MX_EMU
   static size_t configured = 0;
   if (smem > configured) {
@@ -893,7 +694,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
   }
 #endif
   // (inputs of 57..64 columns fill the 227 KB with operand tiles: the pair-exchange buffer of the 256-thread kernel no longer fits beside them)
-  if (g_mx_front_tc_threads == 256 && smem + 5 * 1024 + 256 <= 227 * 1024) {
+  if (smem + 5 * 1024 + 256 <= 227 * 1024) {
 #if !MX_EMU
     static size_t configured2 = 0;
     if (smem > configured2) {
@@ -915,14 +716,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
 extern "C" int mx_set_option(const char* name, int32_t value) {
   if (mx_set_option_common(name, value) == 0) return 0;
   if (!strcmp(name, "front_tc")) { g_mx_front_tc = value; return 0; }
-  if (!strcmp(name, "front_tc_wide")) { g_mx_front_tc_wide = value; return 0; }
-  if (!strcmp(name, "front_tc_wide2")) { g_mx_front_tc_wide2 = value; return 0; }
-  if (!strcmp(name, "front_tc_threads")) { g_mx_front_tc_threads = value; return 0; }
   if (!strcmp(name, "wgrad_tc")) { g_mx_wgrad_tc = value; return 0; }
-  if (!strcmp(name, "wgrad_tc_wide")) { g_mx_wgrad_tc_wide = value; return 0; }
-  if (!strcmp(name, "front_bwd_tc_stream")) { g_mx_front_bwd_tc_stream = value; return 0; }
-  if (!strcmp(name, "mixer_rm")) { g_mx_mixer_rm = value; return 0; }
-  if (!strcmp(name, "front_bwd_rm")) { g_mx_front_bwd_rm = value; return 0; }
 #if !MX_EMU
   if (!strcmp(name, "pdl")) { g_mx_pdl = value; return 0; }
   if (!strcmp(name, "pdl_rows")) { g_mx_pdl_rows = value; return 0; }

@@ -115,6 +115,10 @@ def test_c_abi_status_codes(emu_engine):
     lay = emu_engine.ReplayLayout()
     assert lib.mx_replay_layout_query(C.byref(cfg), C.byref(lay)) != 0 and b"non-positive" in lib.mx_last_error()
     assert lib.mx_set_option(b"mixer_split", 1) == 0
+    for retired in (b"front_tc_wide2", b"front_bwd_mma", b"gru_rows", b"hyper_late", b"side_prio", b"front_tc_threads", b"front_tc_wide",
+                    b"wgrad_tc_wide", b"front_bwd_tc_stream", b"gru_wgrad_split", b"gru_threads", b"gru_fwd_rpc", b"gru_bwd_rpc", b"mixer_rm",
+                    b"mixer_split_rm", b"front_bwd_rm"):
+        assert lib.mx_set_option(retired, 1) == 1 and b"unknown option" in lib.mx_last_error(), retired
     args, pol, tr = qc.build_trainer(QmixConfig(), 4, 4)
     b = emu_engine.Batch()
     b.B = 99

@@ -26,7 +26,8 @@ def test_random_shapes_and_options_vs_oracle(emu_engine, c):
     cfg = QmixConfig(n_agents=c["N"], obs_dim=c["O"], act_dim=c["A"], state_dim=c["S"], gain=1.0, use_per=c["per"], huber=c["hub"], huber_delta=0.6,
                      double_q=c["dq"], prev_act_inp=c["prev"])
     lib.mx_set_option(b"wgrad_tc", c["mode"])
-    lib.mx_set_option(b"front_tc_wide", c["wide"])
+    # wide = 0: inputs wider than 64 take the FFMA forward, narrower ones the tensor cores
+    lib.mx_set_option(b"front_tc", 0 if not c["wide"] and c["O"] + (c["A"] if c["prev"] else 0) > 64 else 1)
     try:
         L, args, pol, tr = qc.oracle_and_trainer(cfg, c["B"], c["T"], debug=False)
         w = np.random.RandomState(c["it"]).rand(c["B"]) * 0.9 + 0.1 if c["per"] else None
@@ -34,7 +35,7 @@ def test_random_shapes_and_options_vs_oracle(emu_engine, c):
         qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=2e-2)
     finally:
         lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide", 1)
+        lib.mx_set_option(b"front_tc", 1)
 
 
 @pytest.mark.parametrize("wgrad_tc", [0, 2], ids=["default", "tc_backward"])

@@ -1,8 +1,10 @@
 """QMIX learner kernels' logic on the CPU fiber emulator vs the reference goldens (and the oracle's trace)."""
 import numpy as np
 import pytest
+import torch
 
 import qmix_checks as qc
+from helpers import rel_err
 
 
 @pytest.mark.parametrize("name", ["qmix_small", "qmix_small_huber_nodq", "qmix_small_per", "qmix_small_hyper1", "qmix_5ag"])
@@ -154,107 +156,86 @@ def test_tanh_networks_match_reference_golden(emu_engine, opts):
         lib.mx_set_option(b"wgrad_tc", -1)
 
 
-@pytest.mark.parametrize("threads", [128, 256])
-@pytest.mark.parametrize("name,debug", [("qmix_small", True), ("qmix_small", False), ("qmix_5ag", False), ("qmix_small_per", False)])
-def test_recurrence_kernel_variants_match_reference_golden(emu_engine, name, debug, threads):
-    """Both CTA widths of the GRU recurrences (option gru_threads: the 128-thread kernels k_gru_fwd2 / k_gru_bwd2 are picked when all rows
-    are resident at once, the 256-thread ones otherwise) against the reference goldens, intermediates included."""
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"gru_threads", threads)
-    try:
-        qc.check_step_against(None, name, intermediates=True, debug=debug)
-    finally:
-        lib.mx_set_option(b"gru_threads", 0)
-
-
-@pytest.mark.parametrize("name,debug", [("qmix_small", True), ("qmix_5ag", False), ("qmix_small_per", False), ("qmix_small_tanh", True)])
-def test_two_rows_per_cta_recurrences_match_reference_golden(emu_engine, name, debug):
-    """Option gru_rows = 2: k_gru_fwd2<2> / k_gru_bwd2<2> carry two sequence rows per CTA through the same register-resident W_hh slice (picked
-    automatically when there are more row-CTAs than two per SM hold at once: SMAC 8m).  Intermediates included; odd row counts leave
-    the last CTA with one empty slot."""
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"gru_rows", 2)
-    try:
-        qc.check_step_against(None, name, intermediates=True, debug=debug)
-    finally:
-        lib.mx_set_option(b"gru_rows", 0)
-
-
-def test_two_rows_per_cta_recurrences_odd_row_count_vs_oracle(emu_engine):
+@pytest.mark.parametrize("B,N,T", [(2, 2, 5), (4, 2, 5), (5, 3, 5), (8, 3, 5), (2, 2, 9), (4, 2, 9), (5, 3, 9), (8, 3, 9)])
+def test_recurrence_kernel_families_vs_oracle(emu_engine, B, N, T):
+    """Both CTA widths of the GRU recurrences, picked by sequence length.  T = 5: the 256-thread k_gru_fwd / k_gru_bwd with 1, 2 or 4 rows
+    per CTA from the row count (R = B N = 4, 8, 15, 24 on the emulator's 4 SMs: forward 1 / 2 / 4 / 4, backward 1 / 1 / 2 / 4).  T = 9: the
+    128-thread k_gru_fwd2 / k_gru_bwd2, one row per CTA.  Forward intermediates, then two steps in lock-step with the oracle."""
     from oracle.qmix import QmixConfig, synth_batch
-    lib = emu_engine.lib()
-    cfg = QmixConfig(n_agents=3, obs_dim=9, act_dim=5, state_dim=11, gain=1.0)
-    B, T = 5, 9            # 15 rows: the eighth CTA of each net has one row and one empty slot
-    lib.mx_set_option(b"gru_rows", 2)
-    try:
-        L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T)
-        batch = synth_batch(cfg, B, T, seed=21, avail_p=0.8, var_len=True) + (None, None)
-        qc.compare_step(L, pol, tr, batch, cfg, steps=2)
-    finally:
-        lib.mx_set_option(b"gru_rows", 0)
+    cfg = QmixConfig(n_agents=N, obs_dim=11, act_dim=5, state_dim=13, gain=1.0)
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T)
+    batch = synth_batch(cfg, B, T, seed=21, avail_p=0.8, var_len=True) + (None, None)
+    for s in range(2):
+        info, prio, _ = tr.train_policy_on_batch(qc.ref_tuple(batch))
+        if s == 0:
+            bad = qc.check_forward_intermediates(tr, L, batch, cfg, B, T)
+            assert not bad, bad
+        qc.check_engine_step(L, pol, tr, batch, cfg, info, prio, {k: v.clone() for k, v in tr.grad_views().items()}, s)
 
 
-@pytest.mark.parametrize("name", ["maddpg_box", "matd3_disc_avail"])
-def test_recurrence_kernel_128_threads_maddpg(emu_engine, name):
-    """R-MADDPG uses the recurrences with an initial state (branch steps, h0) and T1 != T + 1: the 128-thread kernels on those paths."""
-    import maddpg_checks as mdc
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"gru_threads", 128)
-    try:
-        mdc.check_golden(name)
-        lib.mx_set_option(b"gru_rows", 2)          # two rows per CTA on the same paths (initial state h0, T1 != T + 1)
-        mdc.check_golden(name)
-    finally:
-        lib.mx_set_option(b"gru_threads", 0)
-        lib.mx_set_option(b"gru_rows", 0)
+@pytest.mark.parametrize("td3,disc", [(False, False), (True, True)])
+def test_recurrence_kernel_128_threads_maddpg(emu_engine, td3, disc):
+    """R-MADDPG / R-MATD3 at T = 9: the 128-thread recurrences run the actor (T1 = T + 1) and the critic over the buffer sequence, whose
+    backward stores T1 = T steps per sequence (the one-step branch rows with an initial state stay on the 256-thread kernels).  Three
+    updates against the oracle: losses, grad norms, every critic gradient tensor, all four networks."""
+    import maddpg_checks as mc
+    from oracle.maddpg import MaddpgConfig, MaddpgLearner, synth_batch_cont, synth_batch_disc, sample_gumbel
+    from oracle.qmix import randomize_all
+    cfg = MaddpgConfig(act_dim=5 if disc else 2, discrete=disc, td3=td3, actor_update_interval=2 if td3 else 1, gain=1.0)
+    B, T = 4, 9
+    L = MaddpgLearner(cfg, seed=5)
+    randomize_all(L.actor, 1); randomize_all(L.critic, 2)
+    L.sync_targets()
+    randomize_all(L.tgt_actor, 3, 0.05); randomize_all(L.tgt_critic, 4, 0.05)
+    args, pol, tr = mc.build(cfg, B, T)
+    for ours, ref in ((pol.actor, L.actor), (pol.critic, L.critic), (pol.target_actor, L.tgt_actor), (pol.target_critic, L.tgt_critic)):
+        ours.load_state_dict(ref.state_dict())
+    for s in range(3):
+        batch = (synth_batch_disc if disc else synth_batch_cont)(cfg, B, T, seed=40 + s) + (None, None)
+        upd = s % cfg.actor_update_interval == 0
+        torch.manual_seed(77 + s)
+        if disc:
+            noise = sample_gumbel((T + 1, cfg.n_agents * B, cfg.act_dim)).numpy() if td3 else None
+            anoise = sample_gumbel((T, cfg.n_agents * B, cfg.act_dim)).numpy() if upd else None
+        else:
+            noise = torch.empty(T + 1, cfg.n_agents * B, cfg.act_dim).normal_(mean=0, std=cfg.target_noise).numpy() if td3 else None
+            anoise = None
+        torch.manual_seed(77 + s)
+        info, _, _ = tr.shared_train_policy_on_batch("policy_0", mc.ref_tuple(batch))
+        ref, _ = L.step(batch, noise, anoise)
+        assert rel_err(info["critic_loss"].cpu(), ref["critic_loss"]) < 1e-4
+        assert rel_err(info["critic_grad_norm"].cpu(), ref["critic_grad_norm"]) < 1e-4
+        ga, gc = tr.grad_views()
+        coef = min(1.0, cfg.max_grad_norm / (float(ref["critic_grad_norm"]) + 1e-6))
+        cviews = mc.named_views(gc, pol._c_entries)
+        for k, gr in L.critic_grads.items():
+            ok, err, lim = qc.close(cviews[k] / gc[pol.Pc] * coef, gr, 1e-4)
+            assert ok, (s, k, err, lim)
+        assert bool(info["update_actor"]) == bool(ref["update_actor"]) == upd
+        if ref["update_actor"]:
+            assert rel_err(info["actor_loss"].cpu(), ref["actor_loss"]) < 1e-4
+            assert rel_err(info["actor_grad_norm"].cpu(), ref["actor_grad_norm"]) < 2e-4
+            pol.soft_target_updates()
+            L.soft_update()
+    for ours, ref in ((pol.actor, L.actor), (pol.critic, L.critic), (pol.target_actor, L.tgt_actor), (pol.target_critic, L.tgt_critic)):
+        for k, v in ours.state_dict().items():
+            assert float((v.cpu() - ref.state_dict()[k]).abs().max()) <= 5e-3 * cfg.lr * 3 + 1e-7, k
 
 
-@pytest.mark.parametrize("threads", [128, 256])
-@pytest.mark.parametrize("name", ["qmix_small", "qmix_small_prev_act", "qmix_small_tanh"])
-def test_front_tensor_core_kernel_variants_match_reference_golden(emu_engine, name, threads):
-    """k_front_fwd_tc (one thread per accumulator row) and k_front_fwd_tc2 (two threads per row, pair-wise LayerNorm statistics): option
-    front_tc_threads, default 256."""
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"front_tc_threads", threads)
-    try:
-        qc.check_step_against(None, name, intermediates=(name != "qmix_small_prev_act"), debug=True)
-    finally:
-        lib.mx_set_option(b"front_tc_threads", 256)
-
-
-@pytest.mark.parametrize("split", [0, 1])
-@pytest.mark.parametrize("name", ["qmix_small", "qmix_5ag", "qmix_small_per", "qmix_small_tanh"])
-def test_gru_weight_gradient_kernel_split_matches_reference_golden(emu_engine, name, split):
-    """Option gru_wgrad_split: dW_ih / dW_hh / db_ih / db_hh from k_gru_wgrad (its own kernel, launched beside k_front_bwd on the GPU;
-    default) or from inside k_front_bwd (0).  Same gradient partial rows either way; one more launch per step with the split."""
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"gru_wgrad_split", split)
-    lib.mx_set_option(b"wgrad_tc", 0)
-    try:
-        c0 = lib.mx_launch_count()
-        qc.check_step_against(None, name, intermediates=False, debug=False)
-        n = lib.mx_launch_count() - c0
-    finally:
-        lib.mx_set_option(b"gru_wgrad_split", 1)
-        lib.mx_set_option(b"wgrad_tc", -1)
-    test_gru_weight_gradient_kernel_split_matches_reference_golden.counts[(name, split)] = n
-    both = test_gru_weight_gradient_kernel_split_matches_reference_golden.counts
-    if (name, 0) in both and (name, 1) in both:
-        assert both[(name, 1)] > both[(name, 0)], both
-
-
-test_gru_weight_gradient_kernel_split_matches_reference_golden.counts = {}
-
-
-@pytest.mark.parametrize("mma", [0, 1])
-@pytest.mark.parametrize("name", ["qmix_small", "qmix_5ag", "qmix_small_nofn"])
-def test_front_backward_gemm_variants_match_reference_golden(emu_engine, name, mma):
-    """k_front_bwd with its GEMMs on mma.sync 3xTF32 tiles (csrc/mx_mma.cuh, default) and on the FFMA micro-kernels (option front_bwd_mma)."""
-    lib = emu_engine.lib()
-    lib.mx_set_option(b"front_bwd_mma", mma)
-    lib.mx_set_option(b"wgrad_tc", 0)
-    try:
-        qc.check_step_against(None, name, intermediates=False, debug=False)
-    finally:
-        lib.mx_set_option(b"front_bwd_mma", 0)
-        lib.mx_set_option(b"wgrad_tc", -1)
+@pytest.mark.parametrize("obs,prev,relu", [(57, False, True), (60, False, False), (64, False, True), (64, False, False), (50, True, True),
+                                           (55, True, False)])
+def test_one_thread_per_row_front_kernel_vs_oracle(emu_engine, obs, prev, relu):
+    """Input widths 57 .. 64 (with --prev_act_inp: observation + 9 actions) fill the shared memory with operand tiles, so the pair-exchange
+    buffer of k_front_fwd_tc2 no longer fits and the launcher takes k_front_fwd_tc (one thread per accumulator row); ReLU and tanh blocks.
+    Forward intermediates (without the previous-action input, which the oracle's trace does not stack), then two steps in lock-step."""
+    from oracle.qmix import QmixConfig, synth_batch
+    cfg = QmixConfig(n_agents=3, obs_dim=obs, act_dim=9, state_dim=20, gain=1.0, prev_act_inp=prev, relu=relu)
+    B, T = 5, 6
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T)
+    batch = synth_batch(cfg, B, T, seed=8, avail_p=0.8, var_len=True) + (None, None)
+    for s in range(2):
+        info, prio, _ = tr.train_policy_on_batch(qc.ref_tuple(batch))
+        if s == 0 and not prev:
+            bad = qc.check_forward_intermediates(tr, L, batch, cfg, B, T)
+            assert not bad, bad
+        qc.check_engine_step(L, pol, tr, batch, cfg, info, prio, {k: v.clone() for k, v in tr.grad_views().items()}, s)

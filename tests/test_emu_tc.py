@@ -42,29 +42,24 @@ def test_qmix_step_front_paths_match_reference_golden(emu_engine, front_tc):
 @pytest.mark.parametrize("obs_dim", [65, 80, 100, 128])
 def test_wide_input_front_kernel_vs_oracle(emu_engine, obs_dim):
     """64 < obs_dim <= 128 (SMAC 8m / 2s3z observations are 80 wide): fc1's K dimension fed to the tensor core in two chunks that
-    accumulate in the accumulator (k_front_fwd_tc_wide, option front_tc_wide).  More than 128 rows so a CTA runs several tiles."""
+    accumulate in the accumulator (k_front_fwd_tc_wide2).  More than 128 rows so a CTA runs several tiles."""
     from oracle.qmix import QmixConfig, synth_batch
-    lib = emu_engine.lib()
     cfg = QmixConfig(n_agents=5, obs_dim=obs_dim, act_dim=6, state_dim=20, gain=1.0)
     B, T = 12, 5           # 12 * 6 * 5 = 360 rows: 3 tiles for the 2 CTAs per net of the emulator's 4 "SMs"
-    lib.mx_set_option(b"front_tc_wide", 1)
-    try:
-        L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
-        batch = synth_batch(cfg, B, T, seed=4, avail_p=0.7, var_len=True) + (None, None)
-        # parameter bound 1e-2 * lr: an element with |g| ~ eps sees Adam amplify a 1e-6-relative gradient difference (measured 5.3e-3 * lr
-        # at obs 100, with the gradients themselves equal to 9e-7 of their maximum)
-        qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
-    finally:
-        lib.mx_set_option(b"front_tc_wide", 1)
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
+    batch = synth_batch(cfg, B, T, seed=4, avail_p=0.7, var_len=True) + (None, None)
+    # parameter bound 1e-2 * lr: an element with |g| ~ eps sees Adam amplify a 1e-6-relative gradient difference (measured 5.3e-3 * lr
+    # at obs 100, with the gradients themselves equal to 9e-7 of their maximum)
+    qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
 
 
-def test_wide_input_kernel_is_what_runs(emu_engine):
+def test_front_tc_selects_the_wide_tensor_core_kernel(emu_engine):
     from oracle.qmix import QmixConfig, synth_batch
     lib = emu_engine.lib()
     cfg = QmixConfig(n_agents=2, obs_dim=80, act_dim=4, state_dim=10, gain=1.0)
     names = {}
     for opt in (0, 1):
-        lib.mx_set_option(b"front_tc_wide", opt)
+        lib.mx_set_option(b"front_tc", opt)
         try:
             L, args, pol, tr = qc.oracle_and_trainer(cfg, 3, 2, debug=False)
             import ctypes as C
@@ -75,7 +70,7 @@ def test_wide_input_kernel_is_what_runs(emu_engine):
             n = lib.mx_profile_end(None, buf, 8192, ms, 128)
             names[opt] = buf.value.decode().split(";")[:n]
         finally:
-            lib.mx_set_option(b"front_tc_wide", 1)
+            lib.mx_set_option(b"front_tc", 1)
     assert "k_front_fwd" in names[0] and "k_front_fwd_tc_wide" not in names[0]
     assert "k_front_fwd_tc_wide" in names[1] and "k_front_fwd" not in names[1] and "k_tc_prep_weights" in names[1]
 
@@ -136,7 +131,6 @@ def test_tensor_core_backward_wide_inputs_vs_oracle(emu_engine, obs_dim, mode):
     lib = emu_engine.lib()
     cfg = QmixConfig(n_agents=5, obs_dim=obs_dim, act_dim=6, state_dim=20, gain=1.0)
     B, T = 24, 5           # 720 rows: 6 tiles / 12 chunks on the emulator's 4 "SMs"
-    lib.mx_set_option(b"front_tc_wide", 1)
     lib.mx_set_option(b"wgrad_tc", mode)
     try:
         L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
@@ -144,29 +138,6 @@ def test_tensor_core_backward_wide_inputs_vs_oracle(emu_engine, obs_dim, mode):
         qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
     finally:
         lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide", 1)
-
-
-@pytest.mark.parametrize("obs_dim", [80, 128])
-def test_resident_weight_variants_of_the_wide_kernels_vs_oracle(emu_engine, obs_dim):
-    """The defaults stream every weight operand through one chunk buffer so that two CTAs share an SM (k_front_fwd_tc_wide2; k_front_bwd_tc
-    in streamed mode, its LayerNorm sums folded in by k_wgrad_tc from the side array).  Options front_tc_wide2 = 0 / front_bwd_tc_stream = 0
-    select the one-CTA-per-SM kernels with resident weights: same results."""
-    from oracle.qmix import QmixConfig, synth_batch
-    lib = emu_engine.lib()
-    cfg = QmixConfig(n_agents=5, obs_dim=obs_dim, act_dim=6, state_dim=20, gain=1.0)
-    B, T = 24, 5
-    lib.mx_set_option(b"front_tc_wide2", 0)
-    lib.mx_set_option(b"front_bwd_tc_stream", 0)
-    lib.mx_set_option(b"wgrad_tc", 2)
-    try:
-        L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
-        batch = synth_batch(cfg, B, T, seed=4, avail_p=0.7, var_len=True) + (None, None)
-        qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
-    finally:
-        lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide2", 1)
-        lib.mx_set_option(b"front_bwd_tc_stream", 1)
 
 
 def test_config2_full_size_all_tensor_core_kernels_vs_oracle(emu_engine):
@@ -191,13 +162,13 @@ def test_config2_full_size_all_tensor_core_kernels_vs_oracle(emu_engine):
 @pytest.mark.parametrize("name", ["maddpg_box", "matd3_box", "maddpg_disc", "matd3_disc_avail", "maddpg_box_per", "matd3_disc_nofn", "maddpg_box_tanh"])
 def test_maddpg_updates_through_the_tensor_core_backward(emu_engine, name, mode):
     """R-MADDPG / R-MATD3: the critic's (input 60 / 69 wide) and the actor's (18 wide) weight-gradient passes on k_wgrad_tc /
-    k_front_bwd_tc; the frozen-critic pass that only needs the action gradient stays on k_front_bwd."""
+    k_front_bwd_tc; the frozen-critic pass that only needs the action gradient stays on k_front_bwd.  R-MADDPG passes no side array for
+    the LayerNorm sums, so mode 2 runs k_front_bwd_tc with resident weights for inputs up to 64 (actor, Box critic) and 65 .. 128
+    (Discrete critic)."""
     import maddpg_checks as mc
     lib = emu_engine.lib()
-    lib.mx_set_option(b"front_tc_wide", 1)
     lib.mx_set_option(b"wgrad_tc", mode)
     try:
         mc.check_golden(name)
     finally:
         lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide", 1)

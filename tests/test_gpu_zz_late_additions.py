@@ -88,27 +88,23 @@ def test_network_structure_flags_maddpg(gpu_engine, name):
 
 @pytest.mark.parametrize("obs_dim,n_agents,B,T", [(80, 8, 8, 20), (128, 3, 16, 12), (72, 5, 32, 10)])
 def test_wide_input_tensor_core_front_kernel_vs_oracle(gpu_engine, obs_dim, n_agents, B, T):
-    """k_front_fwd_tc_wide (64 < obs_dim <= 128, option front_tc_wide, off by default until timed): emulator-verified indexing; this is its
-    first run on real tensor cores.  Runs under a launch-count check that the wide kernel, not the FFMA one, executed."""
+    """k_front_fwd_tc_wide2 (64 < obs_dim <= 128): emulator-verified indexing on real tensor cores.  Runs under a launch-list check that
+    the wide kernel, not the FFMA one, executed."""
     import ctypes as C
     import numpy as np
     from oracle.qmix import QmixConfig, synth_batch
     lib = gpu_engine.lib()
     cfg = QmixConfig(n_agents=n_agents, obs_dim=obs_dim, act_dim=7, state_dim=40, gain=1.0)
-    lib.mx_set_option(b"front_tc_wide", 1)
-    try:
-        L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
-        tr.use_step_graph = False
-        batch = synth_batch(cfg, B, T, seed=4, avail_p=0.7, var_len=True) + (None, None)
-        lib.mx_profile_begin(gpu_engine.stream_ptr())
-        qc.compare_step(L, pol, tr, batch, cfg, steps=1, param_tol=1e-2)
-        buf = C.create_string_buffer(8192)
-        ms = (C.c_float * 256)()
-        n = lib.mx_profile_end(gpu_engine.stream_ptr(), buf, 8192, ms, 256)
-        assert "k_front_fwd_tc_wide" in buf.value.decode().split(";")[:n]
-        qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
-    finally:
-        lib.mx_set_option(b"front_tc_wide", 1)
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
+    tr.use_step_graph = False
+    batch = synth_batch(cfg, B, T, seed=4, avail_p=0.7, var_len=True) + (None, None)
+    lib.mx_profile_begin(gpu_engine.stream_ptr())
+    qc.compare_step(L, pol, tr, batch, cfg, steps=1, param_tol=1e-2)
+    buf = C.create_string_buffer(8192)
+    ms = (C.c_float * 256)()
+    n = lib.mx_profile_end(gpu_engine.stream_ptr(), buf, 8192, ms, 256)
+    assert "k_front_fwd_tc_wide" in buf.value.decode().split(";")[:n]
+    qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
 
 
 @pytest.mark.parametrize("mode", [1, 2])
@@ -161,7 +157,6 @@ def test_tensor_core_backward_wide_inputs_vs_oracle(gpu_engine, obs_dim, n_agent
     from oracle.qmix import QmixConfig, synth_batch
     lib = gpu_engine.lib()
     cfg = QmixConfig(n_agents=n_agents, obs_dim=obs_dim, act_dim=11, state_dim=60, gain=1.0)
-    lib.mx_set_option(b"front_tc_wide", 1)
     lib.mx_set_option(b"wgrad_tc", mode)
     try:
         L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=False)
@@ -170,7 +165,6 @@ def test_tensor_core_backward_wide_inputs_vs_oracle(gpu_engine, obs_dim, n_agent
         qc.compare_step(L, pol, tr, batch, cfg, steps=2, param_tol=1e-2)
     finally:
         lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide", 1)
 
 
 @pytest.mark.parametrize("mode", [1, 2])
@@ -178,13 +172,11 @@ def test_tensor_core_backward_wide_inputs_vs_oracle(gpu_engine, obs_dim, n_agent
 def test_maddpg_updates_through_the_tensor_core_backward(gpu_engine, name, mode):
     import maddpg_checks as mc
     lib = gpu_engine.lib()
-    lib.mx_set_option(b"front_tc_wide", 1)
     lib.mx_set_option(b"wgrad_tc", mode)
     try:
         mc.check_golden(name)
     finally:
         lib.mx_set_option(b"wgrad_tc", -1)
-        lib.mx_set_option(b"front_tc_wide", 1)
 
 
 @pytest.mark.parametrize("name", ["maddpg_multi_disc", "matd3_multi_box", "matd3_multi_disc"])
