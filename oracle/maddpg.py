@@ -62,7 +62,7 @@ def onehot_of_max(x, avail=None):
     """`onehot_from_logits` without exploration (util.py:106-118): every maximal entry is hot; unavailable -> -1e10."""
     if avail is not None:
         x = torch.where(avail == 0, torch.full_like(x, -1e10), x)
-    return (x == x.max(dim=-1, keepdim=True)[0]).float()
+    return (x == x.max(dim=-1, keepdim=True)[0]).to(x.dtype)
 
 
 def hard_gumbel_softmax(logits, gumbel, avail=None):
@@ -95,7 +95,7 @@ class ActorNet(nn.Module):
 
     def forward(self, x, h0=None):
         if h0 is None:
-            h0 = torch.zeros(x.shape[1], self.hidden)
+            h0 = torch.zeros(x.shape[1], self.hidden, dtype=x.dtype)
         y, hT = self.rnn(x, h0[None])
         return self.act.action_out(y), hT
 
@@ -113,7 +113,7 @@ class CriticNet(nn.Module):
         if not seq:
             s, a = s[None], a[None]
         if h0 is None:
-            h0 = torch.zeros(s.shape[1], self.hidden)
+            h0 = torch.zeros(s.shape[1], self.hidden, dtype=s.dtype)
         y, hT = self.rnn(torch.cat([s, a], dim=2), h0[None])
         qs = [q(y) for q in self.q_outs]
         if not seq:
@@ -125,10 +125,13 @@ class MaddpgLearner(object):
     """Batch = (obs (N,T+1,B,O), share (T+1,B,S), acts (N,T,B,Ac), rewards (N,T,B,1), dones (N,T,B,1), dones_env (T,B,1),
     avail None, weights (B,) | None, idx | None)."""
 
-    def __init__(self, cfg, seed=1):
+    def __init__(self, cfg, seed=1, dtype=torch.float32):
+        """dtype: float32 is the reference's arithmetic; float64 runs the whole update (batch, noise, networks, both Adams, clipping,
+        Polyak) in double precision from the same float32-drawn initial values (tests/row_coverage_checks.py)."""
         self.cfg = cfg
-        self.actor = init_like_reference(ActorNet(cfg), cfg, seed)
-        self.critic = init_like_reference(CriticNet(cfg), cfg, seed + 1)
+        self.dtype = dtype
+        self.actor = init_like_reference(ActorNet(cfg), cfg, seed).to(dtype)
+        self.critic = init_like_reference(CriticNet(cfg), cfg, seed + 1).to(dtype)
         self.sync_targets()
         kw = dict(lr=cfg.lr, eps=cfg.opti_eps, weight_decay=cfg.weight_decay)
         self.actor_opt = torch.optim.Adam(self.actor.parameters(), **kw)
@@ -139,15 +142,14 @@ class MaddpgLearner(object):
         self.tgt_actor = copy.deepcopy(self.actor)
         self.tgt_critic = copy.deepcopy(self.critic)
 
-    @staticmethod
-    def stack(x):
-        x = torch.as_tensor(x, dtype=torch.float32)
+    def stack(self, x):
+        x = torch.as_tensor(x, dtype=getattr(self, "dtype", torch.float32))
         return torch.cat(list(x), dim=-2)          # (N,T,B,D) -> (T, N*B, D), row = n*B + b
 
     def _loss(self, e):
         if self.cfg.huber:
             d = self.cfg.huber_delta
-            small = (e.abs() <= d).float()
+            small = (e.abs() <= d).to(e.dtype)
             return small * e ** 2 / 2 + (1 - small) * d * (e.abs() - d / 2)
         return e ** 2
 
@@ -155,11 +157,12 @@ class MaddpgLearner(object):
         cfg = self.cfg
         obs, share, acts, rew, dones, dones_env, avail, weights, _idx = batch
         N, B, T = cfg.n_agents, obs.shape[2], acts.shape[1]
-        t32 = lambda x: torch.as_tensor(x, dtype=torch.float32)
+        dt = self.dtype
+        t32 = lambda x: torch.as_tensor(x, dtype=dt)
         s = t32(share)
         de = t32(dones_env)
         r = t32(rew[0])
-        curr = torch.cat([torch.zeros(1, B, 1), de[:T - 1]], 0)
+        curr = torch.cat([torch.zeros(1, B, 1, dtype=dt), de[:T - 1]], 0)
         x_all = self.stack(obs)                                        # (T+1, N*B, O)
         av_all = self.stack(avail) if (avail is not None and cfg.discrete) else None
         cent_act = torch.cat(list(t32(acts)), dim=-1)                  # (T, B, N*Ac) agents on the feature axis
@@ -178,7 +181,7 @@ class MaddpgLearner(object):
         q_seq, _ = self.critic(s[:-1], cent_act)
         # 3. target Q
         with torch.no_grad():
-            h = torch.zeros(B, cfg.hidden)
+            h = torch.zeros(B, cfg.hidden, dtype=dt)
             nq = []
             for t in range(T):
                 _, h = self.tgt_critic(s[t], cent_act[t], h)
@@ -187,6 +190,7 @@ class MaddpgLearner(object):
             nq = (1 - de) * torch.stack(nq)
         target = (r + cfg.gamma * nq) * (1 - curr)
         errs = [q * (1 - curr) - target for q in q_seq]
+        self.critic_errs = [e.detach() for e in errs]                  # (T, B, 1) per head: the TD errors of this update
         denom = (1 - curr).sum()
         prio = None
         if cfg.use_per:
@@ -212,8 +216,8 @@ class MaddpgLearner(object):
                 a_seq = hard_gumbel_softmax(a_seq, t32(actor_noise), None if av_all is None else av_all[:-1])
             agent_a = a_seq.split(B, dim=1)
             buf_a = list(t32(acts))
-            dm = torch.cat([torch.cat([torch.zeros(1, B, 1), t32(dones[i])[:T - 1]], 0) for i in range(N)], dim=1)   # (T, N*B, 1)
-            h = torch.zeros(N * B, cfg.hidden)
+            dm = torch.cat([torch.cat([torch.zeros(1, B, 1, dtype=dt), t32(dones[i])[:T - 1]], 0) for i in range(N)], dim=1)   # (T, N*B, 1)
+            h = torch.zeros(N * B, cfg.hidden, dtype=dt)
             s_rep = s[:-1].repeat(1, N, 1)
             batch_cent = cent_act.repeat(1, N, 1)
             repl = []

@@ -52,11 +52,13 @@ class MqmixLearner(object):
     acts (N,B,A), rewards (N,B,1), nobs (N,B,O), nshare (B,S), dones (N,B,1), dones_env (B,1), valid (N,B,1), avail (N,B,A) | None,
     navail (N,B,A) | None, weights (B,) | None, idx | None."""
 
-    def __init__(self, cfg, seed=1, device="cpu"):
+    def __init__(self, cfg, seed=1, device="cpu", dtype=torch.float32):
+        """dtype: as oracle.qmix.QmixLearner (float64: the whole step in double precision, same initial values)."""
         self.cfg = cfg
         self.device = torch.device(device)
-        self.agent = init_like_reference(MAgentNet(cfg), cfg, seed).to(self.device)
-        self.mixer = (VDNMixerNet() if cfg.vdn else init_like_reference(QMixerNet(cfg), cfg, seed + 1)).to(self.device)
+        self.dtype = dtype
+        self.agent = init_like_reference(MAgentNet(cfg), cfg, seed).to(self.device, dtype)
+        self.mixer = (VDNMixerNet() if cfg.vdn else init_like_reference(QMixerNet(cfg), cfg, seed + 1)).to(self.device, dtype)
         self.sync_targets()
         self.params = list(self.agent.parameters()) + list(self.mixer.parameters())      # mqmix.py:57-63
         self.opt = torch.optim.Adam(self.params, lr=cfg.lr, eps=cfg.opti_eps)
@@ -67,15 +69,15 @@ class MqmixLearner(object):
 
     def _stack(self, x):
         """(N,B,D) -> (N*B, D), row = n*B + b (mqmix.py:100-103)."""
-        return torch.as_tensor(np.asarray(x), dtype=torch.float32).to(self.device).reshape(-1, np.asarray(x).shape[-1])
+        return torch.as_tensor(np.asarray(x), dtype=self.dtype).to(self.device).reshape(-1, np.asarray(x).shape[-1])
 
     def loss_terms(self, batch):
-        cfg, dev = self.cfg, self.device
+        cfg, dev, dt = self.cfg, self.device, self.dtype
         obs, share, acts, rew, nobs, nshare, _dones, dones_env, _valid, _avail, navail, weights, _idx = batch
         B = np.asarray(obs).shape[1]
-        s = torch.as_tensor(np.asarray(share), dtype=torch.float32).to(dev)
-        ns = torch.as_tensor(np.asarray(nshare), dtype=torch.float32).to(dev)
-        de = torch.as_tensor(np.asarray(dones_env), dtype=torch.float32).to(dev)
+        s = torch.as_tensor(np.asarray(share), dtype=dt).to(dev)
+        ns = torch.as_tensor(np.asarray(nshare), dtype=dt).to(dev)
+        de = torch.as_tensor(np.asarray(dones_env), dtype=dt).to(dev)
         x, nx, a = self._stack(obs), self._stack(nobs), self._stack(acts)
         nav = self._stack(navail) if navail is not None else None
 
@@ -95,13 +97,13 @@ class MqmixLearner(object):
             tq = torch.cat(tq.split(B, dim=-2), dim=-1)                          # (B, N)
             q_tot_next = self.tgt_mixer(tq.unsqueeze(0), ns.unsqueeze(0))[0]     # (B, 1)
         q_tot = self.mixer(q_taken.unsqueeze(0), s.unsqueeze(0))[0]              # (B, 1)
-        r = torch.as_tensor(np.asarray(rew)[0], dtype=torch.float32).to(dev)     # agent 0's stream (mqmix.py:96)
+        r = torch.as_tensor(np.asarray(rew)[0], dtype=dt).to(dev)     # agent 0's stream (mqmix.py:96)
         y = r + (1 - de) * cfg.gamma * q_tot_next                                # mqmix.py:187
         err = (q_tot - y.detach()).squeeze(-1)                                   # (B,)
         per_elem = self._huber(err) if cfg.huber else err ** 2
         prio = None
         if cfg.use_per:
-            w = torch.as_tensor(np.asarray(weights), dtype=torch.float32).to(dev)
+            w = torch.as_tensor(np.asarray(weights), dtype=dt).to(dev)
             loss = (per_elem * w).mean()                                         # mqmix.py:192-198
             prio = err.abs().detach().cpu().numpy().flatten() + cfg.per_eps
         else:
@@ -110,7 +112,7 @@ class MqmixLearner(object):
 
     def _huber(self, e):
         d = self.cfg.huber_delta
-        small = (e.abs() <= d).float()
+        small = (e.abs() <= d).to(e.dtype)
         return small * e ** 2 / 2 + (1 - small) * d * (e.abs() - d / 2)
 
     def step(self, batch):
@@ -122,6 +124,14 @@ class MqmixLearner(object):
         info = dict(loss=loss.detach(), grad_norm=gnorm.detach() if torch.is_tensor(gnorm) else torch.tensor(gnorm),
                     Q_tot=aux["q_tot"].mean().detach())
         return info, prio, aux
+
+    def grads(self, batch):
+        """Raw (unclipped) gradients, no parameter update."""
+        loss, prio, aux = self.loss_terms(batch)
+        for p in self.params:
+            p.grad = None
+        loss.backward()
+        return loss.detach(), prio, aux
 
     def soft_update(self):
         tau = self.cfg.tau

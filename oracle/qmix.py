@@ -204,14 +204,18 @@ class QmixLearner(object):
     as arrays: obs (N,T+1,B,O), share (T+1,B,S), acts (N,T,B,A), rewards (N,T,B,1),
     dones (N,T,B,1), dones_env (T,B,1), avail (N,T+1,B,A) | None, weights (B,) | None, idx | None."""
 
-    def __init__(self, cfg, seed=1, device="cpu"):
+    def __init__(self, cfg, seed=1, device="cpu", dtype=torch.float32):
         """device: "cpu" (parity oracle, CPU baseline) or a CUDA device -- the same eager PyTorch ops the reference issues with
-        `--cuda` (bench.py's secondary baseline, SURVEY.md section 8(d))."""
+        `--cuda` (bench.py's secondary baseline, SURVEY.md section 8(d)).  dtype: float32 is the reference's arithmetic; float64
+        makes every tensor of the step (batch, networks, Adam moments, clipping, Polyak) double precision, a round-off-free yardstick
+        for the kernels (tests/row_coverage_checks.py).  The initialisation is drawn in float32 either way, so a float64 learner
+        with the same seed holds the same values as a float32 one."""
         self.cfg = cfg
         self.device = torch.device(device)
+        self.dtype = dtype
         in_dim = cfg.obs_dim + cfg.act_dim if cfg.prev_act_inp else cfg.obs_dim
-        self.agent = init_like_reference(AgentNet(cfg, in_dim=in_dim), cfg, seed).to(self.device)
-        self.mixer = (VDNMixerNet() if cfg.vdn else init_like_reference(QMixerNet(cfg), cfg, seed + 1)).to(self.device)
+        self.agent = init_like_reference(AgentNet(cfg, in_dim=in_dim), cfg, seed).to(self.device, dtype)
+        self.mixer = (VDNMixerNet() if cfg.vdn else init_like_reference(QMixerNet(cfg), cfg, seed + 1)).to(self.device, dtype)
         self.sync_targets()
         self.params = list(self.agent.parameters()) + list(self.mixer.parameters())   # qmix.py:66-72
         self.opt = torch.optim.Adam(self.params, lr=cfg.lr, eps=cfg.opti_eps)
@@ -223,7 +227,7 @@ class QmixLearner(object):
     # -- forward pieces ----------------------------------------------------------
     def stack_agents(self, x):
         """(N,T,B,D) -> (T, N*B, D), row = n*B + b (qmix.py:108-109)."""
-        x = torch.as_tensor(x, dtype=torch.float32).to(getattr(self, "device", "cpu"))
+        x = torch.as_tensor(x, dtype=getattr(self, "dtype", torch.float32)).to(getattr(self, "device", "cpu"))
         return torch.cat(list(x), dim=-2)
 
     def loss_terms(self, batch):
@@ -231,14 +235,14 @@ class QmixLearner(object):
         obs, share, acts, rew, _dones, dones_env, avail, weights, _idx = batch
         B = obs.shape[2]
         T = acts.shape[1]
-        dev = self.device
-        s = torch.as_tensor(share, dtype=torch.float32).to(dev)
-        de = torch.as_tensor(dones_env, dtype=torch.float32).to(dev)
+        dev, dt = self.device, self.dtype
+        s = torch.as_tensor(share, dtype=dt).to(dev)
+        de = torch.as_tensor(dones_env, dtype=dt).to(dev)
         x = self.stack_agents(obs)
         a = self.stack_agents(acts)
         av = self.stack_agents(avail) if avail is not None else None
         if cfg.prev_act_inp:        # zeros at t = 0, then the buffer's actions (qmix.py:122-127)
-            x = torch.cat((x, torch.cat((torch.zeros(1, a.shape[1], a.shape[2], device=dev), a), 0)), -1)
+            x = torch.cat((x, torch.cat((torch.zeros(1, a.shape[1], a.shape[2], dtype=dt, device=dev), a), 0)), -1)
 
         q_all, _ = self.agent(x)                                   # (T+1, N*B, A)
         a_idx = a.max(dim=-1)[1]
@@ -254,15 +258,15 @@ class QmixLearner(object):
             tq = torch.cat(tq[1:].split(B, dim=-2), dim=-1)        # (T, B, N)
             q_tot_next = self.tgt_mixer(tq, s[1:])
         q_tot = self.mixer(q_taken, s[:-1])                        # (T, B, 1)
-        r = torch.as_tensor(rew[0], dtype=torch.float32).to(dev)   # agent 0's stream (qmix.py:159)
-        bad = torch.cat([torch.zeros(1, B, 1, device=dev), de[:T - 1]], 0)     # qmix.py:161
+        r = torch.as_tensor(rew[0], dtype=dt).to(dev)   # agent 0's stream (qmix.py:159)
+        bad = torch.cat([torch.zeros(1, B, 1, dtype=dt, device=dev), de[:T - 1]], 0)     # qmix.py:161
         y = r + (1 - de) * cfg.gamma * q_tot_next
         err = (q_tot - y.detach()) * (1 - bad)
         per_elem = self._huber(err) if cfg.huber else err ** 2
         denom = (1 - bad).sum()
         prio = None
         if cfg.use_per:
-            w = torch.as_tensor(weights, dtype=torch.float32).to(dev)
+            w = torch.as_tensor(weights, dtype=dt).to(dev)
             loss = (per_elem.sum(dim=0).flatten() * w).sum() / denom
             td = err.abs().detach().cpu().numpy()
             prio = ((1 - cfg.per_nu) * td.mean(axis=0) + cfg.per_nu * td.max(axis=0)).flatten() + cfg.per_eps
@@ -274,7 +278,7 @@ class QmixLearner(object):
 
     def _huber(self, e):
         d = self.cfg.huber_delta
-        small = (e.abs() <= d).float()
+        small = (e.abs() <= d).to(e.dtype)
         return small * e ** 2 / 2 + (1 - small) * d * (e.abs() - d / 2)
 
     # -- the step ------------------------------------------------------------------
@@ -322,7 +326,7 @@ def agent_trace(net, x):
         g = rb.rnn.rnn
         H = net.hidden
         gi = F.linear(x2, g.weight_ih_l0, g.bias_ih_l0)
-        h = torch.zeros(x.shape[1], H)
+        h = torch.zeros(x.shape[1], H, dtype=x.dtype, device=x.device)
         hs, rs, zs, ns, hns = [], [], [], [], []
         for t in range(x.shape[0]):
             gh = F.linear(h, g.weight_hh_l0, g.bias_hh_l0)
@@ -338,24 +342,25 @@ def agent_trace(net, x):
                     n=torch.stack(ns), hn=torch.stack(hns), y=y, q=q)
 
 
-def synth_batch(cfg, B, T, seed=0, avail_p=None, var_len=False):
-    """Synthetic batch in the reference's sample() layout (BASELINE.md §3 item 2)."""
+def synth_batch(cfg, B, T, seed=0, avail_p=None, var_len=False, dtype=np.float32):
+    """Synthetic batch in the reference's sample() layout (BASELINE.md §3 item 2).  dtype: of the returned arrays; the values are
+    drawn in float32 whatever it is, so a float64 batch holds exactly the float32 batch of the same seed."""
     rs = np.random.RandomState(seed)
     N, O, A, S = cfg.n_agents, cfg.obs_dim, cfg.act_dim, cfg.state_dim
-    obs = rs.randn(N, T + 1, B, O).astype(np.float32)
-    share = rs.randn(T + 1, B, S).astype(np.float32)
+    obs = rs.randn(N, T + 1, B, O).astype(np.float32).astype(dtype)
+    share = rs.randn(T + 1, B, S).astype(np.float32).astype(dtype)
     if avail_p is None:
-        avail = np.ones((N, T + 1, B, A), np.float32)
+        avail = np.ones((N, T + 1, B, A), dtype)
     else:
-        avail = (rs.rand(N, T + 1, B, A) < avail_p).astype(np.float32)
+        avail = (rs.rand(N, T + 1, B, A) < avail_p).astype(dtype)
         avail[..., 0] = 1.0
     # taken actions are always available ones
     logits = rs.rand(N, T, B, A) + 10.0 * avail[:, :T]
     a_idx = logits.argmax(-1)
-    acts = np.eye(A, dtype=np.float32)[a_idx]
-    r = rs.randn(T, B, 1).astype(np.float32)
+    acts = np.eye(A, dtype=dtype)[a_idx]
+    r = rs.randn(T, B, 1).astype(np.float32).astype(dtype)
     rew = np.repeat(r[None], N, axis=0)
-    dones_env = np.zeros((T, B, 1), np.float32)
+    dones_env = np.zeros((T, B, 1), dtype)
     if var_len:
         L = rs.randint(T // 2, T + 1, size=B)
         for b in range(B):

@@ -1,0 +1,576 @@
+"""Row and tile coverage of the QMIX / M-QMIX learners against a float64 oracle: shared by the emulated (CPU) and the GPU test modules.
+
+The lock-step checks (qmix_checks.check_engine_step) compare whole-batch gradients per tensor.  Rows whose gradient is zero -- the
+last N rows of every episode (step T+1 only picks the double-Q arg-max) and the padded tail of a short episode -- and rows whose share of
+a tensor is below that budget are invisible there, and those rows sit exactly at the tail of the row space, where a tile kernel that
+drops, double-counts or mis-addresses its last partial tile goes wrong.  The checks here make every row count:
+
+* isolated episodes: PER on, importance weights one-hot on episode b.  The loss is linear in the weights, so the step's gradient is
+  exactly episode b's (T+1) N agent-net rows and T mixer rows; losing one of them moves it by ~1 / (T N), not 1 / rows.
+* per-row forward: every materialised activation of every row (masked rows included), live and target net, against the float64
+  trace, bounded relative to the row's own largest magnitude.
+* batch size changing on one learner: max_batch, then 1, then a batch one tile smaller, each step against float64 (the optimiser
+  must read only the gradient partials this step wrote).
+
+`TileRules` restates the launchers' tile rules (csrc/agent_bwd.cu front_bwd_pick_rm, csrc/tc_bwd.cu, csrc/tc_linear.cu,
+csrc/mixer.cu) for an SM count, and `pick_shapes` searches (B, T, N) that put the row / transition counts on the tile edges.
+"""
+import ctypes as C
+import itertools
+
+import numpy as np
+import torch
+
+import kink
+import qmix_checks as qc
+from helpers import rel_err
+
+# Isolated-episode gradients: max |engine - float64| <= GRAD_TOL x max |float64| per tensor.  Measured worst case on the emulator
+# (3xTF32 tensor-core layers, FFMA elsewhere) over every shape of tests/test_emu_row_coverage.py: 3.2e-6; on an H100 SXM (132 SMs, default
+# power limit) over tests/test_gpu_row_coverage.py: 4.9e-6 (R-MADDPG 4.6e-6).
+GRAD_TOL = 2e-5
+# Tensors whose gradient is a fixed linear image of ONE sum over the episode's rows of dL/d(output) -- the QMIX mixer's hyper_b2 output
+# bias (sum over the T transitions of dL/dQ_tot), the R-MADDPG critic's output biases and output-LayerNorm bias (sum over the T rows of
+# dL/dQ) -- lose relative precision when those terms cancel: the fp32 sum keeps an absolute error of order eps sum |term| while the
+# result shrinks (measured 3.8e-5 of |sum| on the QMIX bias at S 481, B 1, T 5, and 3.9e-5 on the R-MADDPG critic's at B 1, T 10).  Their
+# bound is GRAD_TOL x max|ref| x sum |term| / |sum term|, the cancellation ratio taken from the float64 TD errors; it equals GRAD_TOL
+# wherever the terms share a sign.
+SUM_OF_OUTPUT_GRADS = ("mixer.hyper_b2.2.bias", "critic.q_outs.0.bias", "critic.q_outs.1.bias", "critic.rnn.rnn.norm.bias")
+
+
+def _cancellation(terms):
+    """sum |t| / |sum t| over a float64 tensor of per-row output gradients (1 where nothing cancels)."""
+    t = terms.double().flatten()
+    s = float(t.sum().abs())
+    a = float(t.abs().sum())
+    return a / s if s > 0.0 else (1.0 if a == 0.0 else float("inf"))
+
+
+# Per-row forward: |engine - float64| <= ROW_TOL x max_j |float64[row, j]| + ROW_ATOL for every row; the recurrent state h (and the gates /
+# Q values computed from it) carry the round-off of up to T + 1 cell steps.  Measured worst: 2.6e-6 on the emulator (T <= 24); 1.3e-5 on
+# an H100 SXM, q_tgt at T = 151 (the mixer's 16 sms + 1 edge), 5.4e-6 at T <= 64.
+ROW_TOL = 2e-5
+# M-QMIX: the engine's TD error of a transition within this many fp32 ulps of max(|Q_tot|, |y|) of the float64 one.
+TD_ULPS = 16
+ROW_ATOL = 1e-6
+
+
+# ---- the launchers' tile rules -------------------------------------------------------------------------------------------
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def _round_up(a, b):
+    return _cdiv(a, b) * b
+
+
+def _ld(k):                 # mx_tile.cuh mx_ld: padded leading dimension of a shared-memory tile
+    return _round_up(k, 8) + 4
+
+
+def _front_bwd_smem_floats(in_dim, TM, gru_ext):         # agent_bwd.cu front_bwd_smem
+    I64, ld64, ldg, ldi = _round_up(in_dim, 64), _ld(64), _ld(192), _ld(_round_up(in_dim, 64))
+    o = TM * ldg + (0 if gru_ext else TM * ld64) + TM * ld64 + (0 if gru_ext else TM * ld64) + 2 * TM * ld64 + 3 * TM * ldi
+    return o + 64 * ld64 + 2 * I64 + 4 * 64 + 3 * TM * 2 + 4 * 64
+
+
+class TileRules(object):
+    """Row tiling of one learner step on `sms` SMs (4 in the emulator, multi_processor_count on a GPU)."""
+
+    def __init__(self, sms):
+        self.sms = int(sms)
+
+    def front_bwd_rm(self, M, in_dim, gru_ext):
+        """front_bwd_pick_rm: 16 RM rows per tile, RM in 2..4, minimising waves x (1 + RM) over the heights that fit 227 KB."""
+        best, best_cost = 2, 1e30
+        for rm in (2, 3, 4):
+            if _front_bwd_smem_floats(in_dim, 16 * rm, gru_ext) * 4 + 16 > 227 * 1024:
+                continue
+            cost = _cdiv(_cdiv(M, 16 * rm), self.sms) * (1.0 + rm)
+            if cost < best_cost - 1e-9:
+                best, best_cost = rm, cost
+        return best
+
+    def bwd_tc_ctas_per_sm(self, in_dim):
+        """k_front_bwd_tc streams its weight operands through one buffer; two CTAs per SM when twice that fits."""
+        kp16 = _round_up(in_dim, 16)
+        total = 2 * 128 * 64 * 4 + 2 * max(kp16, 64) * 64 * 4
+        return 2 if 2 * (total + 2048) <= 227 * 1024 else 1
+
+    def agent_rows(self, M, in_dim):
+        """The backward's row tiling: (kernel, rows per tile, tiles, grid) of each row kernel, and the forward's 128-row tiles."""
+        sms = self.sms
+        out = {}
+        if in_dim > 64:            # k_front_bwd_tc (128-row tiles) + k_wgrad_tc (64-row chunks, one persistent CTA per SM)
+            nt = _cdiv(M, 128)
+            out["k_front_bwd_tc"] = (128, nt, min(self.bwd_tc_ctas_per_sm(in_dim) * sms, nt))
+            nc = _cdiv(M, 64)
+            out["k_wgrad_tc"] = (64, nc, min(sms, nc))
+            out["k_front_fwd_tc_wide"] = (128, nt, min(sms, nt))
+        else:                      # k_front_bwd + k_gru_wgrad: same tile height and grid
+            TM = 16 * self.front_bwd_rm(M, in_dim, True)
+            nt = _cdiv(M, TM)
+            out["k_front_bwd"] = out["k_gru_wgrad"] = (TM, nt, min(sms, nt))
+            nf = _cdiv(M, 128)
+            out["k_front_fwd_tc"] = (128, nf, min(max(sms // 2, 1), nf))
+        return out
+
+    def mixer_rows(self, E):
+        """k_mixer / k_mix_hyper_fwd / k_mix_hyper_bwd: 16 RM transitions per tile, RM = 2 above 16 sms transitions."""
+        TE = 32 if E > 16 * self.sms else 16
+        nt = _cdiv(E, TE)
+        return (TE, nt, min(self.sms, nt))
+
+    def head_rows(self, M):
+        """R-MADDPG's k_head_bwd: 32-row tiles, grid min(sms, tiles) (critic rows B T, actor rows B (T+1) N)."""
+        nt = _cdiv(M, 32)
+        return (32, nt, min(self.sms, nt))
+
+    def row_kernel(self, in_dim):
+        """The kernel whose tiles define the agent-net row edges of a path."""
+        return "k_wgrad_tc" if in_dim > 64 else "k_front_bwd"
+
+
+def _edges(rules, in_dim, N, T, B):
+    """Which row / transition edges the shape (B, T, N) hits."""
+    r = (T + 1) * N
+    M, E = B * r, B * T
+    kern = rules.row_kernel(in_dim)
+    rows = rules.agent_rows(M, in_dim)
+    TM, nt, grid = rows[kern]
+    hits = set()
+    if nt == 1:
+        hits.add("one tile")
+    if M % TM == 1:
+        hits.add("tail 1")
+    if M % TM == TM - 1:
+        hits.add("tail TM-1")
+    for k, name in ((rules.sms, "tiles = sms"), (rules.sms + 1, "tiles = sms+1"), (2 * rules.sms + 1, "tiles = 2 sms+1")):
+        if nt == k:
+            hits.add(name)
+    if "k_front_bwd_tc" in rows:
+        _, nt2, _ = rows["k_front_bwd_tc"]
+        if nt2 == rules.bwd_tc_ctas_per_sm(in_dim) * rules.sms + 1:
+            hits.add("front_bwd_tc tiles = CTAs+1")
+    firsts = [(b * r) // TM for b in range(B)]
+    lasts = [((b + 1) * r - 1) // TM for b in range(B)]
+    if any(f == l for f, l in zip(firsts, lasts)):
+        hits.add("episode inside one tile")
+    if any(l - f >= 2 for f, l in zip(firsts, lasts)):
+        hits.add("episode spans three tiles")
+    if E == 16 * rules.sms:
+        hits.add("E = 16 sms")
+    if E == 16 * rules.sms + 1:
+        hits.add("E = 16 sms+1")
+    return hits, dict(M=M, E=E, TM=TM, tiles=nt, grid=grid)
+
+
+AGENT_TARGETS = ["one tile", "tail 1", "tail TM-1", "tiles = sms", "tiles = sms+1", "tiles = 2 sms+1", "episode inside one tile",
+                 "episode spans three tiles"]
+MIXER_TARGETS = ["E = 16 sms", "E = 16 sms+1"]
+
+
+def pick_shapes(rules, in_dim, Ns=(2, 3), Ts=range(2, 17), Bs=range(1, 65), targets=None, max_rows=None):
+    """(B, T, N) per edge, the cheapest (fewest isolated rows B M) that hits it.  Some edges cannot occur on a path (the tile-height rule
+    minimises waves, so just above `sms` tiles it may take a taller tile): then the nearest tile count that occurs is taken, and the
+    returned note says so.  Returns [(targets hit, (B, T, N), layout, note)], one entry per distinct shape."""
+    targets = list(targets or AGENT_TARGETS + (["front_bwd_tc tiles = CTAs+1"] if in_dim > 64 else []))
+    best, notes = {}, {}
+    cands = []
+    for N, T, B in itertools.product(Ns, Ts, Bs):
+        hits, lay = _edges(rules, in_dim, N, T, B)
+        if max_rows and lay["M"] > max_rows:
+            continue
+        cands.append((B * lay["M"], (B, T, N), hits, lay))
+    cands.sort(key=lambda c: c[0])
+    for tgt in targets:
+        for cost, shape, hits, lay in cands:
+            if tgt in hits:
+                best[tgt] = shape
+                break
+        else:
+            want = {"tiles = sms": rules.sms, "tiles = sms+1": rules.sms + 1, "tiles = 2 sms+1": 2 * rules.sms + 1}.get(tgt)
+            if want is None:
+                raise AssertionError("no shape in the search space hits %r" % tgt)
+            # the nearest count at or above: some CTA still runs one more tile than the others
+            near = min((c for c in cands if c[3]["tiles"] >= want), key=lambda c: (c[3]["tiles"] - want, c[0]))
+            best[tgt] = near[1]
+            notes[tgt] = "%s cannot occur on this path (tile rule); nearest: %d tiles of %d rows" % (tgt, near[3]["tiles"], near[3]["TM"])
+    out = {}
+    for tgt, shape in best.items():
+        out.setdefault(shape, []).append(tgt)
+    res = []
+    for shape, tg in sorted(out.items()):
+        B, T, N = shape
+        res.append((tg, shape, _edges(rules, in_dim, N, T, B)[1], "; ".join(notes[t] for t in tg if t in notes)))
+    return res
+
+
+def pick_mixer_shapes(rules, Ns=(2, 3), Ts=range(1, 40), Bs=range(1, 80)):
+    """(B, T, N) with E = B T = 16 sms and 16 sms + 1 transitions (the mixer's tile height switch), fewest rows."""
+    res = []
+    for tgt, E0 in (("E = 16 sms", 16 * rules.sms), ("E = 16 sms+1", 16 * rules.sms + 1)):
+        for E in range(E0, E0 + 64):      # E0 may be prime beyond the search space: the next count that occurs, still on the same side
+            c = [(B * (T + 1) * N * B, (B, T, N)) for N, T, B in itertools.product(Ns, Ts, Bs) if B * T == E]
+            if c:
+                break
+        assert c, "no shape with %d transitions in the search space" % E0
+        B, T, N = min(c)[1]
+        note = "" if E == E0 else "%s: %d has no factor pair in the search space; %d transitions instead" % (tgt, E0, E)
+        res.append(([tgt], (B, T, N), dict(E=E, tiles=rules.mixer_rows(E)), note))
+    return res
+
+
+MADDPG_TARGETS = ["critic one tile", "critic tail 1", "critic tail 31", "critic tiles = sms+1", "actor tail 1", "actor tail 31"]
+
+
+def pick_maddpg_shapes(rules, N=3, Ts=range(8, 40), Bs=range(1, 200)):
+    """R-MADDPG (B, T) with T >= 8 (the critic's k_gru_bwd2 stores T1 = T steps per sequence) on the edges of k_head_bwd's 32-row tiles:
+    critic rows Mc = B T and actor rows Ma = B (T+1) N.  Returns [(targets, (B, T, N), layout, note)], fewest rows first."""
+    def hits(B, T):
+        Mc, Ma = B * T, B * (T + 1) * N
+        h = set()
+        _, ntc, _ = rules.head_rows(Mc)
+        if ntc == 1:
+            h.add("critic one tile")
+        if Mc % 32 == 1:
+            h.add("critic tail 1")
+        if Mc % 32 == 31:
+            h.add("critic tail 31")
+        if ntc == rules.sms + 1:
+            h.add("critic tiles = sms+1")
+        if Ma % 32 == 1:
+            h.add("actor tail 1")
+        if Ma % 32 == 31:
+            h.add("actor tail 31")
+        return h
+    cands = sorted(((B * B * (T + 1) * N, (B, T)) for T in Ts for B in Bs))
+    out = {}
+    for tgt in MADDPG_TARGETS:
+        for _, (B, T) in cands:
+            if tgt in hits(B, T):
+                out.setdefault((B, T, N), []).append(tgt)
+                break
+        else:
+            raise AssertionError("no R-MADDPG shape in the search space hits %r" % tgt)
+    return [(tg, shape, dict(Mc=shape[0] * shape[1], Ma=shape[0] * (shape[1] + 1) * N), "") for shape, tg in sorted(out.items())]
+
+
+def sample_episodes(B, T, N, TM, grid, every_up_to=16):
+    """Every episode up to `every_up_to`; above, the first, the last and the ones that hold a row where a CTA's next tile starts
+    (the tile boundaries k grid TM) or the last tile starts."""
+    if B <= every_up_to:
+        return list(range(B))
+    r = (T + 1) * N
+    M = B * r
+    rows = {0, M - 1, ((M - 1) // TM) * TM}
+    k = 1
+    while k * grid * TM < M:
+        rows.add(k * grid * TM)
+        rows.add(k * grid * TM - 1)
+        k += 1
+    return sorted({row // r for row in rows})
+
+
+# ---- learners --------------------------------------------------------------------------------------------------------------
+def float64_twin(L):
+    """The float64 learner holding L's state: same networks, same targets, Adam state fresh (as L's before its first step)."""
+    from oracle.qmix import QmixLearner
+    from oracle.mqmix import MqmixLearner
+    cls = MqmixLearner if isinstance(L, MqmixLearner) else QmixLearner
+    L64 = cls(L.cfg, dtype=torch.float64)
+    for dst, src in ((L64.agent, L.agent), (L64.mixer, L.mixer), (L64.tgt_agent, L.tgt_agent), (L64.tgt_mixer, L.tgt_mixer)):
+        dst.load_state_dict(src.state_dict())
+    return L64
+
+
+def qmix_pair(cfg, B, T, debug=True):
+    """(float64 oracle, policy, trainer) with the randomised state of qmix_checks.oracle_and_trainer; trainer max_batch = B."""
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=debug)
+    tr.use_step_graph = False
+    return float64_twin(L), pol, tr
+
+
+def mqmix_pair(cfg, B, debug=False):
+    from oracle.mqmix import MqmixLearner
+    from oracle.qmix import randomize_all
+    import mqmix_checks as mc
+    L = MqmixLearner(cfg, seed=3)
+    randomize_all(L.agent, 1)
+    randomize_all(L.mixer, 2)
+    L.sync_targets()
+    randomize_all(L.tgt_agent, 3, 0.05)
+    randomize_all(L.tgt_mixer, 4, 0.05)
+    args, pol, tr = mc.build(cfg, B, debug)
+    pol.q_network.load_state_dict(L.agent.state_dict())
+    tr.target_q_network.load_state_dict(L.tgt_agent.state_dict())
+    tr.mixer.load_state_dict(L.mixer.state_dict())
+    tr.target_mixer.load_state_dict(L.tgt_mixer.state_dict())
+    return float64_twin(L), pol, tr
+
+
+def last_episode_full_length(batch):
+    """synth_batch(var_len=True) ends every episode at a length in [T/2, T]; make the LAST one run all T steps, so the tail of the row
+    space (all but the final N step-(T+1) rows) and of the transition space carries gradient in its isolated run."""
+    obs, share, acts, rew, dones, dones_env = batch[:6]
+    dones_env = dones_env.copy()
+    dones_env[:, -1, 0] = 0.0
+    dones_env[-1, -1, 0] = 1.0
+    dones = np.repeat(dones_env[None], dones.shape[0], axis=0)
+    return (obs, share, acts, rew, dones, dones_env) + tuple(batch[6:])
+
+
+def maddpg_pair(cfg, B, T):
+    """(float64 oracle, policy, trainer) of R-MADDPG / R-MATD3 with every tensor randomised, trainer max_batch = B."""
+    import maddpg_checks as mc
+    from oracle.maddpg import MaddpgLearner
+    from oracle.qmix import randomize_all
+    L = MaddpgLearner(cfg, seed=5)
+    randomize_all(L.actor, 1)
+    randomize_all(L.critic, 2)
+    L.sync_targets()
+    randomize_all(L.tgt_actor, 3, 0.05)
+    randomize_all(L.tgt_critic, 4, 0.05)
+    args, pol, tr = mc.build(cfg, B, T)
+    L64 = MaddpgLearner(cfg, dtype=torch.float64)
+    for ours, ref, ref64 in ((pol.actor, L.actor, L64.actor), (pol.critic, L.critic, L64.critic), (pol.target_actor, L.tgt_actor, L64.tgt_actor),
+                             (pol.target_critic, L.tgt_critic, L64.tgt_critic)):
+        ours.load_state_dict(ref.state_dict())
+        ref64.load_state_dict(ref.state_dict())
+    return L64, pol, tr
+
+
+def maddpg_isolated_episodes(L64, pol, tr, batch, episodes, B, T, tol=None):
+    """R-MADDPG with one episode isolated per run, from the same state each time.  Critic: PER weights one-hot on episode b, so the
+    critic gradient is exactly episode b's T rows.  Actor: every agent of every other episode is done from its first step, so the actor
+    loss keeps episode b's (T N) rows plus only the first step of the others (the per-agent mask lags the done flag by one step, the first
+    step is always live).  Both clipped gradients against the float64 update.  Returns the worst relative error per tensor."""
+    import copy
+    import maddpg_checks as mc
+    from oracle.maddpg import sample_gumbel
+    tol = GRAD_TOL if tol is None else tol
+    cfg, N = L64.cfg, L64.cfg.n_agents
+    ws0 = tr.workspace.clone()
+    vec0 = [v.clone() for v in pol.actor_vecs + pol.critic_vecs]
+    L0 = copy.deepcopy(L64)
+    worst = {}
+    for b in episodes:
+        tr.workspace.copy_(ws0)
+        for v, v0 in zip(pol.actor_vecs + pol.critic_vecs, vec0):
+            v.copy_(v0)
+        tr.num_updates["policy_0"] = 0
+        L = copy.deepcopy(L0)
+        w = np.zeros(B, np.float32)
+        w[b] = 1.0
+        dones = batch[4].copy()
+        dones[:, :, [x for x in range(B) if x != b], :] = 1.0
+        bt = tuple(batch[:4]) + (dones,) + tuple(batch[5:7]) + (w, np.arange(B))
+        torch.manual_seed(77 + b)
+        anoise = sample_gumbel((T, N * B, cfg.act_dim)).numpy() if cfg.discrete else None
+        torch.manual_seed(77 + b)                    # the trainer draws the actor's Gumbel noise from torch's CPU generator
+        info, _, _ = tr.shared_train_policy_on_batch("policy_0", mc.ref_tuple(bt))
+        ga, gc = tr.grad_views()
+        ref, _ = L.step(bt, None, anoise)
+        assert bool(info["update_actor"]) and bool(ref["update_actor"])
+        errs = {}
+        for tag, flat, P, entries, grads, gn in (("critic", gc, pol.Pc, pol._c_entries, L.critic_grads, ref["critic_grad_norm"]),
+                                                  ("actor", ga, pol.Pa, pol._a_entries, L.actor_grads, ref["actor_grad_norm"])):
+            coef = min(1.0, cfg.max_grad_norm / (float(gn) + 1e-6))
+            views = mc.named_views(flat.detach().cpu().double(), entries)
+            den = float(flat[P])
+            for k, gr in grads.items():
+                ref_k = gr.detach().double()
+                name = tag + "." + k
+                c = 1.0
+                if name in SUM_OF_OUTPUT_GRADS:      # critic output head(s): sums over the episode's T rows of the TD errors (one per head)
+                    c = max(_cancellation(e[:, b]) for e in L.critic_errs)
+                errs[name] = float((views[k] / den * coef - ref_k).abs().max() / (ref_k.abs().max() + 1e-30)) / c
+        bad = {k: e for k, e in errs.items() if e > tol}
+        assert not bad, ("episode %d of %d isolated: gradients off the float64 oracle (bound %.1e x max|ref|)" % (b, B, tol),
+                         sorted(bad.items(), key=lambda kv: -kv[1])[:6])
+        for k, e in errs.items():
+            worst[k] = max(worst.get(k, 0.0), e)
+    tr.workspace.copy_(ws0)
+    for v, v0 in zip(pol.actor_vecs + pol.critic_vecs, vec0):
+        v.copy_(v0)
+    return worst
+
+
+def kernels_run(lib, stream, fn):
+    """Names of the kernels `fn()` launched (mx_profile_begin / mx_profile_end)."""
+    lib.mx_profile_begin(stream)
+    try:
+        fn()
+    finally:
+        buf = C.create_string_buffer(65536)
+        ms = (C.c_float * 2048)()
+        n = lib.mx_profile_end(stream, buf, 65536, ms, 2048)
+    return buf.value.decode().split(";")[:n]
+
+
+# Kernels a test means to pin, and what the launcher runs instead where that kernel does not apply: above the overlap row limit the
+# GPU step runs serially with the fused k_mixer, and k_mid takes only the widths whose per-warp operands fit its shared memory
+# (mid.cu mid_pick_warps / mx_mid_supported) -- otherwise k_qhead + the mixer + k_qhead_bwd run separately.
+KERNEL_ALTERNATIVES = {"k_mix_core": ["k_mixer"], "k_mid": ["k_qhead", "k_qhead_bwd"]}
+
+
+def assert_kernels_ran(names, kernels):
+    for k in kernels:
+        alt = KERNEL_ALTERNATIVES.get(k)
+        assert k in names or (alt and all(a in names for a in alt)), (k, "did not run", names)
+
+
+# ---- the checks ---------------------------------------------------------------------------------------------------------------
+def _grad_errors(gv, L64, ref_scale=1.0, cancel=1.0):
+    """{tensor: max |engine - float64 x ref_scale| / max |float64 x ref_scale|} over the learner's parameters (unused ones must be exactly
+    zero); for SUM_OF_OUTPUT_GRADS the error is further divided by the cancellation ratio `cancel`."""
+    named = dict(("agent." + k, p) for k, p in L64.agent.named_parameters())
+    if not L64.cfg.vdn:
+        named.update(("mixer." + k, p) for k, p in L64.mixer.named_parameters())
+    out = {}
+    for k, p in named.items():
+        ours = gv[k].detach().cpu().double()
+        if p.grad is None:
+            assert float(ours.abs().max()) == 0.0, (k, "unused parameter has a gradient")
+            continue
+        ref = p.grad.detach().double() * ref_scale
+        out[k] = float((ours - ref).abs().max() / (ref.abs().max() + 1e-30)) / (cancel if k in SUM_OF_OUTPUT_GRADS else 1.0)
+    return out
+
+
+def isolated_episode_gradients(L64, tr, batch, episodes, B, T, N, mlp=False, tol=GRAD_TOL):
+    """For each b in `episodes`: one engine step with importance weights e_b from the same state, its unclipped gradient against the
+    float64 oracle's.  ReLU units within round-off of zero may pick the other side (tests/kink.py): a failing comparison is re-run with the
+    engine's ReLU masks forced and must then pass.  Returns the worst relative error per tensor."""
+    sd0 = tr.state_dict()
+    worst = {}
+    for b in episodes:
+        w = np.zeros(B, np.float32)
+        w[b] = 1.0
+        bt = tuple(batch[:-2]) + (w, np.arange(B))
+        tr.load_state_dict(sd0)
+        if mlp:
+            import mqmix_checks as mc
+            tr.train_policy_on_batch(mc._to_dicts(tuple(batch[:-2]), w), True)
+        else:
+            tr.train_policy_on_batch(qc.ref_tuple(bt))
+        gv = {k: v.detach().cpu().clone() for k, v in tr.grad_views().items()}
+        _, _, aux = L64.grads(bt)
+        scale, cancel = 1.0, 1.0
+        if mlp:
+            # one transition: its whole gradient is its TD error times d Q_tot / d theta.  Where Q_tot and the target nearly cancel, the
+            # fp32 TD error carries an error of a few ulps of max(|Q_tot|, |y|) -- relative to the error itself, eps |Q| / |err|, into EVERY
+            # tensor alike (measured 7.2e-5 on an H100 for one of 2 112 transitions).  The engine's TD error must be within TD_ULPS ulps of
+            # that magnitude; the row coverage is then judged against the float64 gradient taken at the engine's TD error
+            e_ref = float(aux["err"].detach()[b])
+            e_eng = float(tr.ws_view("err")[b])
+            mag = max(abs(float(aux["q_tot"].detach().flatten()[b])), abs(float(aux["target"].detach().flatten()[b])))
+            assert abs(e_eng - e_ref) <= TD_ULPS * 2.0 ** -23 * mag, ("transition %d: TD error %r vs float64 %r (|Q| %.3e)" % (b, e_eng, e_ref, mag))
+            scale = e_eng / e_ref if e_ref != 0.0 else 1.0
+        else:
+            cancel = _cancellation(aux["err"].detach()[:, b])
+        errs = _grad_errors(gv, L64, scale, cancel)
+        bad = {k: e for k, e in errs.items() if e > tol}
+        if bad and getattr(L64.cfg, "relu", True):
+            masks = [m.double() for m in kink.engine_masks(tr, B, T, N, mlp=mlp)]
+            _, flips, max_pre = kink.redo_with_engine_masks(L64, lambda LL: LL.grads(bt), masks)
+            assert flips > 0 and max_pre < kink.KINK_TOL, ("episode %d: gradient mismatch not explained by ReLU kinks" % b, flips, max_pre,
+                                                           sorted(bad.items(), key=lambda kv: -kv[1])[:4])
+            errs = _grad_errors(gv, L64, scale, cancel)
+            bad = {k: e for k, e in errs.items() if e > tol}
+        assert not bad, ("episode %d of %d isolated: gradients off the float64 oracle (bound %.1e x max|ref|)" % (b, B, tol),
+                         sorted(bad.items(), key=lambda kv: -kv[1])[:6])
+        for k, e in errs.items():
+            worst[k] = max(worst.get(k, 0.0), e)
+    tr.load_state_dict(sd0)
+    return worst
+
+
+def _rows_close(name, ours, want, rtol, atol, bad, worst):
+    ours = torch.as_tensor(ours).detach().cpu().double()
+    want = torch.as_tensor(want).detach().cpu().double()
+    assert ours.shape == want.shape, (name, ours.shape, want.shape)
+    err = (ours - want).abs().amax(dim=1)
+    scale = want.abs().amax(dim=1)
+    ratio = err / (rtol * scale + atol)
+    worst[name] = max(worst.get(name, 0.0), float((err / (scale + atol / rtol)).max()))
+    if float(ratio.max()) > 1.0:
+        r = int(ratio.argmax())
+        bad.append("%s: row %d of %d off by %.3e (row max %.3e, bound %.3e); %d row(s) out of bound"
+                   % (name, r, ours.shape[0], float(err[r]), float(scale[r]), rtol * float(scale[r]) + atol, int((ratio > 1.0).sum())))
+
+
+def agent_input(L64, batch):
+    """The agent net's input rows as the oracle builds them, (T+1, N B, in_dim) in float64."""
+    x = L64.stack_agents(batch[0])
+    if L64.cfg.prev_act_inp:
+        a = L64.stack_agents(batch[2])
+        x = torch.cat((x, torch.cat((torch.zeros(1, a.shape[1], a.shape[2], dtype=a.dtype), a), 0)), -1)
+    return x
+
+
+def per_row_forward(L64, tr, batch, B, T, N, debug, rtol=ROW_TOL, atol=ROW_ATOL):
+    """Every materialised activation of all M rows (masked ones included) of the live and the target net against the float64 trace
+    of the step the engine just ran; each row bounded relative to its own largest magnitude.  Returns {region: worst err / row max}."""
+    from oracle.qmix import agent_trace
+    M = B * (T + 1) * N
+    A = L64.cfg.act_dim
+    x = agent_input(L64, batch)
+    bad, worst = [], {}
+    rows = lambda v: qc.to_rows(v, N, B)
+    for tag, net in (("live", L64.agent), ("tgt", L64.tgt_agent)):
+        trc = agent_trace(net, x)
+        _rows_close("gi_" + tag, tr.ws_view("gi_" + tag)[:M * 192].view(M, 192), rows(trc["gi"]), rtol, atol, bad, worst)
+        _rows_close("h_" + tag, tr.ws_view("h_" + tag)[:M * 64].view(M, 64), rows(trc["h"]), rtol, atol, bad, worst)
+        if debug:
+            _rows_close("q_" + tag, tr.ws_view("q_" + tag)[:M * A].view(M, A), rows(trc["q"]), rtol, atol, bad, worst)
+        if tag == "live":
+            _rows_close("u1", tr.ws_view("u1")[:M * 64].view(M, 64), rows(trc["u1"]), rtol, atol, bad, worst)
+            _rows_close("u2", tr.ws_view("u2")[:M * 64].view(M, 64), rows(trc["u2"]), rtol, atol, bad, worst)
+            g = tr.ws_view("gates")[:M * 192].view(M, 192)
+            want = torch.cat([rows(trc["r"]), rows(trc["z"]), rows(trc["n"])], 1)
+            _rows_close("gates", g, want, rtol, atol, bad, worst)
+            _rows_close("hn", tr.ws_view("hn")[:M * 64].view(M, 64), rows(trc["hn"]), rtol, atol, bad, worst)
+    assert not bad, "\n".join(bad)
+    return worst
+
+
+def batch_size_sequence(L64, pol, tr, cfg, Bs, T, seed=30, tol=GRAD_TOL, param_tol=5e-3):
+    """Steps at the batch sizes `Bs` on ONE learner (max_batch = Bs[0]), each in lock-step with the float64 oracle: gradients, loss,
+    parameters after Adam, targets after the soft update."""
+    from oracle.qmix import synth_batch
+    worst = {}
+    for s, B in enumerate(Bs):
+        w = np.random.RandomState(seed + 100 + s).rand(B).astype(np.float32) * 0.9 + 0.1
+        batch = synth_batch(cfg, B, T, seed=seed + s, avail_p=0.8, var_len=True) + (w, np.arange(B))
+        info, prio, _ = tr.train_policy_on_batch(qc.ref_tuple(batch))
+        gv = {k: v.detach().cpu().clone() for k, v in tr.grad_views().items()}
+        L0 = kink.snapshot(L64) if getattr(cfg, "relu", True) else None
+        ref, rprio, _ = L64.step(batch)
+        # the oracle's step leaves the CLIPPED gradients in .grad; the engine's views are the unclipped ones
+        clip = lambda r: min(1.0, cfg.max_grad_norm / (float(r["grad_norm"]) + 1e-6))
+        errs = _grad_errors({k: v * clip(ref) for k, v in gv.items()}, L64)
+        bad = {k: e for k, e in errs.items() if e > tol}
+        if bad and L0 is not None:
+            masks = [m.double() for m in kink.engine_masks(tr, B, T, cfg.n_agents, mlp=False)]
+            (ref, rprio, _), flips, max_pre = kink.redo_with_engine_masks(L0, lambda LL: LL.step(batch), masks)
+            assert flips > 0 and max_pre < kink.KINK_TOL, (s, B, "gradient mismatch not explained by ReLU kinks", flips, max_pre, bad)
+            kink.adopt(L64, L0)
+            errs = _grad_errors({k: v * clip(ref) for k, v in gv.items()}, L64)
+            bad = {k: e for k, e in errs.items() if e > tol}
+        assert not bad, ("step %d at B = %d" % (s, B), sorted(bad.items(), key=lambda kv: -kv[1])[:6])
+        for k, e in errs.items():
+            worst[k] = max(worst.get(k, 0.0), e)
+        for k in ("loss", "grad_norm", "Q_tot"):
+            assert rel_err(info[k].cpu(), ref[k]) < tol, (s, B, k, float(info[k]), float(ref[k]))
+        assert rel_err(np.asarray(prio), rprio) < 1e-4, (s, B, "priorities")
+        tr.soft_target_updates()
+        L64.soft_update()
+        for mod, ref_mod in ((pol.q_network, L64.agent), (tr.mixer, L64.mixer)):
+            for k, v in mod.state_dict().items():
+                d = float((v.cpu().double() - ref_mod.state_dict()[k]).abs().max())
+                assert d <= param_tol * cfg.lr * (s + 1) + 1e-7, (s, B, k, d)
+        for mod, ref_mod in ((tr.target_q_network, L64.tgt_agent), (tr.target_mixer, L64.tgt_mixer)):
+            for k, v in mod.state_dict().items():
+                assert float((v.cpu().double() - ref_mod.state_dict()[k]).abs().max()) <= 1e-6, (s, B, k)
+    return worst
