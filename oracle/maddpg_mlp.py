@@ -27,7 +27,7 @@ def onehot_from_logits(logits, avail=None):
     logits = logits.clone()
     if avail is not None:
         logits[avail == 0] = -1e10
-    return (logits == logits.max(-1, keepdim=True)[0]).float()
+    return (logits == logits.max(-1, keepdim=True)[0]).to(logits.dtype)
 
 
 def gumbel_hard(logits, g, avail=None):
@@ -42,9 +42,11 @@ def gumbel_hard(logits, g, avail=None):
 class MlpMaddpg(object):
     def __init__(self, actor, critic, heads, target_actor, target_critic, target_heads, discrete, td3, gamma=0.99, lr=7e-4, eps=1e-5,
                  weight_decay=0.0, max_grad_norm=10.0, tau=0.005, huber=False, huber_delta=10.0, use_per=False, per_eps=1e-6, relu=True,
-                 feature_norm=True):
-        """actor / critic / target_*: {reference key: tensor}; heads / target_heads: {"q_outs.k.weight" / ".bias": tensor}."""
-        t = lambda d, g: {k: torch.as_tensor(v, dtype=torch.float32).detach().clone().requires_grad_(g) for k, v in d.items()}
+                 feature_norm=True, dtype=torch.float32):
+        """actor / critic / target_*: {reference key: tensor}; heads / target_heads: {"q_outs.k.weight" / ".bias": tensor}.  dtype: of
+        every tensor of the update (float64 for the row-coverage checks: batch, nets, heads, Adam, clip and Polyak all in float64)."""
+        self.dtype = dtype
+        t = lambda d, g: {k: torch.as_tensor(v).to(dtype).detach().clone().requires_grad_(g) for k, v in d.items()}
         self.actor, self.critic = t(actor, True), t(critic, True)
         self.target_actor, self.target_critic = t(target_actor, False), t(target_critic, False)
         self.heads, self.target_heads = t(heads, False), t(target_heads, False)
@@ -67,8 +69,9 @@ class MlpMaddpg(object):
         """One shared_train_policy_on_batch of policy_0.  batch: the 13-tuple of mlp_buffer.py (policy_0 entries); target_noise /
         actor_noise: the (N*B, A) draws the reference makes in get_update_info (MATD3) and in the actor update (Discrete)."""
         obs, share, acts, rew, nobs, nshare, _dones, dones_env, valid, avail, navail, weights, _idx = batch
-        f = lambda x: None if x is None else torch.as_tensor(np.asarray(x), dtype=torch.float32)
+        f = lambda x: None if x is None else torch.as_tensor(np.asarray(x)).to(self.dtype)
         p = "policy_0"
+        target_noise, actor_noise = f(target_noise), f(actor_noise)
         obs, nobs, acts = f(obs[p]), f(nobs[p]), f(acts[p])                 # (N, B, .)
         N, B = obs.shape[0], obs.shape[1]
         av = f(avail[p]) if avail is not None and avail[p] is not None else None

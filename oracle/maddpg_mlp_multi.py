@@ -14,47 +14,49 @@ import torch
 from oracle.maddpg_mlp import gumbel_hard, onehot_from_logits
 
 
-def _f(x):
-    return None if x is None else torch.as_tensor(np.asarray(x), dtype=torch.float32)
+def _f(x, dtype=torch.float32):
+    return None if x is None else torch.as_tensor(np.asarray(x)).to(dtype)
 
 
-def step_multi(learners, update_id, batch, target_noise, actor_noise=None):
-    """One shared_train_policy_on_batch(update_id, batch).  learners: {policy_id: MlpMaddpg}; batch: the 13-tuple of mlp_buffer.py with
-    an entry per policy; target_noise: {policy_id: (N_q*B, A_q) draw or None}; actor_noise: p's (N_p*B, A_p) Gumbel draw or None.
-    Returns (train_info, priorities or None, clipped gradients)."""
+def step_multi(learners, update_id, batch, target_noise, actor_noise=None, dtype=torch.float32):
+    """One shared_train_policy_on_batch(update_id, batch).  learners: {policy_id: MlpMaddpg}, all built with `dtype`; batch: the 13-tuple
+    of mlp_buffer.py with an entry per policy; target_noise: {policy_id: (N_q*B, A_q) draw or None}; actor_noise: p's (N_p*B, A_p) Gumbel
+    draw or None.  Returns (train_info, priorities or None, clipped gradients)."""
     obs, share, acts, rew, nobs, nshare, _dones, dones_env, valid, avail, navail, weights, _idx = batch
+    f = lambda x: _f(x, dtype)
+    actor_noise = f(actor_noise)
     ids = sorted(learners)
     p = update_id
     L = learners[p]
-    opt = lambda d, q: None if d is None or d.get(q) is None else _f(d[q])
+    opt = lambda d, q: None if d is None or d.get(q) is None else f(d[q])
     cent_act, cent_nact, start, ind = [], [], None, 0
     with torch.no_grad():
         for q in ids:                                                         # maddpg.py:56-76
             Lq = learners[q]
-            nob = _f(nobs[q])
+            nob = f(nobs[q])
             Nq, B = nob.shape[0], nob.shape[1]
             if q == p:
                 start = ind
-            cent_act.extend(list(_f(acts[q])))
+            cent_act.extend(list(f(acts[q])))
             nav = opt(navail, q)
             out = Lq.actor_out(Lq.target_actor, nob.reshape(Nq * B, -1))
             nav = None if nav is None else nav.reshape(Nq * B, -1)
             if Lq.discrete:
-                nact = gumbel_hard(out, target_noise[q], nav) if Lq.td3 else onehot_from_logits(out, nav)
+                nact = gumbel_hard(out, f(target_noise[q]), nav) if Lq.td3 else onehot_from_logits(out, nav)
             else:
-                nact = out + target_noise[q] if Lq.td3 else out
+                nact = out + f(target_noise[q]) if Lq.td3 else out
             cent_nact.append(torch.cat(nact.split(B, 0), -1))
             ind += Nq
         cent_nact = torch.cat(cent_nact, -1)
-        qn = torch.cat(L.q(L.target_critic, L.target_heads, torch.cat([_f(nshare[p]), cent_nact], 1)), -1).min(-1, keepdim=True)[0]
-        y = _f(rew[p])[0].view(-1, 1) + L.gamma * (1 - _f(dones_env[p]).view(-1, 1)) * qn           # maddpg.py:113-126
+        qn = torch.cat(L.q(L.target_critic, L.target_heads, torch.cat([f(nshare[p]), cent_nact], 1)), -1).min(-1, keepdim=True)[0]
+        y = f(rew[p])[0].view(-1, 1) + L.gamma * (1 - f(dones_env[p]).view(-1, 1)) * qn           # maddpg.py:113-126
     info = {}
-    qs = L.q(L.critic, L.heads, torch.cat([_f(share[p]), torch.cat(cent_act, -1)], 1))
+    qs = L.q(L.critic, L.heads, torch.cat([f(share[p]), torch.cat(cent_act, -1)], 1))
     errors = [y - q for q in qs]
     loss_fn = (lambda e: torch.where(e.abs() <= L.huber_delta, 0.5 * e ** 2, L.huber_delta * (e.abs() - 0.5 * L.huber_delta))) \
         if L.huber else (lambda e: e ** 2)
     if L.use_per:                                                             # maddpg.py:134-144
-        w = _f(weights)
+        w = f(weights)
         critic_loss = torch.stack([(loss_fn(e).flatten() * w).mean() for e in errors]).sum(0)
         prio = np.stack([e.abs().detach().numpy().flatten() for e in errors]).mean(axis=0) + L.per_eps
     else:
@@ -68,7 +70,7 @@ def step_multi(learners, update_id, batch, target_noise, actor_noise=None):
     grads = {"critic": g(L.critic)}
     L.critic_opt.step()
     # actor update, every call (maddpg.py:100, 162-247)
-    ob = _f(obs[p])
+    ob = f(obs[p])
     Np, B = ob.shape[0], ob.shape[1]
     out = L.actor_out(L.actor, ob.reshape(Np * B, -1))
     av = opt(avail, p)
@@ -78,8 +80,8 @@ def step_multi(learners, update_id, batch, target_noise, actor_noise=None):
     for i in range(Np):                                                       # maddpg.py:183-227: agent replace_ind_start + i replaced
         rows.append(torch.cat([pol[i] if j == start + i else cent_act[j] for j in range(len(cent_act))], -1))
     frozen = {k: v.detach() for k, v in L.critic.items()}
-    qa = L.q(frozen, L.heads, torch.cat([_f(share[p]).repeat(Np, 1), torch.cat(rows, 0)], 1))[0]
-    vmask = _f(valid[p]).reshape(Np * B, 1)
+    qa = L.q(frozen, L.heads, torch.cat([f(share[p]).repeat(Np, 1), torch.cat(rows, 0)], 1))[0]
+    vmask = f(valid[p]).reshape(Np * B, 1)
     actor_loss = -(qa * vmask).sum() / vmask.sum()
     L.actor_opt.zero_grad()
     actor_loss.backward()

@@ -4,6 +4,7 @@ import numpy as np
 import torch
 
 from helpers import load_golden, rel_err
+from maddpg_checks import named_views
 
 from oracle.maddpg_mlp import MlpMaddpg
 
@@ -43,22 +44,79 @@ def oracle_from(args, pol):
                      feature_norm=bool(args.use_feature_normalization))
 
 
+def actor_tail(pol):
+    """First float of the actor vector past its trained range: the learner's net layout (qmix.cu mx_net_layout) puts the head in the
+    weight_ih slot (bias at bias_ih), then bias_hh, then the output LayerNorm, which optimise() takes as the end of the actor's range."""
+    bih = min(off for name, off, _, _ in pol._a_entries if name.startswith("act.") and name.endswith(".bias"))
+    return bih + 2 * 3 * 64
+
+
+def engine_grads(tr, pol, p_id=None):
+    """The engine's unclipped gradients of its last step, {"critic": {key: tensor}, "actor": {key: tensor}} in float64: numerator over
+    denominator.  The critic's range stops at its weight_ih slot (the frozen heads sit there), so its four scalars are at the first head's
+    offset; the actor's are at Pa, and every float of its vector past the trained range carries an exactly zero gradient."""
+    ga, gc = (v.detach().cpu().double() for v in tr.grad_views(p_id))
+    c_den = float(gc[pol._h_entries[0][1]])
+    a_den = float(ga[pol.Pa])
+    tail = ga[actor_tail(pol):pol.Pa]
+    assert int((tail != 0).sum()) == 0, ("actor gradient past its trained range", int((tail != 0).sum()))
+    return {"critic": {k: v / c_den for k, v in named_views(gc, pol._c_entries).items()},
+            "actor": {k: v / a_den for k, v in named_views(ga, pol._a_entries).items()}}
+
+
+def clipped_engine_grads(tr, pol, ref_info, max_grad_norm, p_id=None):
+    """engine_grads scaled by torch.nn.utils.clip_grad_norm_'s factor at the reference's grad norms: comparable with the oracle's
+    (clipped) gradients and the fixtures'."""
+    coef = lambda k: min(1.0, max_grad_norm / (float(ref_info[k]) + 1e-6))
+    g = engine_grads(tr, pol, p_id)
+    return {net: {k: v * coef(net + "_grad_norm") for k, v in d.items()} for net, d in g.items()}
+
+
+def actor_tail_params(pol):
+    """The actor's floats past its trained range (live, target, Adam m, v): no update may touch them."""
+    t = actor_tail(pol)
+    return [v[t:].clone() for v in pol.actor_vecs]
+
+
+def assert_actor_tail_unchanged(pol, before):
+    for i, (v, v0) in enumerate(zip(pol.actor_vecs, before)):
+        assert torch.equal(v[actor_tail(pol):], v0), ("actor vector %d changed past the trained range" % i)
+
+
+def grad_errors(ours, ref, rtol=1e-4, tag=""):
+    """{net.key: max |ours - ref| / max |ref|} over every tensor of `ref` ({net: {key: tensor}}); raises listing every tensor beyond
+    rtol x max|ref| (a tensor whose reference is zero must be exactly zero)."""
+    errs, bad = {}, []
+    for net, d in ref.items():
+        for k, r in d.items():
+            r = torch.as_tensor(r).double().reshape(ours[net][k].shape)
+            diff, scale = float((ours[net][k] - r).abs().max()), float(r.abs().max())
+            errs[net + "." + k] = diff / scale if scale > 0 else (0.0 if diff == 0.0 else float("inf"))
+            if diff > rtol * scale:
+                bad.append("%s %s.%s: err %.3e > %.1e x max|ref| %.3e" % (tag, net, k, diff, rtol, scale))
+    assert not bad, "\n".join(bad)
+    return errs
+
+
 def lockstep(args, pol, tr, batches, rtol=1e-4, ptol=2e-5, soft=True):
     """Engine and oracle step through `batches` (soft target update after each); returns the max deviations seen."""
     L = oracle_from(args, pol)
     heads0 = {k: v.clone() for k, v in pol.critic_heads.state_dict().items()}
     theads0 = {k: v.clone() for k, v in pol.target_critic_heads.state_dict().items()}
-    worst = {"info": 0.0, "param": 0.0, "prio": 0.0}
-    for batch in batches:
+    worst = {"info": 0.0, "param": 0.0, "prio": 0.0, "grad": 0.0}
+    for s, batch in enumerate(batches):
         B = np.asarray(batch[0]["policy_0"]).shape[1]
+        tail0 = actor_tail_params(pol)
         rng_before = torch.get_rng_state()
         info, prio, _ = tr.shared_train_policy_on_batch("policy_0", batch)
         rng_after = torch.get_rng_state()
         torch.set_rng_state(rng_before)
         tn, an = tr.draw_target_noise(B), tr.draw_actor_noise(B)          # the same calls, the same draws
         assert torch.equal(torch.get_rng_state(), rng_after)
-        ref, rprio, _ = L.step(batch, tn, an)
+        ref, rprio, grads = L.step(batch, tn, an)
         assert info["update_actor"] is True
+        errs = grad_errors(clipped_engine_grads(tr, pol, ref, args.max_grad_norm), grads, rtol, "step %d" % s)
+        worst["grad"] = max([worst["grad"]] + list(errs.values()))
         for k, v in ref.items():
             d = abs(float(info[k]) - v) / max(1.0, abs(v))
             worst["info"] = max(worst["info"], d)
@@ -78,6 +136,7 @@ def lockstep(args, pol, tr, batches, rtol=1e-4, ptol=2e-5, soft=True):
                 d = float((v.cpu() - ref_sd[k].detach()).abs().max())
                 worst["param"] = max(worst["param"], d)
                 assert d <= ptol, (k, d)
+        assert_actor_tail_unchanged(pol, tail0)
     # the heads are not parameters: byte-identical after every update and target update
     for k, v in pol.critic_heads.state_dict().items():
         assert torch.equal(v, heads0[k]), k
@@ -132,10 +191,18 @@ def engine_against_golden(name, ptol_lr=5e-3):
             assert np.array_equal(v.cpu().numpy(), g["init.%s.%s" % (tag, k)].reshape(v.shape)), (tag, k)
     for s in range(steps):
         torch.set_rng_state(torch.from_numpy(g["s%d.rng_before" % s]))
+        tail0 = actor_tail_params(pol)
         info, prio, _ = tr.shared_train_policy_on_batch("policy_0", golden_batch(g, s))
         assert np.array_equal(torch.get_rng_state().numpy(), g["s%d.rng_after" % s])
         for k in ("critic_loss", "critic_grad_norm", "actor_loss", "actor_grad_norm"):
             assert rel_err(float(info[k]), g["s%d.%s" % (s, k)]) < 1e-4, (s, k)
+        assert_actor_tail_unchanged(pol, tail0)
+        # every clipped gradient tensor the fixture records, 1e-4 x max|ref| each
+        ref = {net: {k: g["s%d.grad.%s.%s" % (s, net, k)] for k in ours if "s%d.grad.%s.%s" % (s, net, k) in g}
+               for net, ours in engine_grads(tr, pol).items()}
+        assert ref["critic"] and ref["actor"], s
+        grad_errors(clipped_engine_grads(tr, pol, {k: g["s%d.%s" % (s, k)] for k in ("critic_grad_norm", "actor_grad_norm")},
+                                         args.max_grad_norm), ref, 1e-4, "step %d" % s)
         if prio is not None:
             assert rel_err(np.asarray(prio), g["s%d.prio" % s]) < 1e-4
         for tag, mod in (("actor", pol.actor), ("critic", pol.critic)):

@@ -8,6 +8,7 @@ import numpy as np
 import torch
 
 from helpers import load_golden, rel_err
+from mlp_maddpg_checks import assert_actor_tail_unchanged, actor_tail_params, clipped_engine_grads, engine_grads, grad_errors
 from mlp_maddpg_multi_checks import FIELDS, golden_batch_multi, golden_draws, golden_expected, golden_rng_before, golden_sd
 
 from oracle.maddpg_mlp_md import MlpMaddpgMD, draw_noise_multi_md, step_multi_md
@@ -83,18 +84,22 @@ def lockstep(args, pols, tr, batches, rtol=1e-4, ptol=2e-5):
     heads0 = {p: ({k: v.clone() for k, v in pol.critic_heads.state_dict().items()},
                   {k: v.clone() for k, v in pol.target_critic_heads.state_dict().items()}) for p, pol in pols.items()}
     shapes = noise_shapes(tr)
-    worst = {"info": 0.0, "param": 0.0, "prio": 0.0}
-    for batch in batches:
+    worst = {"info": 0.0, "param": 0.0, "prio": 0.0, "grad": 0.0}
+    for s, batch in enumerate(batches):
         B = np.asarray(batch[0]["policy_0"]).shape[1]
         for p in sorted(pols):
+            tail0 = actor_tail_params(pols[p])
             rng_before = torch.get_rng_state()
             info, prio, _ = tr.shared_train_policy_on_batch(p, batch)
             rng_after = torch.get_rng_state()
             torch.set_rng_state(rng_before)
             tn, an = draw_noise_multi_md(shapes, p, B)
             assert torch.equal(torch.get_rng_state(), rng_after), p
-            ref, rprio, _ = step_multi_md(learners, p, batch, tn, an)
+            ref, rprio, grads = step_multi_md(learners, p, batch, tn, an)
             assert info["update_actor"] is True
+            assert_actor_tail_unchanged(pols[p], tail0)
+            errs = grad_errors(clipped_engine_grads(tr, pols[p], ref, args.max_grad_norm, p), grads, rtol, "step %d %s" % (s, p))
+            worst["grad"] = max([worst["grad"]] + list(errs.values()))
             for k, v in ref.items():
                 d = abs(float(info[k]) - v) / max(1.0, abs(v))
                 worst["info"] = max(worst["info"], d)
@@ -244,10 +249,19 @@ def engine_against_golden(name, ptol_lr=5e-3):
     for s in range(steps):
         for p in p_ids:
             torch.set_rng_state(torch.from_numpy(golden_rng_before(g, s, p, p_ids)))
+            tail0 = actor_tail_params(pols[p])
             info, prio, _ = tr.shared_train_policy_on_batch(p, golden_batch_multi(g, s, p, p_ids))
             assert np.array_equal(torch.get_rng_state().numpy(), g["s%d.%s.rng_after" % (s, p)]), (s, p)
             for k in ("critic_loss", "critic_grad_norm", "actor_loss", "actor_grad_norm"):
                 assert rel_err(float(info[k]), g["s%d.%s.%s" % (s, p, k)]) < 1e-4, (s, p, k)
+            assert_actor_tail_unchanged(pols[p], tail0)
+            # every clipped gradient tensor the fixture records (each policy's first update), 1e-4 x max|ref| each
+            key = lambda net, k: "s%d.%s.grad.%s.%s" % (s, p, net, k)
+            ref = {net: {k: g[key(net, k)] for k in ours if key(net, k) in g} for net, ours in engine_grads(tr, pols[p], p).items()}
+            if s == 0:
+                assert ref["critic"] and ref["actor"], p
+            norms = {k: g["s%d.%s.%s" % (s, p, k)] for k in ("critic_grad_norm", "actor_grad_norm")}
+            grad_errors(clipped_engine_grads(tr, pols[p], norms, args.max_grad_norm, p), ref, 1e-4, "step %d %s" % (s, p))
             if prio is not None:
                 assert rel_err(np.asarray(prio), g["s%d.%s.prio" % (s, p)]) < 1e-4, (s, p)
             if s == 0:
