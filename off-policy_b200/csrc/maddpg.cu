@@ -430,15 +430,22 @@ __global__ void __launch_bounds__(256) k_mlp_dgi_cols(const float* __restrict__ 
 // =====================================================================================================
 // handle
 // =====================================================================================================
+// The regions of one pass of a network over its rows (offsets in floats into the workspace).  Slot k of gi / h / out belongs to copy k
+// of the network (0: live, 1: target); a pass that runs one copy only has that copy's slot.
+struct MxPassWs {
+  int64_t x;                // critic passes: the packed input rows [M][ldc]
+  int64_t gi[2], h[2];      // [M][3H] GRU input rows (cfg.mlp: the head outputs in columns [0, OD)), [M][H] hidden states
+  int64_t u1, u2, st0, st1, st2, sto, gates, hn;      // the live copy's activations, kept for the backward
+  int64_t out[2];           // head outputs [M][OD]
+  int64_t dout, dh, dgi;    // gradients at the head outputs, the hidden states and the GRU input rows
+};
+
 struct MxMaddpgWs {
-  // actor (rows Ma = B*(T+1)*N)
-  int64_t a_gi[2], a_h[2], a_u1, a_u2, a_st0, a_st1, a_st2, a_sto, a_gates, a_hn, a_out, a_nact, a_dout, a_dh, a_dgi, a_act, a_soft;
-  // critic sequences (rows Mc = B*T)
-  int64_t c_x, c_gi[2], c_h[2], c_u1, c_u2, c_st0, c_st1, c_st2, c_sto, c_gates, c_hn, c_q, c_dq, c_dh, c_dgi, c_err;
-  // target branch (rows Mc)
-  int64_t t_x, t_gi, t_h, t_q, t_qmin;
-  // actor-phase branch (rows Mr = N*B*T)
-  int64_t r_x, r_h0, r_gi, r_h, r_u1, r_u2, r_st0, r_st1, r_st2, r_sto, r_gates, r_hn, r_q, r_dout, r_dh, r_dgi, r_dx;
+  struct : MxPassWs { int64_t act, soft; } a;   // actor rows Ma = B*(T+1)*N; out[1]: target actions; act / soft: the live actor's Gumbel sample
+  struct : MxPassWs { int64_t err; } c;         // critic over the buffer sequences, rows Mc = B*T; err: TD errors [K][Mc]
+  struct : MxPassWs { int64_t qmin; } t;        // target branch, rows Mc (target slots); qmin: min over the target heads
+  struct : MxPassWs { int64_t h0, dx; } r;      // agent-replaced copies, rows Mr = N*B*T (live slots); h0: critic state before the step,
+                                                // dx: gradient at the input rows
   int64_t gpart_a, gpart_c, grad_a, grad_c, spart, info, prio, adam_ta, adam_tc, scal_c, scal_a;
   int64_t tc_da2, tc_da1, tc_imgT, tc_acc, tc_acc_cols;      // scratch of the tensor-core backward (option wgrad_tc), shared by the critic and actor updates
   int64_t cent_acts, cent_nacts;        // [B*T][ca_ld] centralised action vectors assembled from all policies (cent_act_dim > 0)
@@ -470,16 +477,6 @@ static ActSegs act_segs(const mx_maddpg_cfg* c) {
   for (int i = 0; i < c->n_act_seg; ++i) sg.len[i] = c->act_seg[i];
   return sg;
 }
-// k_act_transform arguments for the M actor rows of cfg c.  n_act_seg > 0 is a MultiDiscrete action (one segment included), which takes
-// no available-action mask (MADDPGPolicy.py:73-89); maddpg_check allows it on the MLP learner only
-static ActXformArgs act_xform_args(const mx_maddpg_cfg* c, int M, int mode, const float* avail, int avail_ld) {
-  ActXformArgs ax;
-  memset(&ax, 0, sizeof(ax));
-  ax.M = M; ax.Ac = c->act_dim; ax.mode = mode; ax.sg = act_segs(c);
-  ax.avail = c->n_act_seg > 0 ? nullptr : avail; ax.avail_ld = avail_ld;
-  return ax;
-}
-
 static int maddpg_check(const mx_maddpg_cfg* c) {
   if (!c) { mx_set_error("null cfg"); return 1; }
   if (c->hidden != MX_H) { mx_set_error("hidden_size %d unsupported: kernels are specialised for %d", c->hidden, MX_H); return 1; }
@@ -604,19 +601,23 @@ static int64_t maddpg_ws_layout(const mx_maddpg_cfg* c, int64_t Pa, int64_t Pc, 
   const int64_t ldc = mx_round_up(critic_in_dim(c), 4);
   int64_t o = 0;
   auto tk = [&](int64_t n) { int64_t r = o; o += (n + 63) / 64 * 64; return r; };
-  for (int k = 0; k < 2; ++k) { W->a_gi[k] = tk(Ma * MX_G); W->a_h[k] = tk(Ma * MX_H); }
-  W->a_u1 = tk(Ma * MX_H); W->a_u2 = tk(Ma * MX_H); W->a_st0 = tk(Ma * 2); W->a_st1 = tk(Ma * 2); W->a_st2 = tk(Ma * 2); W->a_sto = tk(Ma * 2);
-  W->a_gates = tk(Ma * MX_G); W->a_hn = tk(Ma * MX_H); W->a_out = tk(Ma * Ac); W->a_nact = tk(Ma * Ac); W->a_dout = tk(Ma * Ac);
-  W->a_dh = tk(Ma * MX_H); W->a_dgi = tk(Ma * MX_G); W->a_act = tk(Ma * Ac); W->a_soft = tk(Ma * Ac);
-  W->c_x = tk(Mc * ldc);
-  for (int k = 0; k < 2; ++k) { W->c_gi[k] = tk(Mc * MX_G); W->c_h[k] = tk(Mc * MX_H); }
-  W->c_u1 = tk(Mc * MX_H); W->c_u2 = tk(Mc * MX_H); W->c_st0 = tk(Mc * 2); W->c_st1 = tk(Mc * 2); W->c_st2 = tk(Mc * 2); W->c_sto = tk(Mc * 2);
-  W->c_gates = tk(Mc * MX_G); W->c_hn = tk(Mc * MX_H); W->c_q = tk(Mc * K); W->c_dq = tk(Mc * K); W->c_dh = tk(Mc * MX_H); W->c_dgi = tk(Mc * MX_G);
-  W->c_err = tk(Mc * K);
-  W->t_x = tk(Mc * ldc); W->t_gi = tk(Mc * MX_G); W->t_h = tk(Mc * MX_H); W->t_q = tk(Mc * K); W->t_qmin = tk(Mc);
-  W->r_x = tk(Mr * ldc); W->r_h0 = tk(Mr * MX_H); W->r_gi = tk(Mr * MX_G); W->r_h = tk(Mr * MX_H); W->r_u1 = tk(Mr * MX_H); W->r_u2 = tk(Mr * MX_H);
-  W->r_st0 = tk(Mr * 2); W->r_st1 = tk(Mr * 2); W->r_st2 = tk(Mr * 2); W->r_sto = tk(Mr * 2); W->r_gates = tk(Mr * MX_G); W->r_hn = tk(Mr * MX_H);
-  W->r_q = tk(Mr * K); W->r_dout = tk(Mr * K); W->r_dh = tk(Mr * MX_H); W->r_dgi = tk(Mr * MX_G); W->r_dx = tk(Mr * ldc);
+  auto acts = [&](MxPassWs& p, int64_t M) {
+    p.u1 = tk(M * MX_H); p.u2 = tk(M * MX_H); p.st0 = tk(M * 2); p.st1 = tk(M * 2); p.st2 = tk(M * 2); p.sto = tk(M * 2);
+    p.gates = tk(M * MX_G); p.hn = tk(M * MX_H);
+  };
+  for (int k = 0; k < 2; ++k) { W->a.gi[k] = tk(Ma * MX_G); W->a.h[k] = tk(Ma * MX_H); }
+  acts(W->a, Ma);
+  W->a.out[0] = tk(Ma * Ac); W->a.out[1] = tk(Ma * Ac); W->a.dout = tk(Ma * Ac);
+  W->a.dh = tk(Ma * MX_H); W->a.dgi = tk(Ma * MX_G); W->a.act = tk(Ma * Ac); W->a.soft = tk(Ma * Ac);
+  W->c.x = tk(Mc * ldc);
+  for (int k = 0; k < 2; ++k) { W->c.gi[k] = tk(Mc * MX_G); W->c.h[k] = tk(Mc * MX_H); }
+  acts(W->c, Mc);
+  W->c.out[0] = tk(Mc * K); W->c.dout = tk(Mc * K); W->c.dh = tk(Mc * MX_H); W->c.dgi = tk(Mc * MX_G);
+  W->c.err = tk(Mc * K);
+  W->t.x = tk(Mc * ldc); W->t.gi[1] = tk(Mc * MX_G); W->t.h[1] = tk(Mc * MX_H); W->t.out[1] = tk(Mc * K); W->t.qmin = tk(Mc);
+  W->r.x = tk(Mr * ldc); W->r.h0 = tk(Mr * MX_H); W->r.gi[0] = tk(Mr * MX_G); W->r.h[0] = tk(Mr * MX_H);
+  acts(W->r, Mr);
+  W->r.out[0] = tk(Mr * K); W->r.dout = tk(Mr * K); W->r.dh = tk(Mr * MX_H); W->r.dgi = tk(Mr * MX_G); W->r.dx = tk(Mr * ldc);
   W->gpart_a = tk((int64_t)npart * Pa); W->gpart_c = tk((int64_t)npart * Pc); W->grad_a = tk(Pa + 8); W->grad_c = tk(Pc + 8);
   W->spart = tk(16); W->info = tk(8); W->prio = tk(B); W->adam_ta = tk(8); W->adam_tc = tk(8); W->scal_c = tk(8); W->scal_a = tk(8);
   {
@@ -682,6 +683,14 @@ static int launch1d(long long work) {
   return (int)g;
 }
 
+// one launch of a file-local kernel, counted and marked for the profiler
+#define MX_RUN(kern, grid, block, s, ...)             \
+  do {                                                \
+    MX_LAUNCH(kern, grid, block, 0, s, __VA_ARGS__);  \
+    MX_COUNT();                                       \
+    MX_MARK(#kern, s);                                \
+  } while (0)
+
 // kernel that only publishes the two loss scalars in the layout k_adam expects: grad[P+0] = denominator, [P+1] = loss numerator
 __global__ void k_set_scalars(float* grad_tail, const float* scal) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -689,7 +698,8 @@ __global__ void k_set_scalars(float* grad_tail, const float* scal) {
   }
 }
 
-static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts, cudaStream_t s) {
+// front_parts / head_parts: the gradient partials k_front_bwd and k_head_bwd wrote
+static int optimise(mx_maddpg* h, bool actor, int front_parts, int head_parts, cudaStream_t s) {
   const mx_maddpg_cfg& c = h->cfg;
   const MxNetLayout& L = actor ? h->actor : h->critic;
   const int64_t P = actor ? h->Pa : h->Pc;
@@ -700,7 +710,7 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
   o.adam_m = actor ? h->m_a : h->m_c; o.adam_v = actor ? h->v_a : h->v_c;
   o.gpart = ws + (actor ? h->W.gpart_a : h->W.gpart_c); o.grad = ws + (actor ? h->W.grad_a : h->W.grad_c); o.P = P;
   o.nseg = 2;
-  o.seg_begin[0] = 0; o.seg_end[0] = L.lno_g; o.seg_parts[0] = parts[0];
+  o.seg_begin[0] = 0; o.seg_end[0] = L.lno_g; o.seg_parts[0] = front_parts;
   o.seg_begin[1] = L.lno_g; o.seg_end[1] = (int)P; o.seg_parts[1] = head_parts;
   if (c.mlp) {        // every gradient comes from k_front_bwd; the critic's trained range stops at its trunk (the frozen heads follow it)
     o.nseg = 1;
@@ -713,10 +723,289 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
   o.lr = c.lr; o.beta1 = c.adam_beta1; o.beta2 = c.adam_beta2; o.eps = c.adam_eps; o.max_grad_norm = c.max_grad_norm; o.tau = c.tau;
   o.weight_decay = c.weight_decay;
   if (mx_launch_grad_reduce(o, s)) return 1;     // (its scalar block bumps the Adam step count; the loss scalars come from the loss kernel)
-  MX_LAUNCH(k_set_scalars, dim3(1), dim3(32), 0, s, o.grad + o.P, (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c)));
-  MX_COUNT();
-  MX_MARK("k_set_scalars", s);
+  MX_RUN(k_set_scalars, dim3(1), dim3(32), s, o.grad + o.P, (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c)));
   return mx_launch_adam(o, s);
+}
+
+// ---- the launches of one update: each builder fills its arguments from (network, pass) and the learner-wide settings; the phase lists
+// below state only what differs between launches (copies of the network, row counts, h0, a data-gradient target, noise)
+enum Net { ACTOR, CRITIC };
+enum { LIVE = 1, TARGET = 2, BOTH = 3 };      // the copies of a network a forward runs; copy k uses slot k of the pass's regions
+
+struct NetRef {             // one network of the learner
+  const MxNetLayout& L;
+  float* th[2];             // live, target parameters
+  float* gpart;             // its gradient partials
+  int64_t P;
+};
+
+struct Step {               // one call of learner h over batch b on stream s
+  mx_maddpg* h;
+  const mx_batch* b;
+  cudaStream_t s;
+  const mx_maddpg_cfg& c;
+  const MxMaddpgWs& W;
+  float* ws;
+  Step(mx_maddpg* h_, const mx_batch* b_, cudaStream_t s_) : h(h_), b(b_), s(s_), c(h_->cfg), W(h_->W), ws(h_->ws) {}
+
+  NetRef net(Net n) const {
+    if (n == ACTOR) return {h->actor, {h->th_a, h->th_a_tgt}, ws + W.gpart_a, h->Pa};
+    return {h->critic, {h->th_c, h->th_c_tgt}, ws + W.gpart_c, h->Pc};
+  }
+  int ldc() const { return mx_round_up(critic_in_dim(&c), 4); }
+  int Ma() const { return b->B * (c.episode_len + 1) * c.n_agents; }      // actor rows
+
+  // every front-layer launch of net n over pass p: input rows (actor: the batch's observations; critic: the pass's packed rows) and settings
+  template <class Args> void front_common(Args& a, Net n, const MxPassWs& p) const {
+    if (n == ACTOR) { a.X = b->obs; a.ldx = b->obs_ld; }
+    else { a.X = ws + p.x; a.ldx = ldc(); }
+    a.feature_norm = c.no_feature_norm ? 0 : 1; a.act_tanh = c.use_tanh;
+    a.L = net(n).L;
+  }
+
+  // front layers of the copies `sel` of net n over the M rows of pass p; keep: also the live copy's activations, for a backward
+  int front_fwd(Net n, const MxPassWs& p, int M, int sel, bool keep) const {
+    const NetRef nr = net(n);
+    FrontFwdArgs a;
+    memset(&a, 0, sizeof(a));
+    front_common(a, n, p);
+    a.M = M;
+    const int first = sel == TARGET ? 1 : 0, nets = sel == BOTH ? 2 : 1;
+    for (int k = 0; k < nets; ++k) { a.theta[k] = nr.th[first + k]; a.gi[k] = ws + p.gi[first + k]; }
+    if (keep) { a.u1 = ws + p.u1; a.u2 = ws + p.u2; a.st0 = ws + p.st0; a.st1 = ws + p.st1; a.st2 = ws + p.st2; }
+    a.tc_acc = ws + W.tc_acc; a.tc_acc_cols = (int)W.tc_acc_cols;
+    return mx_launch_front_fwd(a, nets, s);
+  }
+
+  // GRU of the copies `sel` of net n over pass p: R sequences of T+1 steps, N interleaved per step, starting from h0 (null: zeros)
+  int gru_fwd(Net n, const MxPassWs& p, int sel, int R, int T, int N, const float* h0) const {
+    const NetRef nr = net(n);
+    GruFwdArgs a;
+    memset(&a, 0, sizeof(a));
+    const int first = sel == TARGET ? 1 : 0, nets = sel == BOTH ? 2 : 1;
+    for (int k = 0; k < nets; ++k) { a.theta[k] = nr.th[first + k]; a.gi[k] = ws + p.gi[first + k]; a.hall[k] = ws + p.h[first + k]; }
+    if (sel & LIVE) { a.gates = ws + p.gates; a.hn = ws + p.hn; }
+    a.whh = nr.L.whh; a.bhh = nr.L.bhh; a.R = R; a.T = T; a.N = N; a.h0 = h0;
+    return mx_launch_gru_fwd(a, nets, s);
+  }
+
+  // the head rows of net n: the actor's Linear(H, Ac) is contiguous; the critic's K Linear(H, 1) are (w_k, b_k) at stride H + 4 (maddpg_layouts)
+  template <class Args> void head_rows(Args& a, Net n) const {
+    const MxNetLayout& L = net(n).L;
+    a.lno_g = L.lno_g; a.lno_b = L.lno_b; a.w = L.wq;
+    if (n == ACTOR) { a.b = L.bq; a.OD = c.act_dim; a.b_stride = 1; a.w_stride = MX_H; }
+    else { a.b = L.wq + MX_H; a.OD = c.num_q; a.b_stride = MX_H + 4; a.w_stride = MX_H + 4; }
+  }
+
+  // head of copy `sel` (LIVE or TARGET) of net n over the M rows of pass p (+ noise) into its out slot and / or the minimum into out_min
+  void head_fwd(Net n, const MxPassWs& p, int sel, int M, const float* noise, float* out_min) const {
+    const int k = sel == TARGET ? 1 : 0;
+    HeadArgs a;
+    memset(&a, 0, sizeof(a));
+    head_rows(a, n);
+    a.theta = net(n).th[k]; a.h = ws + p.h[k]; a.M = M;
+    if (k == 0) a.sto = ws + p.sto;
+    a.noise = noise; a.out = ws + p.out[k]; a.out_min = out_min;
+    MX_RUN(k_head_fwd, dim3(launch1d((long long)M * 32)), dim3(256), s, a);
+  }
+
+  // back through the live head of net n over pass p, p.dout -> p.dh; parts: the gradient partials written, or null for a frozen head
+  void head_bwd(Net n, const MxPassWs& p, int M, int* parts) const {
+    const NetRef nr = net(n);
+    const int grid = mx_imin_host(mx_num_sms(), mx_ceil_div(M, 32));
+    HeadBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    head_rows(a, n);
+    a.theta = nr.th[0]; a.h = ws + p.h[0]; a.sto = ws + p.sto; a.dout = ws + p.dout; a.M = M; a.dh_out = ws + p.dh;
+    a.gpart = parts ? nr.gpart : nullptr; a.P = nr.P;
+    if (parts) *parts = grid;
+    MX_RUN(k_head_bwd, dim3(grid), dim3(256), s, a);
+  }
+
+  // back through the live GRU of net n over pass p, p.dh -> p.dgi (R, T, N, T1, h0 as GruBwdArgs)
+  int gru_bwd(Net n, const MxPassWs& p, int R, int T, int N, int T1, const float* h0) const {
+    const NetRef nr = net(n);
+    GruBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.theta = nr.th[0]; a.whh = nr.L.whh; a.hall = ws + p.h[0]; a.gates = ws + p.gates; a.hn = ws + p.hn; a.dh_out = ws + p.dh;
+    a.dgi = ws + p.dgi; a.R = R; a.T = T; a.N = N; a.T1 = T1; a.h0 = h0;
+    return mx_launch_gru_bwd(a, s);
+  }
+
+  // back through the front layers (and GRU input weights) of the live net n over pass p from p.dgi.  dX null: a weight-gradient launch,
+  // with the tensor-core scratch.  dX set: the frozen critic's data gradient only, which takes no tensor-core scratch (neither
+  // tensor-core kernel computes a data gradient)
+  int front_bwd(Net n, const MxPassWs& p, int M, int T, int N, int T1, const float* h0, float* dX, int* parts) const {
+    const NetRef nr = net(n);
+    FrontBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    front_common(a, n, p);
+    a.M = M; a.T = T; a.N = N; a.T1 = T1; a.h0 = h0; a.theta = nr.th[0];
+    a.u1 = ws + p.u1; a.u2 = ws + p.u2; a.st0 = ws + p.st0; a.st1 = ws + p.st1; a.st2 = ws + p.st2; a.dgi = ws + p.dgi;
+    if (c.mlp) a.no_gru = 1;
+    else { a.gates = ws + p.gates; a.hall = ws + p.h[0]; }
+    a.gpart = nr.gpart; a.P = nr.P;
+    if (dX) {
+      a.dX = dX; a.skip_wgrad = 1;
+    } else {
+      a.da2_out = ws + W.tc_da2; a.da1_out = ws + W.tc_da1; a.tc_imgT = ws + W.tc_imgT;
+      a.tc_acc = ws + W.tc_acc; a.tc_acc_cols = (int)W.tc_acc_cols;
+    }
+    int unused = 0;
+    return mx_launch_front_bwd(a, parts ? parts : &unused, s);
+  }
+
+  // the critic's input rows [s | actions] of one pass: mode 0 the buffer actions into c.x, 1 the target actions at the next step into
+  // t.x, 2 the agent-replaced copies into r.x (the recurrent learner: with the critic state before each step)
+  void pack_critic_in(int mode) const {
+    PackArgs pk;
+    memset(&pk, 0, sizeof(pk));
+    pk.mode = mode; pk.B = b->B; pk.T = c.episode_len; pk.N = c.n_agents; pk.S = c.state_dim; pk.Ac = c.act_dim;
+    pk.share = b->share; pk.share_ld = b->share_ld; pk.acts = b->acts; pk.act_ld = b->act_ld; pk.ldx = ldc();
+    if (c.cent_act_dim > 0) {
+      pk.CA = c.cent_act_dim; pk.off = c.act_offset; pk.ca_ld = mx_round_up(c.cent_act_dim, 4); pk.cent_acts = ws + W.cent_acts; pk.cent_nacts = ws + W.cent_nacts;
+    }
+    long long rows = (long long)b->B * c.episode_len;
+    if (mode == 0) {
+      pk.x = ws + W.c.x;
+    } else if (mode == 1) {
+      pk.x = ws + W.t.x; pk.actor_out = ws + W.a.out[1];
+    } else {
+      pk.x = ws + W.r.x; pk.actor_out = ws + (c.discrete ? W.a.act : W.a.out[0]);
+      if (!c.mlp) { pk.hseq = ws + W.c.h[0]; pk.h0 = ws + W.r.h0; }
+      rows *= c.n_agents;
+    }
+    MX_RUN(k_pack_critic_in, dim3(launch1d(rows * pk.ldx)), dim3(256), s, pk);
+  }
+
+  // Discrete actions of the actor rows: mode 0 arg-max one-hot, 1 hard Gumbel-softmax of logits (+ gumbel).  MultiDiscrete (n_act_seg
+  // > 0, one segment included) takes no available-action mask (MADDPGPolicy.py:73-89); maddpg_check allows it on the MLP learner only
+  void act_transform(int mode, const float* logits, const float* gumbel, float* out, float* soft) const {
+    ActXformArgs ax;
+    memset(&ax, 0, sizeof(ax));
+    ax.M = Ma(); ax.Ac = c.act_dim; ax.mode = mode; ax.sg = act_segs(&c);
+    ax.avail = c.n_act_seg > 0 ? nullptr : b->avail; ax.avail_ld = b->act_ld;
+    ax.logits = logits; ax.gumbel = gumbel; ax.out = out; ax.soft = soft;
+    MX_RUN(k_act_transform, dim3(launch1d(Ma())), dim3(256), s, ax);
+  }
+
+  // d(critic input) of the agent-replaced copies -> the actor's head outputs: a.dout, or the MLP actor's "gi" gradient rows a.dgi
+  void scatter_actor_grad() const {
+    MX_RUN(k_scatter_actor_grad, dim3(launch1d(Ma())), dim3(256), s, (const float*)(ws + W.r.dx), ldc(), b->B, c.episode_len, c.n_agents,
+           c.state_dim, c.act_dim, (const float*)(c.discrete ? ws + W.a.soft : nullptr), ws + (c.mlp ? W.a.dgi : W.a.dout), c.act_offset,
+           c.mlp ? (int)MX_G : c.act_dim, act_segs(&c));
+  }
+
+  // cfg.mlp: the head outputs in columns [0, OD) of the "gi" rows at offset gi (+ noise) into out and / or their minimum into out_min
+  void mlp_head_cols(int64_t gi, int M, int OD, const float* noise, float* out, float* out_min) const {
+    MX_RUN(k_mlp_head_cols, dim3(launch1d(M)), dim3(256), s, (const float*)(ws + gi), M, OD, noise, out, out_min);
+  }
+
+  // cfg.mlp: the gradient at the critic's head outputs p.dout as the "gi" gradient rows p.dgi that k_front_bwd reads
+  void mlp_dgi_cols(const MxPassWs& p, int M) const {
+    MX_RUN(k_mlp_dgi_cols, dim3(launch1d((long long)M * MX_G)), dim3(256), s, (const float*)(ws + p.dout), c.num_q, M, ws + p.dgi);
+  }
+
+  // TD target, critic loss, PER priorities: per sequence (recurrent) or the mean over the heads (MLP, maddpg.py:144: no per_nu)
+  void critic_loss() const {
+    const int T = c.episode_len, N = c.n_agents;
+    CriticLossArgs cl;
+    memset(&cl, 0, sizeof(cl));
+    cl.B = b->B; cl.T = T; cl.N = N; cl.K = c.num_q; cl.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; cl.ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : T;
+    cl.qpred = ws + W.c.out[0]; cl.qnext_min = ws + W.t.qmin; cl.rewards = b->rewards; cl.dones_env = b->dones_env;
+    cl.weights = c.use_per ? b->weights : nullptr; cl.gamma = c.gamma; cl.huber_delta = c.huber_delta; cl.per_eps = c.per_eps;
+    if (c.mlp) cl.prio_mean_k = 1;
+    else cl.per_nu = c.per_nu;
+    cl.use_huber = c.use_huber; cl.dq = ws + W.c.dout; cl.err = ws + W.c.err; cl.scal = ws + W.scal_c; cl.prio = c.use_per ? ws + W.prio : nullptr;
+    MX_RUN(k_critic_loss, dim3(1), dim3(256), s, cl);
+  }
+
+  // actor loss through critic head 0 on the agent-replaced copies, masked by the agents' dones or (MLP) by valid_transition
+  void actor_loss() const {
+    const int T = c.episode_len, N = c.n_agents;
+    ActorLossArgs al;
+    memset(&al, 0, sizeof(al));
+    al.B = b->B; al.T = T; al.N = N; al.K = c.num_q; al.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; al.qa = ws + W.r.out[0]; al.dones = b->dones;
+    if (c.mlp) { al.valid = h->valid; al.valid_idx = b->idx; }
+    al.dout = ws + W.r.dout; al.scal = ws + W.scal_a;
+    MX_RUN(k_actor_loss, dim3(1), dim3(256), s, al);
+  }
+
+  // The actor's copies `sel` over its rows Ma = B*(T+1)*N; the target copy's head (+ MATD3 noise) gives the target actions a.out[1],
+  // for Discrete actions arg-max one-hot with the next-avail mask (MADDPG) / a hard Gumbel-softmax sample (MATD3; the head added the
+  // draw).  The MLP actor's live head runs in its step's actor phase.
+  int actor_fwd(int sel, const float* target_noise_dev) const {
+    const int B = b->B, T = c.episode_len, N = c.n_agents;
+    if (front_fwd(ACTOR, W.a, Ma(), sel, (sel & LIVE) != 0)) return 1;
+    if (!c.mlp) {
+      if (gru_fwd(ACTOR, W.a, sel, B * N, T, N, nullptr)) return 1;
+      if (sel & LIVE) head_fwd(ACTOR, W.a, LIVE, Ma(), nullptr, nullptr);
+    }
+    if (!(sel & TARGET)) return 0;
+    const float* noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
+    // cfg.mlp (maddpg.py:64-74): the head sits in the weight_ih slot; the noise rows are the step-1 (next-observation) rows [b][2][N][Ac]
+    if (c.mlp) mlp_head_cols(W.a.gi[1], Ma(), c.act_dim, noise, ws + W.a.out[1], nullptr);
+    else head_fwd(ACTOR, W.a, TARGET, Ma(), noise, nullptr);
+    if (c.discrete) act_transform(c.target_noise > 0.f ? 1 : 0, ws + W.a.out[1], nullptr, ws + W.a.out[1], nullptr);
+    return 0;
+  }
+};
+// ---- recurrent learner: shared_train_policy_on_batch (r_maddpg.py:114-331) ------------------------------------------------------------
+// Several policies (cent_act_dim > 0): the centralised action vectors were assembled by mx_maddpg_cent_contribute.
+static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor) {
+  const MxMaddpgWs& W = st.W;
+  float* ws = st.ws;
+  const int B = st.b->B, T = st.c.episode_len, N = st.c.n_agents;
+  const int Ma = B * (T + 1) * N, Mc = B * T, Mr = N * B * T;
+
+  // ---------- A. actor: live + target over the T+1 steps ----------
+  if (st.actor_fwd(BOTH, target_noise_dev)) return 1;
+
+  // ---------- B. critic over the buffer sequence (live + target) ----------
+  st.pack_critic_in(0);
+  if (st.front_fwd(CRITIC, W.c, Mc, BOTH, true)) return 1;
+  if (st.gru_fwd(CRITIC, W.c, BOTH, B, T - 1, 1, nullptr)) return 1;
+  st.head_fwd(CRITIC, W.c, LIVE, Mc, nullptr, nullptr);
+
+  // ---------- C. target Q: one branch step per (b,t) from the target critic's buffer state ----------
+  st.pack_critic_in(1);
+  if (st.front_fwd(CRITIC, W.t, Mc, TARGET, false)) return 1;
+  if (st.gru_fwd(CRITIC, W.t, TARGET, Mc, 0, 1, ws + W.c.h[1])) return 1;
+  st.head_fwd(CRITIC, W.t, TARGET, Mc, nullptr, ws + W.t.qmin);
+
+  // ---------- D. TD target, critic loss ----------
+  st.critic_loss();
+
+  // ---------- E. critic backward + Adam ----------
+  int head_parts = 0, parts = 0;
+  st.head_bwd(CRITIC, W.c, Mc, &head_parts);
+  if (st.gru_bwd(CRITIC, W.c, B, T, 1, T, nullptr)) return 1;
+  if (st.front_bwd(CRITIC, W.c, Mc, T, 1, T, nullptr, nullptr, &parts)) return 1;
+  if (optimise(st.h, false, parts, head_parts, st.s)) return 1;
+
+  // ---------- F. actor update with the UPDATED critic ----------
+  if (!update_actor) return 0;
+  // live critic recurrence over the buffer sequence again (its parameters just changed)
+  if (st.front_fwd(CRITIC, W.c, Mc, LIVE, false)) return 1;
+  if (st.gru_fwd(CRITIC, W.c, LIVE, B, T - 1, 1, nullptr)) return 1;
+  // the live actor's hard Gumbel-softmax sample (straight-through), r_maddpg.py:277
+  if (st.c.discrete) st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft);
+  st.pack_critic_in(2);
+  if (st.front_fwd(CRITIC, W.r, Mr, LIVE, true)) return 1;
+  if (st.gru_fwd(CRITIC, W.r, LIVE, Mr, 0, 1, ws + W.r.h0)) return 1;
+  st.head_fwd(CRITIC, W.r, LIVE, Mr, nullptr, nullptr);
+  st.actor_loss();
+  // back through the (frozen) critic to its action inputs
+  st.head_bwd(CRITIC, W.r, Mr, nullptr);
+  if (st.gru_bwd(CRITIC, W.r, Mr, 1, 1, 1, ws + W.r.h0)) return 1;
+  if (st.front_bwd(CRITIC, W.r, Mr, 0, 1, 1, ws + W.r.h0, ws + W.r.dx, nullptr)) return 1;
+  st.scatter_actor_grad();
+  // actor backward + Adam
+  int ahead_parts = 0, aparts = 0;
+  st.head_bwd(ACTOR, W.a, Ma, &ahead_parts);
+  if (st.gru_bwd(ACTOR, W.a, B * N, T, N, T + 1, nullptr)) return 1;
+  if (st.front_bwd(ACTOR, W.a, Ma, T, N, 0, nullptr, nullptr, &aparts)) return 1;
+  return optimise(st.h, true, aparts, ahead_parts, st.s);
 }
 
 // ---- cfg.mlp: shared_train_policy_on_batch of the transition-level trainer (maddpg.py:90-249) ---------------------------------------
@@ -728,134 +1017,46 @@ static int optimise(mx_maddpg* h, bool actor, const int parts[2], int head_parts
 // Several policies (cent_act_dim > 0): the centralised action vectors were assembled by mx_maddpg_cent_contribute, so the step runs
 // only the live actor and never reads its own target actions; the batch is this policy's (rewards, dones_env, shared observation,
 // PER weights, maddpg.py:103-107) and the valid_transition store is this policy's [rows][n_agents].
-static int maddpg_step_mlp(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor,
-                           cudaStream_t s) {
-  const mx_maddpg_cfg& c = h->cfg;
-  float* ws = h->ws;
-  const MxMaddpgWs& W = h->W;
-  const int B = b->B, N = c.n_agents, K = c.num_q, Ac = c.act_dim, S = c.state_dim;
+static int maddpg_step_mlp(const Step& st, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor) {
+  const MxMaddpgWs& W = st.W;
+  float* ws = st.ws;
+  const int B = st.b->B, N = st.c.n_agents, K = st.c.num_q, Ac = st.c.act_dim;
   const int Ma = B * 2 * N, Mc = B, Mr = N * B;
-  const int ldc = mx_round_up(critic_in_dim(&c), 4);
-  const MxNetLayout& LA = h->actor;
-  const MxNetLayout& LC = h->critic;
-  const int fnorm = c.no_feature_norm ? 0 : 1;
-  const bool multi = c.cent_act_dim > 0;
 
   // ---------- A. live + target actor on obs and next_obs; target actions a' from the next_obs rows (maddpg.py:64-74) ----------
-  FrontFwdArgs ff;
-  memset(&ff, 0, sizeof(ff));
-  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
-  ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = fnorm; ff.act_tanh = c.use_tanh;
-  ff.theta[0] = h->th_a; ff.theta[1] = h->th_a_tgt; ff.L = LA;
-  ff.gi[0] = ws + W.a_gi[0]; ff.gi[1] = ws + W.a_gi[1];
-  ff.u1 = ws + W.a_u1; ff.u2 = ws + W.a_u2; ff.st0 = ws + W.a_st0; ff.st1 = ws + W.a_st1; ff.st2 = ws + W.a_st2;
-  if (mx_launch_front_fwd(ff, multi ? 1 : 2, s)) return 1;      // several policies: the target actions come from cent_nacts
-  if (!multi) {
-    MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[1], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
-              ws + W.a_nact, nullptr);
-    MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  }
-  if (c.discrete && !multi) {      // onehot_from_logits with the next-avail mask (MADDPG) / hard Gumbel-softmax, the draw already added (MATD3)
-    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
-    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
-  }
+  if (st.actor_fwd(st.c.cent_act_dim > 0 ? LIVE : BOTH, target_noise_dev)) return 1;
 
   // ---------- B. live critic on (s, a), target critic on (s', a'); TD target, loss, priorities (maddpg.py:112-151) ----------
-  PackArgs pk;
-  memset(&pk, 0, sizeof(pk));
-  pk.B = B; pk.T = 1; pk.N = N; pk.S = S; pk.Ac = Ac; pk.share = b->share; pk.share_ld = b->share_ld; pk.acts = b->acts; pk.act_ld = b->act_ld;
-  pk.ldx = ldc;
-  if (multi) { pk.CA = c.cent_act_dim; pk.off = c.act_offset; pk.ca_ld = mx_round_up(c.cent_act_dim, 4); pk.cent_acts = ws + W.cent_acts; pk.cent_nacts = ws + W.cent_nacts; }
-  pk.mode = 0; pk.x = ws + W.c_x;
-  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-  pk.mode = 1; pk.x = ws + W.t_x; pk.actor_out = ws + W.a_nact;
-  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-  FrontFwdArgs fc;
-  memset(&fc, 0, sizeof(fc));
-  fc.tc_acc = ws + W.tc_acc; fc.tc_acc_cols = (int)W.tc_acc_cols;
-  fc.X = ws + W.c_x; fc.ldx = ldc; fc.M = Mc; fc.feature_norm = fnorm; fc.act_tanh = c.use_tanh; fc.theta[0] = h->th_c; fc.L = LC;
-  fc.gi[0] = ws + W.c_gi[0];
-  fc.u1 = ws + W.c_u1; fc.u2 = ws + W.c_u2; fc.st0 = ws + W.c_st0; fc.st1 = ws + W.c_st1; fc.st2 = ws + W.c_st2;
-  if (mx_launch_front_fwd(fc, 1, s)) return 1;
-  FrontFwdArgs ft;
-  memset(&ft, 0, sizeof(ft));
-  ft.tc_acc = ws + W.tc_acc; ft.tc_acc_cols = (int)W.tc_acc_cols;
-  ft.X = ws + W.t_x; ft.ldx = ldc; ft.M = Mc; ft.feature_norm = fnorm; ft.act_tanh = c.use_tanh; ft.theta[0] = h->th_c_tgt; ft.L = LC; ft.gi[0] = ws + W.t_gi;
-  if (mx_launch_front_fwd(ft, 1, s)) return 1;
-  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mc)), dim3(256), 0, s, (const float*)fc.gi[0], Mc, K, (const float*)nullptr, ws + W.c_q, nullptr);
-  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mc)), dim3(256), 0, s, (const float*)ft.gi[0], Mc, K, (const float*)nullptr, nullptr, ws + W.t_qmin);
-  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  CriticLossArgs cl;
-  memset(&cl, 0, sizeof(cl));
-  cl.B = B; cl.T = 1; cl.N = N; cl.K = K; cl.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : N; cl.ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : 1;
-  cl.qpred = ws + W.c_q; cl.qnext_min = ws + W.t_qmin; cl.rewards = b->rewards; cl.dones_env = b->dones_env;
-  cl.weights = c.use_per ? b->weights : nullptr; cl.gamma = c.gamma; cl.huber_delta = c.huber_delta; cl.per_eps = c.per_eps;
-  cl.use_huber = c.use_huber; cl.prio_mean_k = 1; cl.dq = ws + W.c_dq; cl.err = ws + W.c_err; cl.scal = ws + W.scal_c; cl.prio = c.use_per ? ws + W.prio : nullptr;
-  MX_LAUNCH(k_critic_loss, dim3(1), dim3(256), 0, s, cl); MX_COUNT(); MX_MARK("k_critic_loss", s);
+  st.pack_critic_in(0);
+  st.pack_critic_in(1);
+  if (st.front_fwd(CRITIC, W.c, Mc, LIVE, true)) return 1;
+  if (st.front_fwd(CRITIC, W.t, Mc, TARGET, false)) return 1;
+  st.mlp_head_cols(W.c.gi[0], Mc, K, nullptr, ws + W.c.out[0], nullptr);
+  st.mlp_head_cols(W.t.gi[1], Mc, K, nullptr, nullptr, ws + W.t.qmin);
+  st.critic_loss();
 
   // ---------- C. critic backward through the frozen live heads into the trunk; clip + Adam over the trunk ----------
-  MX_LAUNCH(k_mlp_dgi_cols, dim3(launch1d((long long)Mc * MX_G)), dim3(256), 0, s, (const float*)(ws + W.c_dq), K, Mc, ws + W.c_dgi);
-  MX_COUNT(); MX_MARK("k_mlp_dgi_cols", s);
-  int parts[2] = {0, 0};
-  FrontBwdArgs fb;
-  memset(&fb, 0, sizeof(fb));
-  fb.X = ws + W.c_x; fb.ldx = ldc; fb.M = Mc; fb.T = 1; fb.N = 1; fb.feature_norm = fnorm; fb.act_tanh = c.use_tanh; fb.no_gru = 1;
-  fb.theta = h->th_c; fb.L = LC; fb.u1 = fc.u1; fb.u2 = fc.u2; fb.st0 = fc.st0; fb.st1 = fc.st1; fb.st2 = fc.st2; fb.dgi = ws + W.c_dgi;
-  fb.gpart = ws + W.gpart_c; fb.P = h->Pc;
-  fb.da2_out = ws + W.tc_da2; fb.da1_out = ws + W.tc_da1; fb.tc_imgT = ws + W.tc_imgT;      // (option wgrad_tc)
-  fb.tc_acc = ws + W.tc_acc; fb.tc_acc_cols = (int)W.tc_acc_cols;
-  if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
-  if (optimise(h, false, parts, 0, s)) return 1;
+  st.mlp_dgi_cols(W.c, Mc);
+  int parts = 0;
+  if (st.front_bwd(CRITIC, W.c, Mc, 1, 1, 0, nullptr, nullptr, &parts)) return 1;
+  if (optimise(st.h, false, parts, 0, st.s)) return 1;
   if (!update_actor) return 0;
 
   // ---------- D. actor loss through head 0 of the UPDATED critic on the agent-replaced copies, masked by valid_transition ----------
-  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[0], Ma, Ac, (const float*)nullptr, ws + W.a_out, nullptr);
-  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  if (c.discrete) {    // get_actions(obs, avail, use_gumbel=True): hard Gumbel-softmax, straight-through (maddpg.py:209)
-    ActXformArgs ax = act_xform_args(&c, Ma, 1, b->avail, b->act_ld);
-    ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
-    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
-  }
-  pk.mode = 2; pk.x = ws + W.r_x; pk.actor_out = ws + (c.discrete ? W.a_act : W.a_out);
-  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mr * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-  FrontFwdArgs fr;
-  memset(&fr, 0, sizeof(fr));
-  fr.tc_acc = ws + W.tc_acc; fr.tc_acc_cols = (int)W.tc_acc_cols;
-  fr.X = ws + W.r_x; fr.ldx = ldc; fr.M = Mr; fr.feature_norm = fnorm; fr.act_tanh = c.use_tanh; fr.theta[0] = h->th_c; fr.L = LC; fr.gi[0] = ws + W.r_gi;
-  fr.u1 = ws + W.r_u1; fr.u2 = ws + W.r_u2; fr.st0 = ws + W.r_st0; fr.st1 = ws + W.r_st1; fr.st2 = ws + W.r_st2;
-  if (mx_launch_front_fwd(fr, 1, s)) return 1;
-  MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Mr)), dim3(256), 0, s, (const float*)fr.gi[0], Mr, K, (const float*)nullptr, ws + W.r_q, nullptr);
-  MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  ActorLossArgs al;
-  memset(&al, 0, sizeof(al));
-  al.B = B; al.T = 1; al.N = N; al.K = K; al.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : N; al.qa = ws + W.r_q; al.dones = b->dones;
-  al.valid = h->valid; al.valid_idx = b->idx; al.dout = ws + W.r_dout; al.scal = ws + W.scal_a;
-  MX_LAUNCH(k_actor_loss, dim3(1), dim3(256), 0, s, al); MX_COUNT(); MX_MARK("k_actor_loss", s);
+  st.mlp_head_cols(W.a.gi[0], Ma, Ac, nullptr, ws + W.a.out[0], nullptr);
+  // get_actions(obs, avail, use_gumbel=True): hard Gumbel-softmax, straight-through (maddpg.py:209)
+  if (st.c.discrete) st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft);
+  st.pack_critic_in(2);
+  if (st.front_fwd(CRITIC, W.r, Mr, LIVE, true)) return 1;
+  st.mlp_head_cols(W.r.gi[0], Mr, K, nullptr, ws + W.r.out[0], nullptr);
+  st.actor_loss();
   // back through the frozen critic (trunk and live head 0) to its action inputs, then into the actor's head rows
-  MX_LAUNCH(k_mlp_dgi_cols, dim3(launch1d((long long)Mr * MX_G)), dim3(256), 0, s, (const float*)(ws + W.r_dout), K, Mr, ws + W.r_dgi);
-  MX_COUNT(); MX_MARK("k_mlp_dgi_cols", s);
-  FrontBwdArgs fbr;
-  memset(&fbr, 0, sizeof(fbr));
-  fbr.X = ws + W.r_x; fbr.ldx = ldc; fbr.M = Mr; fbr.T = 1; fbr.N = 1; fbr.feature_norm = fnorm; fbr.act_tanh = c.use_tanh; fbr.no_gru = 1;
-  fbr.theta = h->th_c; fbr.L = LC; fbr.u1 = fr.u1; fbr.u2 = fr.u2; fbr.st0 = fr.st0; fbr.st1 = fr.st1; fbr.st2 = fr.st2; fbr.dgi = ws + W.r_dgi;
-  fbr.gpart = ws + W.gpart_c; fbr.P = h->Pc; fbr.dX = ws + W.r_dx; fbr.skip_wgrad = 1;
-  int dummy = 0;
-  if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
-  MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, 1, N, S, Ac,
-            (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dgi, c.act_offset, (int)MX_G, act_segs(&c));
-  MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
-  FrontBwdArgs fba;
-  memset(&fba, 0, sizeof(fba));
-  fba.X = b->obs; fba.ldx = b->obs_ld; fba.M = Ma; fba.T = 1; fba.N = N; fba.feature_norm = fnorm; fba.act_tanh = c.use_tanh; fba.no_gru = 1;
-  fba.theta = h->th_a; fba.L = LA; fba.u1 = ff.u1; fba.u2 = ff.u2; fba.st0 = ff.st0; fba.st1 = ff.st1; fba.st2 = ff.st2; fba.dgi = ws + W.a_dgi;
-  fba.gpart = ws + W.gpart_a; fba.P = h->Pa;
-  fba.da2_out = ws + W.tc_da2; fba.da1_out = ws + W.tc_da1; fba.tc_imgT = ws + W.tc_imgT;
-  fba.tc_acc = ws + W.tc_acc; fba.tc_acc_cols = (int)W.tc_acc_cols;
-  int aparts[2] = {0, 0};
-  if (mx_launch_front_bwd(fba, &aparts[0], s)) return 1;
-  return optimise(h, true, aparts, 0, s);
+  st.mlp_dgi_cols(W.r, Mr);
+  if (st.front_bwd(CRITIC, W.r, Mr, 1, 1, 0, nullptr, ws + W.r.dx, nullptr)) return 1;
+  st.scatter_actor_grad();
+  int aparts = 0;
+  if (st.front_bwd(ACTOR, W.a, Ma, 1, N, 0, nullptr, nullptr, &aparts)) return 1;
+  return optimise(st.h, true, aparts, 0, st.s);
 }
 
 extern "C" int mx_maddpg_step(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, int32_t* update_actor_out, void* stream) {
@@ -874,211 +1075,9 @@ extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* t
   if (c.target_noise > 0.f && !target_noise_dev) { mx_set_error("maddpg step: MATD3 target noise expected"); return 1; }
   const bool update_actor = h->force_update_actor >= 0 ? h->force_update_actor != 0
                                                      : (h->num_updates % (c.actor_update_interval > 0 ? c.actor_update_interval : 1)) == 0;
-  {
-    const bool upd = update_actor;
-    if (c.discrete && upd && !actor_noise_dev) { mx_set_error("maddpg step: discrete actor update needs the Gumbel draws (actor_noise_dev)"); return 1; }
-  }
-  cudaStream_t s = (cudaStream_t)stream;
-  if (c.mlp) {
-    if (maddpg_step_mlp(h, b, target_noise_dev, actor_noise_dev, update_actor, s)) return 1;
-    if (update_actor_out) *update_actor_out = update_actor ? 1 : 0;
-    if (h->force_update_actor < 0) h->num_updates += 1;
-    return 0;
-  }
-  float* ws = h->ws;
-  const MxMaddpgWs& W = h->W;
-  const int B = b->B, T = c.episode_len, N = c.n_agents, K = c.num_q, Ac = c.act_dim, S = c.state_dim;
-  const int Ma = B * (T + 1) * N, Mc = B * T, Mr = N * B * T;
-  const int ldc = mx_round_up(critic_in_dim(&c), 4);
-  const MxNetLayout& LA = h->actor;
-  const MxNetLayout& LC = h->critic;
-  const int hstride = MX_H + 4;
-  const bool multi = c.cent_act_dim > 0;       // several policies: the centralised action vectors were assembled by mx_maddpg_cent_contribute
-
-  // ---------- A. actor: live + target over the T+1 steps ----------
-  FrontFwdArgs ff;
-  memset(&ff, 0, sizeof(ff));
-  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
-  ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
-  ff.theta[0] = h->th_a; ff.theta[1] = h->th_a_tgt; ff.L = LA;
-  ff.gi[0] = ws + W.a_gi[0]; ff.gi[1] = ws + W.a_gi[1];
-  ff.u1 = ws + W.a_u1; ff.u2 = ws + W.a_u2; ff.st0 = ws + W.a_st0; ff.st1 = ws + W.a_st1; ff.st2 = ws + W.a_st2;
-  if (mx_launch_front_fwd(ff, 2, s)) return 1;
-  GruFwdArgs gf;
-  memset(&gf, 0, sizeof(gf));
-  gf.theta[0] = h->th_a; gf.theta[1] = h->th_a_tgt; gf.whh = LA.whh; gf.bhh = LA.bhh;
-  gf.gi[0] = ff.gi[0]; gf.gi[1] = ff.gi[1]; gf.hall[0] = ws + W.a_h[0]; gf.hall[1] = ws + W.a_h[1];
-  gf.gates = ws + W.a_gates; gf.hn = ws + W.a_hn; gf.R = B * N; gf.T = T; gf.N = N;
-  if (mx_launch_gru_fwd(gf, 2, s)) return 1;
-  HeadArgs ha;
-  memset(&ha, 0, sizeof(ha));
-  ha.lno_g = LA.lno_g; ha.lno_b = LA.lno_b; ha.w = LA.wq; ha.b = LA.bq; ha.OD = Ac; ha.b_stride = 1; ha.w_stride = MX_H; ha.M = Ma;
-  ha.theta = h->th_a; ha.h = gf.hall[0]; ha.sto = ws + W.a_sto; ha.out = ws + W.a_out;
-  MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
-  ha.theta = h->th_a_tgt; ha.h = gf.hall[1]; ha.sto = nullptr; ha.out = ws + W.a_nact; ha.noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
-  MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
-  if (c.discrete) {      // target actions: arg-max one-hot (MADDPG) / hard Gumbel-softmax sample (MATD3; the head added the draw)
-    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
-    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
-  }
-
-  // ---------- B. critic over the buffer sequence (live + target) ----------
-  PackArgs pk;
-  memset(&pk, 0, sizeof(pk));
-  pk.B = B; pk.T = T; pk.N = N; pk.S = S; pk.Ac = Ac; pk.share = b->share; pk.share_ld = b->share_ld; pk.acts = b->acts; pk.act_ld = b->act_ld;
-  pk.ldx = ldc;
-  if (multi) { pk.CA = c.cent_act_dim; pk.off = c.act_offset; pk.ca_ld = mx_round_up(c.cent_act_dim, 4); pk.cent_acts = ws + W.cent_acts; pk.cent_nacts = ws + W.cent_nacts; }
-  pk.mode = 0; pk.x = ws + W.c_x;
-  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-  FrontFwdArgs fc;
-  memset(&fc, 0, sizeof(fc));
-  fc.tc_acc = ws + W.tc_acc; fc.tc_acc_cols = (int)W.tc_acc_cols;
-  fc.X = ws + W.c_x; fc.ldx = ldc; fc.M = Mc; fc.feature_norm = c.no_feature_norm ? 0 : 1; fc.act_tanh = c.use_tanh;
-  fc.theta[0] = h->th_c; fc.theta[1] = h->th_c_tgt; fc.L = LC;
-  fc.gi[0] = ws + W.c_gi[0]; fc.gi[1] = ws + W.c_gi[1];
-  fc.u1 = ws + W.c_u1; fc.u2 = ws + W.c_u2; fc.st0 = ws + W.c_st0; fc.st1 = ws + W.c_st1; fc.st2 = ws + W.c_st2;
-  if (mx_launch_front_fwd(fc, 2, s)) return 1;
-  GruFwdArgs gc;
-  memset(&gc, 0, sizeof(gc));
-  gc.theta[0] = h->th_c; gc.theta[1] = h->th_c_tgt; gc.whh = LC.whh; gc.bhh = LC.bhh;
-  gc.gi[0] = fc.gi[0]; gc.gi[1] = fc.gi[1]; gc.hall[0] = ws + W.c_h[0]; gc.hall[1] = ws + W.c_h[1];
-  gc.gates = ws + W.c_gates; gc.hn = ws + W.c_hn; gc.R = B; gc.T = T - 1; gc.N = 1;
-  if (mx_launch_gru_fwd(gc, 2, s)) return 1;
-  HeadArgs hc;
-  memset(&hc, 0, sizeof(hc));
-  hc.lno_g = LC.lno_g; hc.lno_b = LC.lno_b; hc.w = LC.wq; hc.b = LC.wq + MX_H; hc.OD = K; hc.b_stride = hstride; hc.w_stride = hstride; hc.M = Mc;
-  hc.theta = h->th_c; hc.h = gc.hall[0]; hc.sto = ws + W.c_sto; hc.out = ws + W.c_q;
-  MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Mc * 32)), dim3(256), 0, s, hc); MX_COUNT(); MX_MARK("k_head_fwd", s);
-
-  // ---------- C. target Q: one branch step per (b,t) from the target critic's buffer state ----------
-  pk.mode = 1; pk.x = ws + W.t_x; pk.actor_out = ws + W.a_nact;
-  MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mc * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-  FrontFwdArgs ft;
-  memset(&ft, 0, sizeof(ft));
-  ft.tc_acc = ws + W.tc_acc; ft.tc_acc_cols = (int)W.tc_acc_cols;
-  ft.X = ws + W.t_x; ft.ldx = ldc; ft.M = Mc; ft.feature_norm = c.no_feature_norm ? 0 : 1; ft.act_tanh = c.use_tanh; ft.theta[0] = h->th_c_tgt; ft.L = LC; ft.gi[0] = ws + W.t_gi;
-  if (mx_launch_front_fwd(ft, 1, s)) return 1;
-  GruFwdArgs gt;
-  memset(&gt, 0, sizeof(gt));
-  gt.theta[0] = h->th_c_tgt; gt.whh = LC.whh; gt.bhh = LC.bhh; gt.gi[0] = ft.gi[0]; gt.hall[0] = ws + W.t_h;
-  gt.gates = nullptr; gt.hn = nullptr; gt.R = Mc; gt.T = 0; gt.N = 1; gt.h0 = gc.hall[1];
-  if (mx_launch_gru_fwd(gt, 1, s)) return 1;
-  HeadArgs ht = hc;
-  ht.theta = h->th_c_tgt; ht.h = gt.hall[0]; ht.sto = nullptr; ht.out = ws + W.t_q; ht.out_min = ws + W.t_qmin;
-  MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Mc * 32)), dim3(256), 0, s, ht); MX_COUNT(); MX_MARK("k_head_fwd", s);
-
-  // ---------- D. TD target, critic loss ----------
-  CriticLossArgs cl;
-  memset(&cl, 0, sizeof(cl));
-  cl.B = B; cl.T = T; cl.N = N; cl.K = K; cl.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; cl.ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : T; cl.qpred = ws + W.c_q; cl.qnext_min = ws + W.t_qmin; cl.rewards = b->rewards; cl.dones_env = b->dones_env;
-  cl.weights = c.use_per ? b->weights : nullptr; cl.gamma = c.gamma; cl.huber_delta = c.huber_delta; cl.per_nu = c.per_nu; cl.per_eps = c.per_eps;
-  cl.use_huber = c.use_huber; cl.dq = ws + W.c_dq; cl.err = ws + W.c_err; cl.scal = ws + W.scal_c; cl.prio = c.use_per ? ws + W.prio : nullptr;
-  MX_LAUNCH(k_critic_loss, dim3(1), dim3(256), 0, s, cl); MX_COUNT(); MX_MARK("k_critic_loss", s);
-
-  // ---------- E. critic backward + Adam ----------
-  const int head_grid = mx_imin_host(mx_num_sms(), mx_ceil_div(Mc, 32));
-  HeadBwdArgs hb;
-  memset(&hb, 0, sizeof(hb));
-  hb.theta = h->th_c; hb.lno_g = LC.lno_g; hb.lno_b = LC.lno_b; hb.w = LC.wq; hb.b = LC.wq + MX_H; hb.OD = K; hb.b_stride = hstride; hb.w_stride = hstride;
-  hb.h = gc.hall[0]; hb.sto = ws + W.c_sto; hb.dout = ws + W.c_dq; hb.M = Mc; hb.dh_out = ws + W.c_dh; hb.gpart = ws + W.gpart_c; hb.P = h->Pc;
-  MX_LAUNCH(k_head_bwd, dim3(head_grid), dim3(256), 0, s, hb); MX_COUNT(); MX_MARK("k_head_bwd", s);
-  GruBwdArgs gb;
-  memset(&gb, 0, sizeof(gb));
-  gb.theta = h->th_c; gb.whh = LC.whh; gb.hall = gc.hall[0]; gb.gates = gc.gates; gb.hn = gc.hn; gb.dh_out = hb.dh_out; gb.dgi = ws + W.c_dgi;
-  gb.R = B; gb.T = T; gb.N = 1; gb.T1 = T;
-  if (mx_launch_gru_bwd(gb, s)) return 1;
-  int parts[2] = {0, 0};
-  FrontBwdArgs fb;
-  memset(&fb, 0, sizeof(fb));
-  fb.X = ws + W.c_x; fb.ldx = ldc; fb.M = Mc; fb.T = T; fb.N = 1; fb.T1 = T; fb.feature_norm = c.no_feature_norm ? 0 : 1; fb.act_tanh = c.use_tanh; fb.theta = h->th_c; fb.L = LC;
-  fb.u1 = fc.u1; fb.u2 = fc.u2; fb.st0 = fc.st0; fb.st1 = fc.st1; fb.st2 = fc.st2; fb.dgi = gb.dgi; fb.gates = gc.gates; fb.hall = gc.hall[0];
-  fb.gpart = ws + W.gpart_c; fb.P = h->Pc;
-  fb.da2_out = ws + W.tc_da2; fb.da1_out = ws + W.tc_da1; fb.tc_imgT = ws + W.tc_imgT;      // (option wgrad_tc)
-  fb.tc_acc = ws + W.tc_acc; fb.tc_acc_cols = (int)W.tc_acc_cols;
-  if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
-  if (optimise(h, false, parts, head_grid, s)) return 1;
-
-  // ---------- F. actor update with the UPDATED critic ----------
-  if (update_actor) {
-    // live critic recurrence over the buffer sequence again (its parameters just changed)
-    FrontFwdArgs f2;
-    memset(&f2, 0, sizeof(f2));
-    f2.tc_acc = ws + W.tc_acc; f2.tc_acc_cols = (int)W.tc_acc_cols;
-    f2.X = ws + W.c_x; f2.ldx = ldc; f2.M = Mc; f2.feature_norm = c.no_feature_norm ? 0 : 1; f2.act_tanh = c.use_tanh; f2.theta[0] = h->th_c; f2.L = LC; f2.gi[0] = ws + W.c_gi[0];
-    if (mx_launch_front_fwd(f2, 1, s)) return 1;
-    GruFwdArgs g2;
-    memset(&g2, 0, sizeof(g2));
-    g2.theta[0] = h->th_c; g2.whh = LC.whh; g2.bhh = LC.bhh; g2.gi[0] = f2.gi[0]; g2.hall[0] = ws + W.c_h[0]; g2.R = B; g2.T = T - 1; g2.N = 1;
-    g2.gates = ws + W.c_gates; g2.hn = ws + W.c_hn;
-    if (mx_launch_gru_fwd(g2, 1, s)) return 1;
-    if (c.discrete) {    // the live actor's hard Gumbel-softmax sample (straight-through), r_maddpg.py:277
-      ActXformArgs ax = act_xform_args(&c, Ma, 1, b->avail, b->act_ld);
-      ax.logits = ws + W.a_out; ax.gumbel = actor_noise_dev; ax.out = ws + W.a_act; ax.soft = ws + W.a_soft;
-      MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
-    }
-    pk.mode = 2; pk.x = ws + W.r_x; pk.actor_out = ws + (c.discrete ? W.a_act : W.a_out); pk.hseq = g2.hall[0]; pk.h0 = ws + W.r_h0;
-    MX_LAUNCH(k_pack_critic_in, dim3(launch1d((long long)Mr * ldc)), dim3(256), 0, s, pk); MX_COUNT(); MX_MARK("k_pack_critic_in", s);
-    FrontFwdArgs fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.tc_acc = ws + W.tc_acc; fr.tc_acc_cols = (int)W.tc_acc_cols;
-    fr.X = ws + W.r_x; fr.ldx = ldc; fr.M = Mr; fr.feature_norm = c.no_feature_norm ? 0 : 1; fr.act_tanh = c.use_tanh; fr.theta[0] = h->th_c; fr.L = LC; fr.gi[0] = ws + W.r_gi;
-    fr.u1 = ws + W.r_u1; fr.u2 = ws + W.r_u2; fr.st0 = ws + W.r_st0; fr.st1 = ws + W.r_st1; fr.st2 = ws + W.r_st2;
-    if (mx_launch_front_fwd(fr, 1, s)) return 1;
-    GruFwdArgs gr;
-    memset(&gr, 0, sizeof(gr));
-    gr.theta[0] = h->th_c; gr.whh = LC.whh; gr.bhh = LC.bhh; gr.gi[0] = fr.gi[0]; gr.hall[0] = ws + W.r_h;
-    gr.gates = ws + W.r_gates; gr.hn = ws + W.r_hn; gr.R = Mr; gr.T = 0; gr.N = 1; gr.h0 = ws + W.r_h0;
-    if (mx_launch_gru_fwd(gr, 1, s)) return 1;
-    HeadArgs hr = hc;
-    hr.theta = h->th_c; hr.h = gr.hall[0]; hr.sto = ws + W.r_sto; hr.out = ws + W.r_q; hr.out_min = nullptr; hr.M = Mr;
-    MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Mr * 32)), dim3(256), 0, s, hr); MX_COUNT(); MX_MARK("k_head_fwd", s);
-    ActorLossArgs al;
-    memset(&al, 0, sizeof(al));
-    al.B = B; al.T = T; al.N = N; al.K = K; al.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; al.qa = ws + W.r_q; al.dones = b->dones; al.dout = ws + W.r_dout; al.scal = ws + W.scal_a;
-    MX_LAUNCH(k_actor_loss, dim3(1), dim3(256), 0, s, al); MX_COUNT(); MX_MARK("k_actor_loss", s);
-    // back through the (frozen) critic to its action inputs
-    HeadBwdArgs hbr = hb;
-    hbr.h = gr.hall[0]; hbr.sto = ws + W.r_sto; hbr.dout = ws + W.r_dout; hbr.M = Mr; hbr.dh_out = ws + W.r_dh; hbr.gpart = nullptr;
-    MX_LAUNCH(k_head_bwd, dim3(mx_imin_host(mx_num_sms(), mx_ceil_div(Mr, 32))), dim3(256), 0, s, hbr); MX_COUNT(); MX_MARK("k_head_bwd", s);
-    GruBwdArgs gbr;
-    memset(&gbr, 0, sizeof(gbr));
-    gbr.theta = h->th_c; gbr.whh = LC.whh; gbr.hall = gr.hall[0]; gbr.gates = gr.gates; gbr.hn = gr.hn; gbr.dh_out = hbr.dh_out; gbr.dgi = ws + W.r_dgi;
-    gbr.R = Mr; gbr.T = 1; gbr.N = 1; gbr.T1 = 1; gbr.h0 = ws + W.r_h0;
-    if (mx_launch_gru_bwd(gbr, s)) return 1;
-    FrontBwdArgs fbr;
-    memset(&fbr, 0, sizeof(fbr));
-    fbr.X = ws + W.r_x; fbr.ldx = ldc; fbr.M = Mr; fbr.T = 0; fbr.N = 1; fbr.T1 = 1; fbr.h0 = ws + W.r_h0; fbr.feature_norm = c.no_feature_norm ? 0 : 1; fbr.act_tanh = c.use_tanh; fbr.theta = h->th_c; fbr.L = LC;
-    fbr.u1 = fr.u1; fbr.u2 = fr.u2; fbr.st0 = fr.st0; fbr.st1 = fr.st1; fbr.st2 = fr.st2; fbr.dgi = gbr.dgi; fbr.gates = gr.gates; fbr.hall = gr.hall[0];
-    fbr.gpart = ws + W.gpart_c; fbr.P = h->Pc; fbr.dX = ws + W.r_dx; fbr.skip_wgrad = 1;
-    int dummy = 0;
-    if (mx_launch_front_bwd(fbr, &dummy, s)) return 1;
-    MX_LAUNCH(k_scatter_actor_grad, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)(ws + W.r_dx), ldc, B, T, N, S, Ac,
-              (const float*)(c.discrete ? ws + W.a_soft : nullptr), ws + W.a_dout, multi ? c.act_offset : 0, Ac, act_segs(&c));
-    MX_COUNT(); MX_MARK("k_scatter_actor_grad", s);
-    // actor backward + Adam
-    const int ahead_grid = mx_imin_host(mx_num_sms(), mx_ceil_div(Ma, 32));
-    HeadBwdArgs hba;
-    memset(&hba, 0, sizeof(hba));
-    hba.theta = h->th_a; hba.lno_g = LA.lno_g; hba.lno_b = LA.lno_b; hba.w = LA.wq; hba.b = LA.bq; hba.OD = Ac; hba.b_stride = 1; hba.w_stride = MX_H;
-    hba.h = gf.hall[0]; hba.sto = ws + W.a_sto; hba.dout = ws + W.a_dout; hba.M = Ma; hba.dh_out = ws + W.a_dh; hba.gpart = ws + W.gpart_a; hba.P = h->Pa;
-    MX_LAUNCH(k_head_bwd, dim3(ahead_grid), dim3(256), 0, s, hba); MX_COUNT(); MX_MARK("k_head_bwd", s);
-    GruBwdArgs gba;
-    memset(&gba, 0, sizeof(gba));
-    gba.theta = h->th_a; gba.whh = LA.whh; gba.hall = gf.hall[0]; gba.gates = gf.gates; gba.hn = gf.hn; gba.dh_out = hba.dh_out; gba.dgi = ws + W.a_dgi;
-    gba.R = B * N; gba.T = T; gba.N = N; gba.T1 = T + 1;
-    if (mx_launch_gru_bwd(gba, s)) return 1;
-    FrontBwdArgs fba;
-    memset(&fba, 0, sizeof(fba));
-    fba.X = b->obs; fba.ldx = b->obs_ld; fba.M = Ma; fba.T = T; fba.N = N; fba.feature_norm = c.no_feature_norm ? 0 : 1; fba.act_tanh = c.use_tanh; fba.theta = h->th_a; fba.L = LA;
-    fba.u1 = ff.u1; fba.u2 = ff.u2; fba.st0 = ff.st0; fba.st1 = ff.st1; fba.st2 = ff.st2; fba.dgi = gba.dgi; fba.gates = gf.gates; fba.hall = gf.hall[0];
-    fba.gpart = ws + W.gpart_a; fba.P = h->Pa;
-    fba.da2_out = ws + W.tc_da2; fba.da1_out = ws + W.tc_da1; fba.tc_imgT = ws + W.tc_imgT;
-    fba.tc_acc = ws + W.tc_acc; fba.tc_acc_cols = (int)W.tc_acc_cols;
-    int aparts[2] = {0, 0};
-    if (mx_launch_front_bwd(fba, &aparts[0], s)) return 1;
-    if (optimise(h, true, aparts, ahead_grid, s)) return 1;
-  }
+  if (c.discrete && update_actor && !actor_noise_dev) { mx_set_error("maddpg step: discrete actor update needs the Gumbel draws (actor_noise_dev)"); return 1; }
+  const Step st(h, b, (cudaStream_t)stream);
+  if ((c.mlp ? maddpg_step_mlp : maddpg_step_rnn)(st, target_noise_dev, actor_noise_dev, update_actor)) return 1;
   if (update_actor_out) *update_actor_out = update_actor ? 1 : 0;
   if (h->force_update_actor < 0) h->num_updates += 1;      // (graph replays count in mx_graph_launch)
   return 0;
@@ -1118,42 +1117,11 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
   if (!b->obs || !b->acts) { mx_set_error("mx_maddpg_cent_contribute: missing batch field"); return 1; }
   if (c.target_noise > 0.f && !target_noise_dev) { mx_set_error("mx_maddpg_cent_contribute: MATD3 target noise expected"); return 1; }
   cudaStream_t s = (cudaStream_t)stream;
-  float* ws = src->ws;
-  const MxMaddpgWs& W = src->W;
+  if (Step(src, b, s).actor_fwd(TARGET, target_noise_dev)) return 1;
+  // cfg.mlp: k_cent_scatter's row (b*(T+1)+t+1)*N+n with T = 1, t = 0 is the next-observation step the target actor ran on
   const int B = b->B, T = c.episode_len, N = c.n_agents, Ac = c.act_dim;
-  const int Ma = B * (T + 1) * N;
-  const MxNetLayout& LA = src->actor;
-  FrontFwdArgs ff;
-  memset(&ff, 0, sizeof(ff));
-  ff.tc_acc = ws + W.tc_acc; ff.tc_acc_cols = (int)W.tc_acc_cols;
-  ff.X = b->obs; ff.ldx = b->obs_ld; ff.M = Ma; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
-  ff.theta[0] = src->th_a_tgt; ff.L = LA; ff.gi[0] = ws + W.a_gi[1];
-  if (mx_launch_front_fwd(ff, 1, s)) return 1;
-  if (c.mlp) {
-    // maddpg.py:64-74: no recurrence, the head sits in the weight_ih slot (as maddpg_step_mlp phase A).  The noise rows are the
-    // step-1 (next-observation) rows [b][2][N][Ac]; k_cent_scatter's row (b*(T+1)+t+1)*N+n with T = 1, t = 0 is that same step.
-    MX_LAUNCH(k_mlp_head_cols, dim3(launch1d(Ma)), dim3(256), 0, s, (const float*)ff.gi[0], Ma, Ac, c.target_noise > 0.f ? target_noise_dev : nullptr,
-              ws + W.a_nact, nullptr);
-    MX_COUNT(); MX_MARK("k_mlp_head_cols", s);
-  } else {
-    GruFwdArgs gf;
-    memset(&gf, 0, sizeof(gf));
-    gf.theta[0] = src->th_a_tgt; gf.whh = LA.whh; gf.bhh = LA.bhh; gf.gi[0] = ff.gi[0]; gf.hall[0] = ws + W.a_h[1]; gf.R = B * N; gf.T = T; gf.N = N;
-    if (mx_launch_gru_fwd(gf, 1, s)) return 1;
-    HeadArgs ha;
-    memset(&ha, 0, sizeof(ha));
-    ha.lno_g = LA.lno_g; ha.lno_b = LA.lno_b; ha.w = LA.wq; ha.b = LA.bq; ha.OD = Ac; ha.b_stride = 1; ha.w_stride = MX_H; ha.M = Ma;
-    ha.theta = src->th_a_tgt; ha.h = gf.hall[0]; ha.out = ws + W.a_nact; ha.noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
-    MX_LAUNCH(k_head_fwd, dim3(launch1d((long long)Ma * 32)), dim3(256), 0, s, ha); MX_COUNT(); MX_MARK("k_head_fwd", s);
-  }
-  if (c.discrete) {      // one-hot with the next-avail mask (MADDPG) / hard Gumbel-softmax (MATD3)
-    ActXformArgs ax = act_xform_args(&c, Ma, c.target_noise > 0.f ? 1 : 0, b->avail, b->act_ld);
-    ax.logits = ws + W.a_nact; ax.out = ws + W.a_nact;
-    MX_LAUNCH(k_act_transform, dim3(launch1d(Ma)), dim3(256), 0, s, ax); MX_COUNT(); MX_MARK("k_act_transform", s);
-  }
-  MX_LAUNCH(k_cent_scatter, dim3(launch1d((long long)B * T * N * Ac)), dim3(256), 0, s, (const float*)(ws + W.a_nact), b->acts, b->act_ld, B, T, N, Ac,
-            dst->ws + dst->W.cent_acts, dst->ws + dst->W.cent_nacts, mx_round_up(d.cent_act_dim, 4), c.act_offset);
-  MX_COUNT(); MX_MARK("k_cent_scatter", s);
+  MX_RUN(k_cent_scatter, dim3(launch1d((long long)B * T * N * Ac)), dim3(256), s, (const float*)(src->ws + src->W.a.out[1]), b->acts, b->act_ld, B, T,
+         N, Ac, dst->ws + dst->W.cent_acts, dst->ws + dst->W.cent_nacts, mx_round_up(d.cent_act_dim, 4), c.act_offset);
   return MX_CHECK_LAUNCH("cent_contribute");
 }
 
