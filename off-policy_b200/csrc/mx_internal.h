@@ -99,7 +99,7 @@ struct MxQmixWs {           // offsets in floats into the workspace
   int64_t qall[2];          // [net][M][A]  (debug + greedy)
   int64_t greedy;           // int32 [M]
   int64_t q_taken, q_next;  // [B*T][N]
-  int64_t qtot, qtot_next, err, huberp;  // [B*T]
+  int64_t qtot, qtot_next, err;  // [B*T]
   int64_t dq_taken;         // [B*T][N]
   int64_t dh_out;           // [M][H]
   int64_t dgi;              // [M][3H]
@@ -126,6 +126,10 @@ struct MxQmixWs {           // offsets in floats into the workspace
   int64_t total;
 };
 
+// the QMIX step's fork / join points (qmix.cu), one event each: mx_qmix_prefork's fork and its weight images done; the hypernet
+// forward's fork and join; the hypernet backward's fork; the step's final join; the GRU weight gradients' fork
+enum MxQmixEvent { MX_EV_FORK, MX_EV_PREP, MX_EV_BATCH, MX_EV_HYPER, MX_EV_CORE, MX_EV_HBWD, MX_EV_GBWD, MX_EV_COUNT };
+
 struct mx_qmix {
   mx_qmix_cfg cfg;
   MxNetLayout agent;
@@ -144,11 +148,11 @@ struct mx_qmix {
   int p2p_rank = 0, p2p_world = 0;
   float* p2p_blocks[16] = {nullptr};
   uint32_t* p2p_counter = nullptr;
-#if !MX_EMU
   // forked branch for the state-only kernels (weight-image prep, mixer hypernets): one non-blocking stream + fork/join events;
-  // inside a stream capture the same record/wait calls turn into parallel graph branches
+  // inside a stream capture the same record/wait calls turn into parallel graph branches.  The emulator has neither.
   cudaStream_t side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_prep = nullptr, ev_batch = nullptr, ev_hyper = nullptr, ev_core = nullptr, ev_hbwd = nullptr, ev_gbwd = nullptr;
+#if !MX_EMU
+  cudaEvent_t ev[MX_EV_COUNT] = {};
 #endif
   int prep_pending = 0;    // mx_qmix_prefork() already launched the weight-image prep for the coming step
   int imgT_fresh = 0;      // the transposed images (tensor-core backward) were rebuilt with the forward ones for this step

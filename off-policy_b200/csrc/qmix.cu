@@ -143,7 +143,7 @@ static int64_t ws_layout(const mx_qmix_cfg* c, int64_t P, int npart, MxQmixWs* W
   W->gates = tk(M * MX_G); W->hn = tk(M * MX_H);
   W->greedy = tk(M);
   W->q_taken = tk(E * N); W->q_next = tk(E * N);
-  W->qtot = tk(E); W->qtot_next = tk(E); W->err = tk(E); W->huberp = tk(E);
+  W->qtot = tk(E); W->qtot_next = tk(E); W->err = tk(E);
   W->dq_taken = tk(E * N);
   W->dh_out = tk(M * MX_H);
   W->dgi = tk(M * MX_G);
@@ -213,8 +213,7 @@ extern "C" int mx_qmix_create(const mx_qmix_cfg* c, float* theta, float* theta_t
   if (q->wide && !q->split_ok) { mx_set_error("mx_qmix_create: state_dim %d needs the wide-state mixer, which supports mixer_hidden <= 64", c->state_dim); delete q; return 1; }
 #if !MX_EMU
   if (cudaStreamCreateWithFlags(&q->side, cudaStreamNonBlocking) != cudaSuccess) { mx_set_error("mx_qmix_create: cudaStreamCreate failed"); delete q; return 1; }
-  cudaEvent_t* evs[7] = {&q->ev_fork, &q->ev_prep, &q->ev_batch, &q->ev_hyper, &q->ev_core, &q->ev_hbwd, &q->ev_gbwd};
-  for (cudaEvent_t* e : evs) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+  for (cudaEvent_t& e : q->ev) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
 #endif
   *out = q;
   return 0;
@@ -222,8 +221,7 @@ extern "C" int mx_qmix_create(const mx_qmix_cfg* c, float* theta, float* theta_t
 extern "C" void mx_qmix_destroy(mx_qmix* q) {
   if (!q) return;
 #if !MX_EMU
-  cudaEvent_t evs[7] = {q->ev_fork, q->ev_prep, q->ev_batch, q->ev_hyper, q->ev_core, q->ev_hbwd, q->ev_gbwd};
-  for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : q->ev) if (e) cudaEventDestroy(e);
   if (q->side) cudaStreamDestroy(q->side);
 #endif
   delete q;
@@ -316,18 +314,28 @@ static OptimArgs optim_args(mx_qmix* q, int B, const int parts[4], bool after_ex
 
 // ---- forked branch helpers ------------------------------------------------------------------------------------------
 // `side` runs work that does not depend on the agent nets; events order it against the caller's stream.  While the caller's
-// stream is being captured the same calls fork / join the capture, i.e. the graph gets two parallel branches.
+// stream is being captured the same calls fork / join the capture, i.e. the graph gets two parallel branches.  The emulator has
+// no events and no side stream: it runs every launch on the caller's stream, and the event calls do nothing.
 #if !MX_EMU
 static inline bool want_overlap(const mx_qmix* q, int B) {     // the policy decision
   if (!g_mx_overlap || !q->side) return false;
   const long long rows = (long long)B * (q->cfg.episode_len + 1) * q->cfg.n_agents;
   return g_mx_overlap >= 2 || rows <= g_mx_overlap_rows;     // large batches are throughput-bound: a second branch only adds contention
 }
-// per-kernel profiling (mx_profile_begin) times the same kernels back to back on one stream
-static inline bool use_overlap(const mx_qmix* q, int B) { return want_overlap(q, B) && !g_mx_prof_on; }
-static inline void fork_to_side(mx_qmix* q, cudaEvent_t ev, cudaStream_t s) { cudaEventRecord(ev, s); cudaStreamWaitEvent(q->side, ev, 0); }
-static inline void join_from_side(mx_qmix* q, cudaEvent_t ev, cudaStream_t s) { cudaEventRecord(ev, q->side); cudaStreamWaitEvent(s, ev, 0); }
+static inline void ev_record(mx_qmix* q, int e, cudaStream_t s) { cudaEventRecord(q->ev[e], s); }
+static inline void ev_wait(mx_qmix* q, int e, cudaStream_t s) { cudaStreamWaitEvent(s, q->ev[e], 0); }
+static inline void set_pdl_auto(int M) { g_mx_pdl_auto = M <= g_mx_pdl_rows ? 1 : 0; }
+#else
+// as wanted on a device: the policy keeps mixer_split = 1 on the split pipeline, which the emulator then runs serially
+static inline bool want_overlap(const mx_qmix*, int) { return true; }
+static inline void ev_record(mx_qmix*, int, cudaStream_t) {}
+static inline void ev_wait(mx_qmix*, int, cudaStream_t) {}
+static inline void set_pdl_auto(int) {}
 #endif
+// per-kernel profiling (mx_profile_begin) times the same kernels back to back on one stream
+static inline bool use_overlap(const mx_qmix* q, int B) { return q->side && want_overlap(q, B) && !g_mx_prof_on; }
+static inline void fork_to_side(mx_qmix* q, int e, cudaStream_t s) { ev_record(q, e, s); ev_wait(q, e, q->side); }
+static inline void join_from_side(mx_qmix* q, int e, cudaStream_t s) { ev_record(q, e, q->side); ev_wait(q, e, s); }
 
 static int launch_prep(mx_qmix* q, cudaStream_t s) {
   const float* const th2[2] = {q->theta, q->theta_tgt};
@@ -344,221 +352,210 @@ static int launch_prep(mx_qmix* q, cudaStream_t s) {
 // Parameter-only work of the coming step (TF32 hi/lo weight images of the front layers), started on the side branch so that it
 // overlaps the index draw and the gather.  Optional: mx_qmix_backward_only does it itself when this was not called.
 int mx_qmix_prefork(mx_qmix* q, int B, void* stream) {
-#if !MX_EMU
   if (!use_overlap(q, B) || !mx_front_tc_usable(q->agent.in_dim, true) || q->prep_pending) return 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  fork_to_side(q, q->ev_fork, s);
+  fork_to_side(q, MX_EV_FORK, (cudaStream_t)stream);
   if (launch_prep(q, q->side)) return 1;
-  cudaEventRecord(q->ev_prep, q->side);
+  ev_record(q, MX_EV_PREP, q->side);
   q->prep_pending = 1;
-#else
-  (void)q; (void)B; (void)stream;
-#endif
   return 0;
 }
+
+// ---- the launches of one step: the schedule is decided once, each builder fills its arguments from the learner and the batch, and
+// backward_core below lists the phases
+namespace {
+struct Step {
+  mx_qmix* q;
+  const mx_batch* b;
+  cudaStream_t s, side;       // the caller's stream; the side branch, or s when the step runs serially
+  const mx_qmix_cfg& c;
+  const MxQmixWs& W;
+  float* ws;
+  int B, T, N, M, ld_tn, ld_t;      // ld_tn, ld_t: episode strides of the batch's [B][T][N] and [B][T] fields
+  const float* X; int ldx;    // agent-net input rows: the observations, or [obs | previous action] packed by pack_input (prev_act_inp)
+  bool overlap, wanted;       // the side branch runs beside the agent nets; the policy's wish (profiling turns overlap off)
+  bool split;                 // the mixer as hypernet forward / core / hypernet backward, not the fused k_mixer
+  bool mid;                   // the core is k_mid: the Q head, the mixer core and the Q head's backward in one launch
+  bool gsplit;                // the GRU weight gradients as their own kernel (k_gru_wgrad), beside k_front_bwd when forked
+  int parts[4] = {0, 0, 0, 0};      // gradient partials of front_bwd, the Q head, the mixer; scalar partials
+  MixerArgs mx{};
+  FrontFwdArgs ff{};
+  MidArgs md{};
+  FrontBwdArgs fb{};
+
+  Step(mx_qmix* q_, const mx_batch* b_, cudaStream_t s_) : q(q_), b(b_), s(s_), c(q_->cfg), W(q_->W), ws(q_->ws) {
+    B = b->B; T = c.episode_len; N = c.n_agents; M = B * (T + 1) * N;
+    ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : T;
+    X = c.prev_act_inp ? ws + W.xin : b->obs;
+    ldx = c.prev_act_inp ? mx_round_up(c.obs_dim + c.act_dim, 4) : b->obs_ld;
+
+    mx.theta = q->theta; mx.theta_tgt = q->theta_tgt; mx.L = q->mix; mx.vdn = c.vdn;
+    mx.share = b->share; mx.share_ld = b->share_ld;
+    mx.q_taken = ws + W.q_taken; mx.q_next = ws + W.q_next;
+    mx.rewards = b->rewards; mx.dones_env = b->dones_env; mx.weights = c.use_per ? b->weights : nullptr;
+    mx.ld_tn = ld_tn; mx.ld_t = ld_t;
+    mx.B = B; mx.T = T; mx.N = N; mx.gamma = c.gamma; mx.huber_delta = c.huber_delta; mx.use_huber = c.use_huber;
+    mx.qtot = ws + W.qtot; mx.qtot_next = ws + W.qtot_next; mx.err = ws + W.err; mx.dq_taken = ws + W.dq_taken;
+    mx.gpart = ws + W.gpart; mx.P = q->P; mx.spart = ws + W.spart;
+    mx.hyp_h1 = ws + W.hyp_h1; mx.hyp_h2 = ws + W.hyp_h2; mx.hyp_hb = ws + W.hyp_hb;
+    for (int k = 0; k < 2; ++k) { mx.hyp_p1[k] = ws + W.hyp_p1[k]; mx.hyp_b1[k] = ws + W.hyp_b1[k]; mx.hyp_p2[k] = ws + W.hyp_p2[k]; mx.hyp_b2[k] = ws + W.hyp_b2[k]; }
+    mx.d_q = ws + W.d_q; mx.d_hp = ws + W.d_hp; mx.d_p2 = ws + W.d_p2; mx.d_p1 = ws + W.d_p1;
+    mx.gH = mx_round_up(c.hyper_hidden, 4); mx.gM = mx_round_up(c.mixer_hidden, 4); mx.gP = mx_round_up(c.n_agents * c.mixer_hidden, 4);
+    mx.wide = q->wide; mx.wl = q->wl;
+    if (q->wide) { mx.wimg = ws + W.wimg; mx.pre = ws + W.pre; mx.d_pre = ws + W.d_pre; }
+
+    ff.X = X; ff.ldx = ldx; ff.M = M; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
+    ff.theta[0] = q->theta; ff.theta[1] = q->theta_tgt; ff.L = q->agent;
+    ff.gi[0] = ws + W.gi[0]; ff.gi[1] = ws + W.gi[1];
+    ff.u1 = ws + W.u1; ff.u2 = ws + W.u2; ff.st0 = ws + W.st0; ff.st1 = ws + W.st1; ff.st2 = ws + W.st2;
+    if (mx_front_tc_usable(q->agent.in_dim, true)) {     // the TF32 hi/lo weight images, rebuilt by weight_images()
+      ff.tc_img[0] = ws + W.tcimg[0]; ff.tc_img[1] = ws + W.tcimg[1];
+      ff.tc_acc = ws + W.tcacc; ff.tc_acc_cols = (int)W.tcacc_cols;
+    }
+
+    md.mix = mx;
+    head<true, true>(md);
+    // the live net's backward through its front layers from the "gi" gradient rows, and through the GRU weights unless cfg.mlp
+    fb.X = X; fb.ldx = ldx; fb.M = M; fb.T = T; fb.N = N; fb.feature_norm = c.no_feature_norm ? 0 : 1; fb.act_tanh = c.use_tanh;
+    fb.theta = q->theta; fb.L = q->agent; fb.u1 = ff.u1; fb.u2 = ff.u2; fb.st0 = ff.st0; fb.st1 = ff.st1; fb.st2 = ff.st2;
+    fb.dgi = ws + W.dgi; fb.gpart = mx.gpart; fb.P = q->P;
+    if (c.mlp) fb.no_gru = 1;
+    else { fb.gates = ws + W.gates; fb.hall = ws + W.hall[0]; }
+    fb.ln_part = ws + W.lnpart; fb.ln_part_rows = 2 * q->npart;
+    fb.da2_out = ws + W.da2; fb.da1_out = ws + W.da1; fb.tc_imgT = ws + W.tcimgT;
+    fb.tc_acc = ws + W.tcacc; fb.tc_acc_cols = (int)W.tcacc_cols;
+
+    overlap = use_overlap(q, B); wanted = want_overlap(q, B);
+    side = overlap ? q->side : s;
+    // the split mixer only pays off when its hypernet kernels run beside the agent nets (serial, the fused k_mixer moves less data)
+    split = q->wide || (q->split_ok && (g_mx_mixer_split >= 2 || (g_mx_mixer_split == 1 && wanted)));
+    // the debug mode of the parity tests keeps the separate kernels because it materialises every per-action Q value
+    mid = !c.mlp && split && g_mx_mid_fused && !q->debug && mx_mid_supported(md);
+    gsplit = mx_gru_wgrad_split_usable(fb);      // never with cfg.mlp (no_gru)
+  }
+
+  void fork(int e) { if (overlap) fork_to_side(q, e, s); }
+  void join(int e) { if (overlap) join_from_side(q, e, s); }
+
+  // the Q values a forward selects and, in debug mode, every per-action value and the greedy action (k_qhead, k_mlp_qselect)
+  template <class Args> void q_outputs(Args& a) const {
+    a.q_taken = ws + W.q_taken; a.q_next = ws + W.q_next;
+    a.greedy = q->debug ? reinterpret_cast<int32_t*>(ws + W.greedy) : nullptr;
+    a.qall0 = q->debug ? ws + W.qall[0] : nullptr; a.qall1 = q->debug ? ws + W.qall[1] : nullptr;
+  }
+  // the Q head (post-GRU LayerNorm + Linear) and the rows it reads: k_qhead, k_mid, k_qhead_bwd.  FWD: the forward over both nets;
+  // GRAD: the backward into dh_out and the head's gradient partials
+  template <bool FWD, bool GRAD, class Args> void head(Args& a) const {
+    a.wq = q->agent.wq; a.bq = q->agent.bq; a.lno_g = q->agent.lno_g; a.lno_b = q->agent.lno_b;
+    a.act_idx = b->act_idx; a.T = T; a.N = N; a.A = c.act_dim; a.ld_tn = ld_tn;
+    if constexpr (FWD) { a.hall[0] = ws + W.hall[0]; a.hall[1] = ws + W.hall[1]; a.avail = b->avail; a.act_ld = b->act_ld; a.double_q = c.double_q; }
+    if constexpr (GRAD) { a.dh_out = ws + W.dh_out; a.gpart = mx.gpart; a.P = q->P; }
+  }
+
+  // ---- the phases ----
+  int pack_input() const {    // prev_act_inp: network input = [obs | previous action], packed once per step into the workspace
+    if (!c.prev_act_inp) return 0;
+    if (!b->acts) { mx_set_error("qmix step: prev_act_inp needs the batch's one-hot actions"); return 1; }
+    return mx_launch_pack_prev_act(b->obs, b->obs_ld, b->acts, b->act_ld, ws + W.xin, ldx, B, T, N, c.obs_dim, c.act_dim, s);
+  }
+
+  // weights changed in the last Adam / Polyak: rebuild the TF32 hi/lo images (18k elements per net), unless mx_qmix_prefork()
+  // launched it on the side branch before the batch was sampled
+  int weight_images() const {
+    if (!ff.tc_img[0]) return 0;
+    if (!q->prep_pending) return launch_prep(q, s);
+    ev_wait(q, MX_EV_PREP, s); q->prep_pending = 0;
+    return 0;
+  }
+
+  // the mixer's hypernetworks depend on the sampled states and the parameters only: forked branch beside the agent nets, before the
+  // front kernel (forked after it, beside the recurrence, the hypernet CTAs cost more)
+  int hyper_fwd_forked() {
+    if (!(split && overlap)) return 0;
+    fork(MX_EV_BATCH);
+    return mx_launch_mix_hyper_fwd(mx, side);
+  }
+
+  // the mixer between the agents' Q values and their gradient.  Split: the hypernet forward (here, unless it was forked), the core
+  // -- k_mid, or k_mix_core between k_qhead and k_qhead_bwd -- then the hypernet backward, beside the agent-net backward when forked.
+  // Otherwise the fused k_mixer.
+  int mixer() {
+    if (!split) { const int rc = mx_launch_mixer(mx, &parts[2], s); parts[3] = parts[2]; return rc; }
+    if (!overlap && mx_launch_mix_hyper_fwd(mx, s)) return 1;
+    join(MX_EV_HYPER);
+    if (mid ? mx_launch_mid(md, &parts[1], s) : mx_launch_mix_core(mx, &parts[3], s)) return 1;
+    if (mid) parts[3] = parts[1];
+    fork(MX_EV_CORE);
+    return mx_launch_mix_hyper_bwd(mx, &parts[2], side);
+  }
+  int mlp_qselect() const {
+    MlpQSelArgs a{};
+    a.gi[0] = ff.gi[0]; a.gi[1] = ff.gi[1]; a.act_idx = b->act_idx; a.avail = b->avail; a.act_ld = b->act_ld; a.ld_tn = ld_tn;
+    a.B = B; a.N = N; a.A = c.act_dim; a.double_q = c.double_q;
+    q_outputs(a);
+    return mx_launch_mlp_qselect(a, s);
+  }
+  int gru_fwd() const {
+    GruFwdArgs a{};
+    a.theta[0] = q->theta; a.theta[1] = q->theta_tgt; a.whh = q->agent.whh; a.bhh = q->agent.bhh;
+    a.gi[0] = ff.gi[0]; a.gi[1] = ff.gi[1]; a.hall[0] = ws + W.hall[0]; a.hall[1] = ws + W.hall[1];
+    a.gates = ws + W.gates; a.hn = ws + W.hn; a.R = B * N; a.T = T; a.N = N;
+    return mx_launch_gru_fwd(a, 2, s);
+  }
+  int qhead() const {
+    QHeadArgs a{};
+    head<true, false>(a);
+    q_outputs(a);
+    a.theta[0] = q->theta; a.theta[1] = q->theta_tgt; a.sto = ws + W.sto; a.M = M;
+    return mx_launch_qhead(a, s);
+  }
+  int qhead_bwd() {
+    QHeadBwdArgs a{};
+    head<false, true>(a);
+    a.theta = q->theta; a.hall = ws + W.hall[0]; a.sto = ws + W.sto; a.dq_taken = mx.dq_taken; a.M = M;
+    return mx_launch_qhead_bwd(a, &parts[1], s);
+  }
+  int gru_bwd() const {
+    GruBwdArgs a{};
+    a.theta = q->theta; a.whh = q->agent.whh; a.hall = ws + W.hall[0]; a.gates = ws + W.gates; a.hn = ws + W.hn; a.dh_out = ws + W.dh_out;
+    a.dgi = ws + W.dgi; a.R = B * N; a.T = T; a.N = N;
+    return mx_launch_gru_bwd(a, s);
+  }
+
+  // k_gru_wgrad on the side branch (gsplit), k_front_bwd, then the one join of everything the side branch still runs
+  int front_bwd() {
+    fb.tc_imgT_ready = q->imgT_fresh; q->imgT_fresh = 0;
+    if (gsplit) { fb.gru_wgrad_ext = 1; fork(MX_EV_GBWD); if (mx_launch_gru_wgrad(fb, side)) return 1; }
+    if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
+    if (split || gsplit) join(MX_EV_HBWD);
+    return 0;
+  }
+};
+}  // namespace
 
 // everything of the step up to (not including) the optimiser: forward, loss, backward; leaves the per-CTA gradient partials and
 // fills `*oa` with the optimiser's arguments
 static int backward_core(mx_qmix* q, const mx_batch* b, void* stream, OptimArgs* oa) {
   if (check_batch(q, b)) return 1;
-  const mx_qmix_cfg& c = q->cfg;
-  cudaStream_t s = (cudaStream_t)stream;
-  float* ws = q->ws;
-  const MxQmixWs& W = q->W;
-  const int B = b->B, T = c.episode_len, N = c.n_agents;
-  const int M = B * (T + 1) * N;
-#if !MX_EMU
-  g_mx_pdl_auto = M <= g_mx_pdl_rows ? 1 : 0;      // programmatic dependent launches for this step's kernels (and the sample that follows it)
-  const bool overlap = use_overlap(q, B), wanted = want_overlap(q, B);
-  cudaStream_t side = overlap ? q->side : s;
-#else
-  const bool overlap = false, wanted = true;
-  cudaStream_t side = s;
-#endif
-  // the split mixer only pays off when its hypernet kernels run beside the agent nets (serial, the fused k_mixer moves less data)
-  const bool split = q->wide || (q->split_ok && (g_mx_mixer_split >= 2 || (g_mx_mixer_split == 1 && wanted)));
+  Step st(q, b, (cudaStream_t)stream);
+  set_pdl_auto(st.M);      // programmatic dependent launches for this step's kernels (and the sample that follows it)
 
-  MixerArgs mx;
-  memset(&mx, 0, sizeof(mx));
-  mx.theta = q->theta; mx.theta_tgt = q->theta_tgt; mx.L = q->mix; mx.vdn = c.vdn;
-  mx.share = b->share; mx.share_ld = b->share_ld;
-  mx.q_taken = ws + W.q_taken; mx.q_next = ws + W.q_next;
-  mx.rewards = b->rewards; mx.dones_env = b->dones_env; mx.weights = c.use_per ? b->weights : nullptr;
-  const int ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N, ld_t = b->ep_t_ld > 0 ? b->ep_t_ld : T;
-  mx.ld_tn = ld_tn; mx.ld_t = ld_t;
-  mx.B = B; mx.T = T; mx.N = N; mx.gamma = c.gamma; mx.huber_delta = c.huber_delta; mx.use_huber = c.use_huber;
-  mx.qtot = ws + W.qtot; mx.qtot_next = ws + W.qtot_next; mx.err = ws + W.err; mx.dq_taken = ws + W.dq_taken;
-  mx.gpart = ws + W.gpart; mx.P = q->P; mx.spart = ws + W.spart;
-  mx.hyp_h1 = ws + W.hyp_h1; mx.hyp_h2 = ws + W.hyp_h2; mx.hyp_hb = ws + W.hyp_hb;
-  for (int k = 0; k < 2; ++k) { mx.hyp_p1[k] = ws + W.hyp_p1[k]; mx.hyp_b1[k] = ws + W.hyp_b1[k]; mx.hyp_p2[k] = ws + W.hyp_p2[k]; mx.hyp_b2[k] = ws + W.hyp_b2[k]; }
-  mx.d_q = ws + W.d_q; mx.d_hp = ws + W.d_hp; mx.d_p2 = ws + W.d_p2; mx.d_p1 = ws + W.d_p1;
-  mx.gH = mx_round_up(c.hyper_hidden, 4); mx.gM = mx_round_up(c.mixer_hidden, 4); mx.gP = mx_round_up(c.n_agents * c.mixer_hidden, 4);
-  mx.wide = q->wide; mx.wl = q->wl;
-  if (q->wide) { mx.wimg = ws + W.wimg; mx.pre = ws + W.pre; mx.d_pre = ws + W.d_pre; }
-
-  const float* X = b->obs;
-  int ldx = b->obs_ld;
-  if (c.prev_act_inp) {       // network input = [obs | previous action]: packed once per step into the workspace
-    if (!b->acts) { mx_set_error("qmix step: prev_act_inp needs the batch's one-hot actions"); return 1; }
-    ldx = mx_round_up(c.obs_dim + c.act_dim, 4);
-    if (mx_launch_pack_prev_act(b->obs, b->obs_ld, b->acts, b->act_ld, ws + W.xin, ldx, B, T, N, c.obs_dim, c.act_dim, s)) return 1;
-    X = ws + W.xin;
-  }
-  FrontFwdArgs ff;
-  memset(&ff, 0, sizeof(ff));
-  ff.X = X; ff.ldx = ldx; ff.M = M; ff.feature_norm = c.no_feature_norm ? 0 : 1; ff.act_tanh = c.use_tanh;
-  ff.theta[0] = q->theta; ff.theta[1] = q->theta_tgt; ff.L = q->agent;
-  ff.gi[0] = ws + W.gi[0]; ff.gi[1] = ws + W.gi[1];
-  ff.u1 = ws + W.u1; ff.u2 = ws + W.u2; ff.st0 = ws + W.st0; ff.st1 = ws + W.st1; ff.st2 = ws + W.st2;
-  if (mx_front_tc_usable(q->agent.in_dim, true)) {       // weights changed in the last Adam / Polyak: rebuild the TF32 hi/lo images (18k elements per net)
-    if (q->prep_pending) {                      // mx_qmix_prefork() launched it on the side branch before the batch was sampled
-#if !MX_EMU
-      cudaStreamWaitEvent(s, q->ev_prep, 0);
-#endif
-      q->prep_pending = 0;
-    } else if (launch_prep(q, s)) return 1;
-    ff.tc_img[0] = ws + W.tcimg[0]; ff.tc_img[1] = ws + W.tcimg[1];
-    ff.tc_acc = ws + W.tcacc; ff.tc_acc_cols = (int)W.tcacc_cols;
-  }
-  // the mixer's hypernetworks depend on the sampled states and the parameters only: forked branch beside the agent nets, before the
-  // front kernel (forked after it, beside the recurrence, the hypernet CTAs cost more)
-#if !MX_EMU
-  if (split && overlap) fork_to_side(q, q->ev_batch, s);
-#endif
-  if (split && overlap) { if (mx_launch_mix_hyper_fwd(mx, side)) return 1; }
-  if (mx_launch_front_fwd(ff, 2, s)) return 1;
-
-  if (c.mlp) {      // ---- transition-level variant (M_QMix / M_VDN): no recurrence, Q = columns [0, A) of the "gi" rows ----
-    int parts[4] = {0, 0, 0, 0};
-    MlpQSelArgs qs;
-    memset(&qs, 0, sizeof(qs));
-    qs.gi[0] = ff.gi[0]; qs.gi[1] = ff.gi[1]; qs.act_idx = b->act_idx; qs.avail = b->avail; qs.act_ld = b->act_ld; qs.ld_tn = ld_tn;
-    qs.B = B; qs.N = N; qs.A = c.act_dim; qs.double_q = c.double_q; qs.q_taken = ws + W.q_taken; qs.q_next = ws + W.q_next;
-    qs.qall0 = q->debug ? ws + W.qall[0] : nullptr; qs.qall1 = q->debug ? ws + W.qall[1] : nullptr;
-    qs.greedy = q->debug ? reinterpret_cast<int32_t*>(ws + W.greedy) : nullptr;
-    if (mx_launch_mlp_qselect(qs, s)) return 1;
-    if (split) {
-      if (!overlap) { if (mx_launch_mix_hyper_fwd(mx, s)) return 1; }
-#if !MX_EMU
-      else join_from_side(q, q->ev_hyper, s);
-#endif
-      if (mx_launch_mix_core(mx, &parts[3], s)) return 1;
-#if !MX_EMU
-      if (overlap) fork_to_side(q, q->ev_core, s);
-#endif
-      if (mx_launch_mix_hyper_bwd(mx, &parts[2], side)) return 1;
-    } else {
-      if (mx_launch_mixer(mx, &parts[2], s)) return 1;
-      parts[3] = parts[2];
-    }
-    if (mx_launch_mlp_dgi(mx.dq_taken, b->act_idx, ld_tn, ws + W.dgi, B, N, s)) return 1;
-    FrontBwdArgs fbm;
-    memset(&fbm, 0, sizeof(fbm));
-    fbm.X = X; fbm.ldx = ldx; fbm.M = M; fbm.T = T; fbm.N = N; fbm.feature_norm = c.no_feature_norm ? 0 : 1; fbm.act_tanh = c.use_tanh; fbm.no_gru = 1;
-    fbm.theta = q->theta; fbm.L = q->agent; fbm.u1 = ff.u1; fbm.u2 = ff.u2; fbm.st0 = ff.st0; fbm.st1 = ff.st1; fbm.st2 = ff.st2;
-    fbm.dgi = ws + W.dgi; fbm.gpart = mx.gpart; fbm.P = q->P;
-    fbm.ln_part = ws + W.lnpart; fbm.ln_part_rows = 2 * q->npart;
-    fbm.da2_out = ws + W.da2; fbm.da1_out = ws + W.da1; fbm.tc_imgT = ws + W.tcimgT; fbm.tc_imgT_ready = q->imgT_fresh; q->imgT_fresh = 0;      // (option wgrad_tc)
-    fbm.tc_acc = ws + W.tcacc; fbm.tc_acc_cols = (int)W.tcacc_cols;
-    if (mx_launch_front_bwd(fbm, &parts[0], s)) return 1;
-#if !MX_EMU
-    if (split && overlap) join_from_side(q, q->ev_hbwd, s);
-#endif
-    *oa = optim_args(q, B, parts);
-    return 0;
-  }
-
-  GruFwdArgs gf;
-  memset(&gf, 0, sizeof(gf));
-  gf.theta[0] = q->theta; gf.theta[1] = q->theta_tgt; gf.whh = q->agent.whh; gf.bhh = q->agent.bhh;
-  gf.gi[0] = ff.gi[0]; gf.gi[1] = ff.gi[1]; gf.hall[0] = ws + W.hall[0]; gf.hall[1] = ws + W.hall[1];
-  gf.gates = ws + W.gates; gf.hn = ws + W.hn; gf.R = B * N; gf.T = T; gf.N = N;
-  if (mx_launch_gru_fwd(gf, 2, s)) return 1;
-
-  QHeadArgs qh;
-  memset(&qh, 0, sizeof(qh));
-  qh.theta[0] = q->theta; qh.theta[1] = q->theta_tgt;
-  qh.wq = q->agent.wq; qh.bq = q->agent.bq; qh.lno_g = q->agent.lno_g; qh.lno_b = q->agent.lno_b;
-  qh.hall[0] = gf.hall[0]; qh.hall[1] = gf.hall[1]; qh.sto = ws + W.sto;
-  qh.act_idx = b->act_idx; qh.avail = b->avail; qh.act_ld = b->act_ld;
-  qh.M = M; qh.T = T; qh.N = N; qh.A = c.act_dim; qh.double_q = c.double_q; qh.ld_tn = ld_tn;
-  qh.q_taken = ws + W.q_taken; qh.q_next = ws + W.q_next;
-  qh.greedy = q->debug ? reinterpret_cast<int32_t*>(ws + W.greedy) : nullptr;
-  qh.qall0 = q->debug ? ws + W.qall[0] : nullptr; qh.qall1 = q->debug ? ws + W.qall[1] : nullptr;
-
-  int parts[4] = {0, 0, 0, 0};
-  MidArgs md;
-  memset(&md, 0, sizeof(md));
-  md.mix = mx;
-  md.wq = qh.wq; md.bq = qh.bq; md.lno_g = qh.lno_g; md.lno_b = qh.lno_b; md.hall[0] = qh.hall[0]; md.hall[1] = qh.hall[1];
-  md.act_idx = qh.act_idx; md.avail = qh.avail; md.act_ld = qh.act_ld; md.T = T; md.N = N; md.A = c.act_dim; md.double_q = c.double_q; md.ld_tn = ld_tn;
-  md.dh_out = ws + W.dh_out; md.gpart = mx.gpart; md.P = q->P;
-  // the three latency-bound launches between the recurrences (Q head, mixer core, Q head backward) as one kernel; the debug mode
-  // of the parity tests keeps the separate kernels because it materialises every per-action Q value
-  const bool mid = split && g_mx_mid_fused && !q->debug && mx_mid_supported(md);
-  if (mid) {
-    if (!overlap) { if (mx_launch_mix_hyper_fwd(mx, s)) return 1; }
-#if !MX_EMU
-    else join_from_side(q, q->ev_hyper, s);
-#endif
-    if (mx_launch_mid(md, &parts[1], s)) return 1;
-    parts[3] = parts[1];
-#if !MX_EMU
-    if (overlap) fork_to_side(q, q->ev_core, s);
-#endif
-    if (mx_launch_mix_hyper_bwd(mx, &parts[2], side)) return 1;
+  if (st.pack_input()) return 1;
+  if (st.weight_images()) return 1;
+  if (st.hyper_fwd_forked()) return 1;
+  if (mx_launch_front_fwd(st.ff, 2, st.s)) return 1;
+  if (q->cfg.mlp) {      // transition-level variant (M_QMix / M_VDN): no recurrence, Q = columns [0, A) of the "gi" rows
+    if (st.mlp_qselect()) return 1;
+    if (st.mixer()) return 1;
+    if (mx_launch_mlp_dgi(st.mx.dq_taken, b->act_idx, st.ld_tn, st.ws + st.W.dgi, st.B, st.N, st.s)) return 1;
   } else {
-    if (mx_launch_qhead(qh, s)) return 1;
-    if (split) {
-      if (!overlap) { if (mx_launch_mix_hyper_fwd(mx, s)) return 1; }
-#if !MX_EMU
-      else join_from_side(q, q->ev_hyper, s);
-#endif
-      if (mx_launch_mix_core(mx, &parts[3], s)) return 1;
-#if !MX_EMU
-      if (overlap) fork_to_side(q, q->ev_core, s);
-#endif
-      if (mx_launch_mix_hyper_bwd(mx, &parts[2], side)) return 1;      // beside k_qhead_bwd / k_gru_bwd / k_front_bwd when forked
-    } else {
-      if (mx_launch_mixer(mx, &parts[2], s)) return 1;
-      parts[3] = parts[2];
-    }
-    QHeadBwdArgs hb;
-    memset(&hb, 0, sizeof(hb));
-    hb.theta = q->theta; hb.wq = q->agent.wq; hb.bq = q->agent.bq; hb.lno_g = q->agent.lno_g; hb.lno_b = q->agent.lno_b;
-    hb.hall = gf.hall[0]; hb.sto = qh.sto; hb.act_idx = b->act_idx; hb.dq_taken = mx.dq_taken;
-    hb.M = M; hb.T = T; hb.N = N; hb.A = c.act_dim; hb.ld_tn = ld_tn; hb.dh_out = ws + W.dh_out; hb.gpart = mx.gpart; hb.P = q->P;
-    if (mx_launch_qhead_bwd(hb, &parts[1], s)) return 1;
+    if (st.gru_fwd()) return 1;
+    if (!st.mid && st.qhead()) return 1;      // k_mid runs the Q head and its backward around the mixer core
+    if (st.mixer()) return 1;
+    if (!st.mid && st.qhead_bwd()) return 1;
+    if (st.gru_bwd()) return 1;
   }
-
-  GruBwdArgs gb;
-  memset(&gb, 0, sizeof(gb));
-  gb.theta = q->theta; gb.whh = q->agent.whh; gb.hall = gf.hall[0]; gb.gates = gf.gates; gb.hn = gf.hn; gb.dh_out = ws + W.dh_out;
-  gb.dgi = ws + W.dgi; gb.R = B * N; gb.T = T; gb.N = N;
-  if (mx_launch_gru_bwd(gb, s)) return 1;
-
-  FrontBwdArgs fb;
-  memset(&fb, 0, sizeof(fb));
-  fb.X = X; fb.ldx = ldx; fb.M = M; fb.T = T; fb.N = N; fb.feature_norm = c.no_feature_norm ? 0 : 1; fb.act_tanh = c.use_tanh;
-  fb.theta = q->theta; fb.L = q->agent; fb.u1 = ff.u1; fb.u2 = ff.u2; fb.st0 = ff.st0; fb.st1 = ff.st1; fb.st2 = ff.st2;
-  fb.dgi = gb.dgi; fb.gates = gf.gates; fb.hall = gf.hall[0]; fb.gpart = mx.gpart; fb.P = q->P;
-  fb.ln_part = ws + W.lnpart; fb.ln_part_rows = 2 * q->npart;
-  fb.da2_out = ws + W.da2; fb.da1_out = ws + W.da1; fb.tc_imgT = ws + W.tcimgT; fb.tc_imgT_ready = q->imgT_fresh; q->imgT_fresh = 0;      // used when the tensor-core weight-gradient kernel is enabled (option wgrad_tc)
-  fb.tc_acc = ws + W.tcacc; fb.tc_acc_cols = (int)W.tcacc_cols;
-  const bool gsplit = mx_gru_wgrad_split_usable(fb);      // GRU weight gradients as their own kernel, beside k_front_bwd when forked
-  if (gsplit) {
-    fb.gru_wgrad_ext = 1;
-#if !MX_EMU
-    if (overlap) fork_to_side(q, q->ev_gbwd, s);
-#endif
-    if (mx_launch_gru_wgrad(fb, side)) return 1;
-  }
-  if (mx_launch_front_bwd(fb, &parts[0], s)) return 1;
-
-#if !MX_EMU
-  if ((split || gsplit) && overlap) join_from_side(q, q->ev_hbwd, s);
-#endif
-  *oa = optim_args(q, B, parts);
+  if (st.front_bwd()) return 1;
+  *oa = optim_args(q, st.B, st.parts);
   return 0;
 }
 
