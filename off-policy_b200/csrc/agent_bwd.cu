@@ -876,6 +876,13 @@ static int front_bwd_pick_rm(int M, int in_dim, int sms, bool gru_ext) {
   return best;
 }
 
+// The 32-row tile (RM 2, front_bwd_pick_rm's fallback) must fit; its input tiles are round_up(in_dim, 64) wide.
+int mx_front_bwd_max_in_dim(bool gru_ext) {
+  int w = 0;
+  while ((size_t)front_bwd_smem(w + 64, 32, gru_ext).total * sizeof(float) + 16 <= 227 * 1024) w += 64;
+  return w;
+}
+
 template <int RM>
 static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s) {
   const int TM = 16 * RM;

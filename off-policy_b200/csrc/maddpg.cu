@@ -507,6 +507,15 @@ static int maddpg_check(const mx_maddpg_cfg* c) {
   if (c->mlp && c->episode_len != 1) {
     mx_set_error("mx_maddpg: the MLP (transition-level) variant takes transitions as episodes of length 1"); return 1;
   }
+  {     // every net's backward (and the critic's data gradient) runs k_front_bwd without k_gru_wgrad beside it
+    const int lim = mx_front_bwd_max_in_dim(false);
+    if (c->obs_dim > lim) { mx_set_error("mx_maddpg: actor input width %d (obs_dim) exceeds %d, the widest k_front_bwd's shared memory holds", c->obs_dim, lim); return 1; }
+    if (critic_in_dim(c) > lim) {
+      mx_set_error("mx_maddpg: critic input width %d (state_dim %d + %d action columns) exceeds %d, the widest k_front_bwd's shared memory holds",
+                   critic_in_dim(c), c->state_dim, cent_act_width(c), lim);
+      return 1;
+    }
+  }
   return 0;
 }
 

@@ -199,6 +199,9 @@ int mx_launch_tc_prep_weights_T(const float* theta, const MxNetLayout& L, float*
 bool mx_tc_prep_T_wanted(int in_dim);
 size_t mx_tc_imageT_floats(int in_dim);
 int mx_launch_front_bwd(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s);
+// the widest agent-net input k_front_bwd's shared memory holds (gru_ext: with k_gru_wgrad beside it, as in the recurrent QMIX step);
+// the learners refuse wider inputs at creation
+int mx_front_bwd_max_in_dim(bool gru_ext);
 int mx_launch_wgrad_tc(const FrontBwdArgs& a, int nparts, cudaStream_t s);
 bool mx_wgrad_tc_usable(const FrontBwdArgs& a);
 

@@ -59,6 +59,14 @@ static int check_cfg(const mx_qmix_cfg* c) {
   if (!c->vdn && c->hyper_layers != 1 && c->hyper_layers != 2) { mx_set_error("hypernet_layers must be 1 or 2"); return 1; }
   if (c->mlp && c->episode_len != 1) { mx_set_error("mx_qmix: the MLP (transition-level) variant stores transitions as episodes of length 1"); return 1; }
   if (c->mlp && c->prev_act_inp) { mx_set_error("mx_qmix: prev_act_inp is a recurrent-policy option"); return 1; }
+  {     // the recurrent step runs k_gru_wgrad beside k_front_bwd above 128 input columns; the MLP variant has no GRU
+    const int in_dim = c->obs_dim + (c->prev_act_inp ? c->act_dim : 0), lim = mx_front_bwd_max_in_dim(!c->mlp);
+    if (in_dim > lim) {
+      mx_set_error("mx_qmix: agent input width %d (obs_dim %d%s) exceeds %d, the widest k_front_bwd's shared memory holds", in_dim, c->obs_dim,
+                   c->prev_act_inp ? " + act_dim with prev_act_inp" : "", lim);
+      return 1;
+    }
+  }
   return 0;
 }
 

@@ -9,6 +9,9 @@ ReLU layers forced to the ENGINE's (u > 0 of the activations the engine saved), 
 from the kink they were.  The caller then demands (a) every flipped unit had |pre-activation| below `KINK_TOL` in the oracle and
 (b) the 1e-4 comparison passes against the re-run.  A real kernel error cannot pass: it either flips no unit or flips units far
 from zero, or still disagrees afterwards.
+
+The QMIX mixer's |hyper_w1(s)| and |hyper_w2(s)| have the same kind of kink at zero: `resolve_abs_kinks` settles the hypernet outputs
+within `ABS_KINK_TOL` of zero in the float64 reference of a whole-batch gradient comparison.
 """
 import copy
 
@@ -81,3 +84,60 @@ def snapshot(L):
 def adopt(L, L2):
     """Continue the lock-step run from the re-run's state."""
     L.__dict__.update(L2.__dict__)
+
+
+ABS_KINK_TOL = 1e-6
+
+
+def resolve_abs_kinks(L64, batch, gv, g64):
+    """The mixer takes |hyper_w1(s)| and |hyper_w2(s)|: an output element within round-off of zero may take the other sign in fp32, and
+    then its whole loss gradient enters its hypernet with the opposite sign.  For every live element within ABS_KINK_TOL of its
+    transition's largest output, the sign whose float64 gradient is closer to the engine's at that output's bias is adopted into g64
+    (the element's share of the hypernet's weight and bias gradients, through the hidden ReLU of a 2-layer hypernet).  Returns
+    [(module, t, b, column, |o| / max |o|)] of the flips adopted.
+
+    This cannot hide a sign error in the kernels: such an error acts on every element of the hypernet output, not only on those within
+    ABS_KINK_TOL of zero (a handful per step), so the columns and tensors it reaches keep their full float64 comparison; a flip is adopted
+    only where it moves the bias gradient of its own column closer to the engine's, and everything the caller compares afterwards, that
+    column included, must still meet its bound.  g64 holds the float64 gradients by parameter name ("mixer.hyper_w1.2.bias", ...) and
+    is updated in place; gv the engine's."""
+    share = torch.as_tensor(batch[1], dtype=torch.float64)[:-1]
+    store = {}
+    hooks = []
+    for name in ("hyper_w1", "hyper_w2"):
+        def hook(m, i, out, name=name):
+            out.retain_grad()
+            store[name] = out
+        hooks.append(getattr(L64.mixer, name).register_forward_hook(hook))
+    for p in L64.params:
+        p.grad = None
+    loss, _, aux = L64.loss_terms(batch)
+    loss.backward()
+    for h in hooks:
+        h.remove()
+    live = (1 - aux["bad"]).squeeze(-1) > 0
+    flips = []
+    for name in ("hyper_w1", "hyper_w2"):
+        m = getattr(L64.mixer, name)
+        two = isinstance(m, torch.nn.Sequential)
+        out_lin = m[2] if two else m
+        pre = "mixer.%s.%s" % (name, "2." if two else "")
+        o, g_o = store[name].detach(), store[name].grad
+        rel = o.abs() / o.abs().amax(-1, keepdim=True)
+        for t, b, j in ((rel < ABS_KINK_TOL) & live.unsqueeze(-1)).nonzero().tolist():
+            d = -2.0 * float(g_o[t, b, j])                      # the element's gradient with the other sign
+            diff = float(gv[pre + "bias"][j] - g64[pre + "bias"][j])
+            if abs(diff - d) >= abs(diff):
+                continue
+            x = share[t, b]
+            g64[pre + "bias"][j] += d
+            if two:
+                hid_pre = m[0](x).detach()
+                g64[pre + "weight"][j] += d * torch.relu(hid_pre)
+                dh = d * out_lin.weight.detach()[j] * (hid_pre > 0).double()
+                g64["mixer.%s.0.weight" % name] += torch.outer(dh, x)
+                g64["mixer.%s.0.bias" % name] += dh
+            else:
+                g64[pre + "weight"][j] += d * x
+            flips.append((name, t, b, j, float(rel[t, b, j])))
+    return flips

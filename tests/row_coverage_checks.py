@@ -55,6 +55,13 @@ TD_ULPS = 16
 ROW_ATOL = 1e-6
 
 
+def td_ulps(in_dim):
+    """TD_ULPS up to 32 input columns, in proportion above: the input LayerNorm and fc1 sum over in_dim terms, and one transition's fp32
+    TD error carries that round-off.  Measured on the emulator (N 3, B 11), worst over the transitions, in ulps of max(|Q_tot|, |y|): obs 20
+    engine 5, fp32 oracle 7; obs 129 engine 30, fp32 oracle 37; obs 320 engine 114, fp32 oracle 68."""
+    return TD_ULPS * max(1, _cdiv(in_dim, 32))
+
+
 # ---- the launchers' tile rules -------------------------------------------------------------------------------------------
 def _cdiv(a, b):
     return -(-a // b)
@@ -74,6 +81,50 @@ def _front_bwd_smem_floats(in_dim, TM, gru_ext):         # agent_bwd.cu front_bw
     return o + 64 * ld64 + 2 * I64 + 4 * 64 + 3 * TM * 2 + 4 * 64
 
 
+SMEM_BYTES = 227 * 1024
+
+
+def front_bwd_max_in_dim(gru_ext):
+    """agent_bwd.cu mx_front_bwd_max_in_dim: the widest input whose 32-row k_front_bwd tile fits (384 with k_gru_wgrad beside it, as in
+    the recurrent QMIX step; 320 without, as in M-QMIX and both MADDPG learners).  The learners refuse wider inputs at creation."""
+    w = 0
+    while _front_bwd_smem_floats(w + 64, 32, gru_ext) * 4 + 16 <= SMEM_BYTES:
+        w += 64
+    return w
+
+
+def mid_warps(N, A, ME=32):
+    """mid.cu mid_pick_warps / mx_mid_supported: k_mid's warps per CTA (16 or 8), 0 where its per-warp operand staging does not fit in
+    220 KB even with 8 warps (the step then runs k_qhead + the mixer core + k_qhead_bwd)."""
+    if not (ME <= 64 and A <= 64 and N <= 32):
+        return 0
+    AR = 64 if A > 32 else 32
+    gP, gM = _round_up(N * ME, 4), _round_up(ME, 4)
+    for W in (16, 8):
+        total = 2 * AR * 66 + 2 * AR + 4 * 64 + W * 66 + W * A * 64 + W * AR + 2 * W * 64
+        total += W * ((3 * N * 64 + 2 * gP + 4 * gM + N * AR + 3) & ~3)
+        if total * 4 + 16 <= 220 * 1024:
+            return W
+    return 0
+
+
+def mix_wide_state(S, N, ME=32, HY=64):
+    """mixer.cu mx_mix_wide_state: the state moves to the tensor-core GEMMs (k_mixw_fwd / k_mixw_wgrad) when a 32-transition mixer tile
+    of round_up(S, 64) state columns no longer fits beside the hypernet tiles (N ME columns of them)."""
+    S64, H64, P64, M64 = _round_up(S, 64), _round_up(HY, 64), _round_up(N * ME, 64), _round_up(ME, 64)
+    TE = 32
+    total = TE * _ld(S64) + 3 * TE * _ld(H64) + TE * _ld(P64) + 3 * TE * _ld(M64) + TE * 32 + 8 * TE + 64 * _ld(max(S64, H64))
+    return total * 4 + 16 > SMEM_BYTES
+
+
+def min_wide_state(N, ME=32, HY=64):
+    """The narrowest state that takes the wide-state path at N agents."""
+    S = 1
+    while not mix_wide_state(S, N, ME, HY):
+        S += 1
+    return S
+
+
 class TileRules(object):
     """Row tiling of one learner step on `sms` SMs (4 in the emulator, multi_processor_count on a GPU)."""
 
@@ -84,7 +135,7 @@ class TileRules(object):
         """front_bwd_pick_rm: 16 RM rows per tile, RM in 2..4, minimising waves x (1 + RM) over the heights that fit 227 KB."""
         best, best_cost = 2, 1e30
         for rm in (2, 3, 4):
-            if _front_bwd_smem_floats(in_dim, 16 * rm, gru_ext) * 4 + 16 > 227 * 1024:
+            if _front_bwd_smem_floats(in_dim, 16 * rm, gru_ext) * 4 + 16 > SMEM_BYTES:
                 continue
             cost = _cdiv(_cdiv(M, 16 * rm), self.sms) * (1.0 + rm)
             if cost < best_cost - 1e-9:
@@ -97,11 +148,21 @@ class TileRules(object):
         total = 2 * 128 * 64 * 4 + 2 * max(kp16, 64) * 64 * 4
         return 2 if 2 * (total + 2048) <= 227 * 1024 else 1
 
-    def agent_rows(self, M, in_dim):
-        """The backward's row tiling: (kernel, rows per tile, tiles, grid) of each row kernel, and the forward's 128-row tiles."""
+    def agent_rows(self, M, in_dim, gru_ext=True):
+        """The row tiling {kernel: (rows per tile, tiles, grid)} of the backward's row kernels and of the forward (its grid per net).
+        gru_ext: the recurrent QMIX step, whose k_gru_wgrad runs beside k_front_bwd (M-QMIX has no GRU: False)."""
         sms = self.sms
         out = {}
-        if in_dim > 64:            # k_front_bwd_tc (128-row tiles) + k_wgrad_tc (64-row chunks, one persistent CTA per SM)
+        if in_dim > 128:           # FFMA throughout: k_front_fwd<2> (32-row tiles, the two nets share the SMs); k_front_bwd and
+            # k_gru_wgrad (recurrent step) on front_bwd_pick_rm's tiles, their heights filtered by round_up(in_dim, 64)-wide smem tiles
+            TM = 16 * self.front_bwd_rm(M, in_dim, gru_ext)
+            nt = _cdiv(M, TM)
+            out["k_front_bwd"] = (TM, nt, min(sms, nt))
+            if gru_ext:
+                out["k_gru_wgrad"] = out["k_front_bwd"]
+            nf = _cdiv(M, 32)
+            out["k_front_fwd"] = (32, nf, min(max(sms // 2, 1), nf))
+        elif in_dim > 64:          # k_front_bwd_tc (128-row tiles) + k_wgrad_tc (64-row chunks, one persistent CTA per SM)
             nt = _cdiv(M, 128)
             out["k_front_bwd_tc"] = (128, nt, min(self.bwd_tc_ctas_per_sm(in_dim) * sms, nt))
             nc = _cdiv(M, 64)
@@ -128,7 +189,7 @@ class TileRules(object):
 
     def row_kernel(self, in_dim):
         """The kernel whose tiles define the agent-net row edges of a path."""
-        return "k_wgrad_tc" if in_dim > 64 else "k_front_bwd"
+        return "k_wgrad_tc" if 64 < in_dim <= 128 else "k_front_bwd"
 
 
 def _edges(rules, in_dim, N, T, B):
@@ -174,7 +235,7 @@ def pick_shapes(rules, in_dim, Ns=(2, 3), Ts=range(2, 17), Bs=range(1, 65), targ
     """(B, T, N) per edge, the cheapest (fewest isolated rows B M) that hits it.  Some edges cannot occur on a path (the tile-height rule
     minimises waves, so just above `sms` tiles it may take a taller tile): then the nearest tile count that occurs is taken, and the
     returned note says so.  Returns [(targets hit, (B, T, N), layout, note)], one entry per distinct shape."""
-    targets = list(targets or AGENT_TARGETS + (["front_bwd_tc tiles = CTAs+1"] if in_dim > 64 else []))
+    targets = list(targets or AGENT_TARGETS + (["front_bwd_tc tiles = CTAs+1"] if 64 < in_dim <= 128 else []))
     best, notes = {}, {}
     cands = []
     for N, T, B in itertools.product(Ns, Ts, Bs):
@@ -286,26 +347,40 @@ def float64_twin(L):
 
 def qmix_pair(cfg, B, T, debug=True):
     """(float64 oracle, policy, trainer) with the randomised state of qmix_checks.oracle_and_trainer; trainer max_batch = B."""
-    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=debug)
+    L, args, pol, tr = qc.oracle_and_trainer(cfg, B, T, debug=debug, vdn=cfg.vdn)
     tr.use_step_graph = False
     return float64_twin(L), pol, tr
 
 
 def mqmix_pair(cfg, B, debug=False):
+    """(float64 oracle, policy, trainer) of M-QMIX, or M-VDN when cfg.vdn, with every tensor randomised; trainer max_batch = B."""
     from oracle.mqmix import MqmixLearner
     from oracle.qmix import randomize_all
     import mqmix_checks as mc
     L = MqmixLearner(cfg, seed=3)
     randomize_all(L.agent, 1)
-    randomize_all(L.mixer, 2)
+    if not cfg.vdn:
+        randomize_all(L.mixer, 2)
     L.sync_targets()
     randomize_all(L.tgt_agent, 3, 0.05)
-    randomize_all(L.tgt_mixer, 4, 0.05)
-    args, pol, tr = mc.build(cfg, B, debug)
+    if not cfg.vdn:
+        randomize_all(L.tgt_mixer, 4, 0.05)
+    if cfg.vdn:
+        from offpolicy._b200 import capi
+        from offpolicy.algorithms.mvdn.algorithm.mVDNPolicy import M_VDNPolicy
+        from offpolicy.algorithms.mvdn.mvdn import M_VDN
+        args = qc.make_args(cfg, B)
+        info = dict(obs_space=[cfg.obs_dim], share_obs_space=[cfg.state_dim], act_space=qc.Discrete(cfg.act_dim), cent_obs_dim=cfg.state_dim,
+                    cent_act_dim=cfg.act_dim * cfg.n_agents)
+        pol = M_VDNPolicy({"args": args, "device": capi.device()}, info)
+        tr = M_VDN(args, cfg.n_agents, {"policy_0": pol}, lambda a: "policy_0", device=capi.device())
+        capi.lib().mx_qmix_set_debug(tr.handle, 1 if debug else 0)
+    else:
+        args, pol, tr = mc.build(cfg, B, debug)
+        tr.mixer.load_state_dict(L.mixer.state_dict())
+        tr.target_mixer.load_state_dict(L.tgt_mixer.state_dict())
     pol.q_network.load_state_dict(L.agent.state_dict())
     tr.target_q_network.load_state_dict(L.tgt_agent.state_dict())
-    tr.mixer.load_state_dict(L.mixer.state_dict())
-    tr.target_mixer.load_state_dict(L.tgt_mixer.state_dict())
     return float64_twin(L), pol, tr
 
 
@@ -438,7 +513,7 @@ def _grad_errors(gv, L64, ref_scale=1.0, cancel=1.0):
     return out
 
 
-def isolated_episode_gradients(L64, tr, batch, episodes, B, T, N, mlp=False, tol=GRAD_TOL):
+def isolated_episode_gradients(L64, tr, batch, episodes, B, T, N, mlp=False, tol=GRAD_TOL, ulps=TD_ULPS):
     """For each b in `episodes`: one engine step with importance weights e_b from the same state, its unclipped gradient against the
     float64 oracle's.  ReLU units within round-off of zero may pick the other side (tests/kink.py): a failing comparison is re-run with the
     engine's ReLU masks forced and must then pass.  Returns the worst relative error per tensor."""
@@ -465,7 +540,7 @@ def isolated_episode_gradients(L64, tr, batch, episodes, B, T, N, mlp=False, tol
             e_ref = float(aux["err"].detach()[b])
             e_eng = float(tr.ws_view("err")[b])
             mag = max(abs(float(aux["q_tot"].detach().flatten()[b])), abs(float(aux["target"].detach().flatten()[b])))
-            assert abs(e_eng - e_ref) <= TD_ULPS * 2.0 ** -23 * mag, ("transition %d: TD error %r vs float64 %r (|Q| %.3e)" % (b, e_eng, e_ref, mag))
+            assert abs(e_eng - e_ref) <= ulps * 2.0 ** -23 * mag, ("transition %d: TD error %r vs float64 %r (|Q| %.3e)" % (b, e_eng, e_ref, mag))
             scale = e_eng / e_ref if e_ref != 0.0 else 1.0
         else:
             cancel = _cancellation(aux["err"].detach()[:, b])
@@ -518,6 +593,12 @@ def per_row_forward(L64, tr, batch, B, T, N, debug, rtol=ROW_TOL, atol=ROW_ATOL)
     x = agent_input(L64, batch)
     bad, worst = [], {}
     rows = lambda v: qc.to_rows(v, N, B)
+    # the input LayerNorm's (mean, rstd) per row: above 128 columns k_front_fwd computes them in its own strided loop
+    if L64.cfg.feature_norm:
+        xr = rows(x)
+        mean = xr.mean(1, keepdim=True)
+        rstd = 1.0 / torch.sqrt(((xr - mean) ** 2).mean(1, keepdim=True) + 1e-5)
+        _rows_close("st0", tr.ws_view("st0")[:M * 2].view(M, 2), torch.cat([mean, rstd], 1), rtol, atol, bad, worst)
     for tag, net in (("live", L64.agent), ("tgt", L64.tgt_agent)):
         trc = agent_trace(net, x)
         _rows_close("gi_" + tag, tr.ws_view("gi_" + tag)[:M * 192].view(M, 192), rows(trc["gi"]), rtol, atol, bad, worst)
@@ -532,6 +613,137 @@ def per_row_forward(L64, tr, batch, B, T, N, debug, rtol=ROW_TOL, atol=ROW_ATOL)
             _rows_close("gates", g, want, rtol, atol, bad, worst)
             _rows_close("hn", tr.ws_view("hn")[:M * 64].view(M, 64), rows(trc["hn"]), rtol, atol, bad, worst)
     assert not bad, "\n".join(bad)
+    return worst
+
+
+GREEDY_MARGIN = 1e-3
+
+
+def per_transition(L64, tr, batch, B, T, N, debug, agent_values=True, rtol=ROW_TOL, atol=ROW_ATOL):
+    """One engine step with every importance weight 1 from the trainer's current state (restored afterwards), then every transition
+    (b, t) against float64: q_taken / q_next per agent, Q_tot, the target net's Q_tot at t+1 and the TD error, and dq_taken per
+    (transition, agent) -- agent N-1 included, the last lane of the mixer's agent loop.  Each transition is bounded relative to its own
+    largest value; Q_tot also by how far its agents' round-off reaches it; the TD error relative to the larger of those scales of Q_tot
+    and y (it is their difference), and dq_taken (the TD error times d Q_tot / dq)
+    against the float64 one taken at the engine's TD error.  In debug mode also the greedy action of every row whose float64 arg-max
+    leads the runner-up available action by more than GREEDY_MARGIN.  agent_values=False where k_mid ran: it keeps q_taken, q_next and
+    dq_taken in registers and writes only the per-transition values.  Returns {field: worst err / scale}."""
+    sd0 = tr.state_dict()
+    w = np.ones(B, np.float32)
+    bt = tuple(batch[:-2]) + (w, np.arange(B))
+    tr.train_policy_on_batch(qc.ref_tuple(bt))
+    E = B * T
+    ws = lambda name, n: tr.ws_view(name)[:n].detach().cpu().double()
+    _, _, aux = L64.loss_terms(bt)
+    q_taken = aux["q_taken"]
+    numer = (L64._huber(aux["err"]) if L64.cfg.huber else aux["err"] ** 2).sum()
+    dq = torch.autograd.grad(numer, q_taken)[0].detach()                       # d (sum of per-transition losses) / dq, (T, B, N)
+    per_e = lambda v: v.detach().permute(1, 0, 2).reshape(E, -1)               # (T, B, X) -> [b T + t][X]
+    bad, worst = [], {}
+    if agent_values:
+        _rows_close("q_taken", ws("q_taken", E * N).view(E, N), per_e(q_taken), rtol, atol, bad, worst)
+        _rows_close("q_next", ws("q_next", E * N).view(E, N), per_e(aux["tq_next"]), rtol, atol, bad, worst)
+    qt, qn, y = per_e(aux["q_tot"]), per_e(aux["q_tot_next"]), per_e(aux["target"])
+    # Q_tot sums N agent terms that cancel: the agents' Q values carry their rows' round-off (within rtol of each), which reaches Q_tot
+    # as sum_n |dQ_tot/dq_n| |q_n|, not as |Q_tot| (measured on an H100 at N 32, T 12: 9.4e-5 of |Q_tot|).  Each transition's scale is
+    # that first-order propagation, or |Q_tot| where it is larger
+    share = torch.as_tensor(batch[1], dtype=torch.float64)
+    prop = []
+    for mixer, q_in, s_in in ((L64.mixer, q_taken.detach(), share[:-1]), (L64.tgt_mixer, aux["tq_next"].detach(), share[1:])):
+        q_in = q_in.clone().requires_grad_(True)
+        jac = torch.autograd.grad(mixer(q_in, s_in).sum(), q_in)[0]
+        prop.append(per_e((jac * q_in).detach().abs()).sum(1, keepdim=True))
+    _rows_close("qtot", torch.cat([ws("qtot", E).view(E, 1), prop[0]], 1), torch.cat([qt, prop[0]], 1), rtol, atol, bad, worst)
+    _rows_close("qtot_next", torch.cat([ws("qtot_next", E).view(E, 1), prop[1]], 1), torch.cat([qn, prop[1]], 1), rtol, atol, bad, worst)
+    live = 1.0 - per_e(aux["bad"])
+    err_ref = per_e(aux["err"])
+    err_eng = ws("err", E).view(E, 1)
+    mag = torch.maximum(torch.maximum(qt.abs(), y.abs()), prop[0] + L64.cfg.gamma * prop[1]) * live
+    _rows_close("err", torch.cat([err_eng, mag], 1), torch.cat([err_ref, mag], 1), rtol, atol, bad, worst)
+    if agent_values:
+        ratio = torch.where(err_ref != 0, err_eng / torch.where(err_ref != 0, err_ref, torch.ones_like(err_ref)), torch.ones_like(err_ref))
+        dq_eng = ws("dq_taken", E * N).view(E, N)
+        dq_ref = per_e(dq) * ratio
+        # the engine keeps gradient numerators: dq_taken is d(sum of losses)/dq up to one constant factor of the loss convention
+        s = float((dq_eng * dq_ref).sum() / max(float((dq_ref * dq_ref).sum()), 1e-300))
+        assert abs(s - round(s)) < 1e-3 and round(s) != 0, ("dq_taken is not an integer multiple of d(sum of losses)/dq", s)
+        _rows_close("dq_taken", dq_eng, dq_ref * round(s), rtol, atol, bad, worst)
+    if debug:
+        from oracle.qmix import masked_argmax
+        M = B * (T + 1) * N
+        q_all = aux["q_all"].detach()
+        av = L64.stack_agents(batch[6]) if batch[6] is not None else None
+        qm = q_all.clone()
+        if av is not None:
+            qm[av == 0] = -1e300
+        top2 = qm.topk(2, dim=-1)[0]
+        margin = qc.to_rows((top2[..., 0] - top2[..., 1]).unsqueeze(-1), N, B).flatten()
+        want = qc.to_rows(masked_argmax(q_all, av).unsqueeze(-1).double(), N, B).flatten()
+        got = tr.ws_view("greedy", torch.int32)[:M].detach().cpu().double()
+        sure = margin > GREEDY_MARGIN
+        wrong = (got != want) & sure
+        assert not bool(wrong.any()), ("greedy action off the float64 arg-max on %d of %d decided rows" % (int(wrong.sum()), int(sure.sum())),
+                                       int(wrong.nonzero()[0]))
+        worst["greedy decided rows"] = float(sure.sum())
+    tr.load_state_dict(sd0)
+    assert not bad, "\n".join(bad)
+    return worst
+
+
+# The wide-state GEMMs (3xTF32 on the tensor cores) against float64 on the engine's own operands: max |engine - float64| per block
+# within GEMM_TOL x max |float64| of that block (the whole-K fp32 round-off; single-pass TF32 would be ~1e-3).
+GEMM_TOL = 2e-6
+
+
+def wide_state_blocks(cfg):
+    """mixer.cu mx_mix_wide_layout: the four stacked state-reading layers [(parameter prefix, first column, rows)] and Cp, the stacked
+    columns per net padded to 16.  Block 0 / 1: hyper_w1 / hyper_w2's first (or only) layer, 2: hyper_b2's first layer, 3: hyper_b1."""
+    N, ME, HY = cfg.n_agents, cfg.mixer_hidden, cfg.hyper_hidden
+    two = cfg.hyper_layers == 2
+    spec = [("hyper_w1.0" if two else "hyper_w1", HY if two else N * ME), ("hyper_w2.0" if two else "hyper_w2", HY if two else ME),
+            ("hyper_b2.0", HY), ("hyper_b1", ME)]
+    out, c = [], 0
+    for name, rows in spec:
+        out.append((name, c, rows))
+        c += _round_up(rows, 4)
+    return out, _round_up(c, 16)
+
+
+def state_gemm_blocks(L64, tr, batch, B, T, tol=GEMM_TOL):
+    """After one engine step on `batch` (max_batch = B): every stacked block of the state GEMMs against float64.
+    k_mixw_fwd: pre[net][row][c] = share[row] . W_net[c] + b_net[c] over all B (T+1) state rows, live and target net.
+    k_mixw_wgrad: gradient partial 0 of each block's weight and bias = d_pre[e]^T share[row(e)] summed over the B T elements, d_pre
+    being the engine's own (the hypernet backward's output).  Returns {block / quantity: worst err / max |ref|}."""
+    blocks, Cp = wide_state_blocks(L64.cfg)
+    R, E = B * (T + 1), B * T
+    X = torch.as_tensor(batch[1], dtype=torch.float64).permute(1, 0, 2).reshape(R, -1)        # engine row b (T+1) + t
+    Xl = X.view(B, T + 1, -1)[:, :T].reshape(E, -1)                                            # element b T + t reads row b (T+1) + t
+    pre = tr.ws_view("hyp_pre").detach().cpu().double()
+    assert pre.numel() == 2 * R * Cp, (pre.numel(), 2 * R * Cp)
+    pre = pre.view(2, R, Cp)
+    d_pre = tr.ws_view("d_pre").detach().cpu().double().view(E, Cp)
+    gpart = tr.ws_view("gpart").detach().cpu().double()
+    offs = dict((n, o) for n, o, r, c in tr.entries)
+    worst, bad = {}, []
+
+    def close(tag, ours, ref):
+        e = float((ours - ref).abs().max() / (ref.abs().max() + 1e-300))
+        worst[tag] = e
+        if e > tol:
+            bad.append((tag, e))
+
+    for name, c0, rows in blocks:
+        for net, mixer in ((0, L64.mixer), (1, L64.tgt_mixer)):
+            sd = mixer.state_dict()
+            W, b = sd[name + ".weight"].double(), sd[name + ".bias"].double()
+            close("%s fwd net %d" % (name, net), pre[net, :, c0:c0 + rows], X @ W.T + b)
+        dp = d_pre[:, c0:c0 + rows]
+        W = L64.mixer.state_dict()[name + ".weight"]
+        o = offs["mixer." + name + ".weight"]
+        close("%s dW" % name, gpart[o:o + W.numel()].view(W.shape), dp.T @ Xl)
+        o = offs["mixer." + name + ".bias"]
+        close("%s db" % name, gpart[o:o + rows], dp.sum(0))
+    assert not bad, bad
     return worst
 
 

@@ -45,9 +45,10 @@ def test_27m_vs_30m_vs_oracle(gpu_engine):
     """B = 32 with avail masks and variable episode lengths, one step in the product configuration: loss, grad_norm, Q_tot, every
     gradient tensor (worst element at 3 % of the 1e-4 budget), the Adam update and the soft update.  Consecutive steps are covered by
     test_27m_vs_30m_graph_replay_equals_eager (loss and grad_norm of three steps).  A second step checked element-wise at this shape
-    exceeds the budget on a few reductions over the whole batch (relative L2 up to 2e-4; the mixer's hyper_w1 at 36 actions, the agent's
-    feature_norm / fc1 at 32 actions on the one-action-per-lane kernels) and does so unchanged when the oracle restarts from the
-    engine's parameters, so it is not drift of the Q-head kernels; its cause is not established."""
+    exceeds the budget on a few reductions over the whole batch (relative L2 up to 2e-4).  tests/test_gpu_smac_widths.py
+    test_27m_vs_30m_two_steps_against_float64 measured the cause: the mixer's hyper_w1 by one |.| kink (an output 2.5e-9 of its
+    transition's largest takes the other sign in fp32), the agent's feature_norm / fc1 by round-off the fp32 oracle shares to two
+    digits; that test judges both steps against float64."""
     from oracle.qmix import synth_batch
     torch.set_num_threads(8)
     cfg = _cfg27()
