@@ -44,10 +44,12 @@ int mx_abi_version(void);
  * struct mirrors at load time. */
 int64_t mx_sizeof(const char* struct_name);
 /* Host fences for pinned staging buffers a binding reuses: alloc once (id >= 0, -1 on error); record after enqueueing the copy that reads
- * the buffer; wait before rewriting it (returns at once if never recorded).  Not thread-safe; at most 256 fences per process. */
+ * the buffer; wait before rewriting it (returns at once if never recorded); release when the buffer is dropped (waits for its last
+ * record; the id may then be handed out again).  Not thread-safe; at most 256 fences held at once per process. */
 int mx_host_fence_alloc(void);
 int mx_host_fence_record(int id, void* stream);
 int mx_host_fence_wait(int id);
+int mx_host_fence_release(int id);
 /* 1 when built by nvcc for sm_90a, 0 for the CPU-emulated unit-test build (tests/emu; never shipped) */
 int mx_is_cuda_build(void);
 
@@ -328,6 +330,10 @@ int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, 
  * captured graph reads the store as it is at replay time. */
 int mx_maddpg_set_valid(mx_maddpg* h, const float* valid_dev);
 int64_t mx_maddpg_num_updates(const mx_maddpg* h);   /* updates done so far (self.num_updates[p_id], r_maddpg.py:125) */
+int mx_maddpg_set_num_updates(mx_maddpg* h, int64_t n);   /* restore the update count (checkpoint resume); n >= 0 */
+/* Named workspace region (byte offset, length in 4-byte words): "adam_ta" / "adam_tc", the actor / critic Adam step counters (fp64)
+ * a checkpoint saves beside the parameter vectors.  Non-zero and mx_last_error for an unknown name. */
+int mx_maddpg_ws_lookup(const mx_maddpg* h, const char* name, int64_t* byte_offset, int64_t* n_elems);
 /* device fp32[8]: critic_loss, critic_grad_norm, -, denom, actor_loss, actor_grad_norm, -, denom */
 const float* mx_maddpg_info(mx_maddpg* h);
 const float* mx_maddpg_priorities(mx_maddpg* h);

@@ -57,22 +57,43 @@ extern "C" int mx_abi_version(void) { return MX_ABI_VERSION; }
 // The drop-in buffers reuse a few pinned host blocks (insert staging, sampled-index ring); a block may be rewritten only after the copy
 // that read it has completed.  A pool of timing-less CUDA events behind three tiny calls: a torch.cuda.Event().record() costs the
 // host ~8 us per call (it resolves the current stream object first), these ~1 us.
+// A released fence goes to a free list and is handed out again, so a process may create and drop buffers without running out.
 #define MX_MAX_FENCES 256
 #if !MX_EMU
 static cudaEvent_t g_fence[MX_MAX_FENCES];
 static unsigned char g_fence_set[MX_MAX_FENCES];
 #endif
 static int g_fence_n = 0;
+static unsigned char g_fence_live[MX_MAX_FENCES];
+static int g_fence_free[MX_MAX_FENCES];
+static int g_fence_nfree = 0;
+static bool fence_ok(int id) { return id >= 0 && id < g_fence_n && g_fence_live[id]; }
 extern "C" int mx_host_fence_alloc(void) {
-  if (g_fence_n >= MX_MAX_FENCES) { mx_set_error("mx_host_fence_alloc: out of fences"); return -1; }
+  if (g_fence_nfree > 0) {
+    const int id = g_fence_free[--g_fence_nfree];
+    g_fence_live[id] = 1;
+    return id;
+  }
+  if (g_fence_n >= MX_MAX_FENCES) { mx_set_error("mx_host_fence_alloc: out of fences (%d held)", MX_MAX_FENCES); return -1; }
 #if !MX_EMU
   if (cudaEventCreateWithFlags(&g_fence[g_fence_n], cudaEventDisableTiming) != cudaSuccess) { mx_set_error("mx_host_fence_alloc: cudaEventCreate failed"); return -1; }
   g_fence_set[g_fence_n] = 0;
 #endif
+  g_fence_live[g_fence_n] = 1;
   return g_fence_n++;
 }
+extern "C" int mx_host_fence_release(int id) {
+  if (!fence_ok(id)) { mx_set_error("mx_host_fence_release: bad fence"); return 1; }
+#if !MX_EMU
+  if (g_fence_set[id]) cudaEventSynchronize(g_fence[id]);      // the copy it guards has finished before the id is handed out again
+  g_fence_set[id] = 0;
+#endif
+  g_fence_live[id] = 0;
+  g_fence_free[g_fence_nfree++] = id;
+  return 0;
+}
 extern "C" int mx_host_fence_record(int id, void* stream) {
-  if (id < 0 || id >= g_fence_n) { mx_set_error("mx_host_fence_record: bad fence"); return 1; }
+  if (!fence_ok(id)) { mx_set_error("mx_host_fence_record: bad fence"); return 1; }
 #if !MX_EMU
   if (cudaEventRecord(g_fence[id], (cudaStream_t)stream) != cudaSuccess) { mx_set_error("mx_host_fence_record: cudaEventRecord failed"); return 1; }
   g_fence_set[id] = 1;
@@ -82,7 +103,7 @@ extern "C" int mx_host_fence_record(int id, void* stream) {
   return 0;
 }
 extern "C" int mx_host_fence_wait(int id) {       // returns once everything enqueued before the last record of this fence has completed
-  if (id < 0 || id >= g_fence_n) { mx_set_error("mx_host_fence_wait: bad fence"); return 1; }
+  if (!fence_ok(id)) { mx_set_error("mx_host_fence_wait: bad fence"); return 1; }
 #if !MX_EMU
   if (g_fence_set[id]) {
     const cudaError_t e = cudaEventSynchronize(g_fence[id]);      // also the first place an asynchronous fault of earlier work surfaces

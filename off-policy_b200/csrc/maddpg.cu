@@ -1162,6 +1162,24 @@ extern "C" int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, do
   return mx_graph_capture_seq(seq, [h]() { h->num_updates += 1; }, stream, out);
 }
 extern "C" int64_t mx_maddpg_num_updates(const mx_maddpg* h) { return h->num_updates; }
+extern "C" int mx_maddpg_set_num_updates(mx_maddpg* h, int64_t n) {
+  if (!h) { mx_set_error("mx_maddpg_set_num_updates: null handle"); return 1; }
+  if (n < 0) { mx_set_error("mx_maddpg_set_num_updates: update count %lld < 0", (long long)n); return 1; }
+  h->num_updates = n;
+  return 0;
+}
+
+// named regions of the workspace, length in 4-byte words (as mx_qmix_ws_lookup): the actor / critic Adam step counters (fp64 words),
+// the resumable state a checkpoint must carry besides the parameter vectors
+extern "C" int mx_maddpg_ws_lookup(const mx_maddpg* h, const char* name, int64_t* byte_offset, int64_t* n_elems) {
+  if (!h || !name) { mx_set_error("mx_maddpg_ws_lookup: null argument"); return 1; }
+  struct Ent { const char* n; int64_t off, cnt; };
+  const Ent tab[] = {{"adam_ta", h->W.adam_ta, 8}, {"adam_tc", h->W.adam_tc, 8}};
+  for (const Ent& e : tab)
+    if (!strcmp(e.n, name)) { *byte_offset = e.off * 4; *n_elems = e.cnt; return 0; }
+  mx_set_error("mx_maddpg_ws_lookup: unknown region '%s'", name);
+  return 1;
+}
 
 // cfg.mlp: the critic's target update stops at its trunk -- the target heads stay the target critic's own initialisation
 static int64_t critic_tracked(const mx_maddpg* h) { return h->cfg.mlp ? (int64_t)h->critic.wih : h->Pc; }

@@ -93,6 +93,7 @@ def _declare(lib):
         "mx_host_fence_alloc": (C.c_int, []),
         "mx_host_fence_record": (C.c_int, [C.c_int, vp]),
         "mx_host_fence_wait": (C.c_int, [C.c_int]),
+        "mx_host_fence_release": (C.c_int, [C.c_int]),
         "mx_is_cuda_build": (C.c_int, []),
         "mx_launch_count": (i64, []),
         "mx_replay_layout_query": (C.c_int, [C.POINTER(ReplayCfg), C.POINTER(ReplayLayout)]),
@@ -151,6 +152,8 @@ def _declare(lib):
         "mx_tc_linear_probe": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
         "mx_maddpg_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(vp)]),
         "mx_maddpg_num_updates": (i64, [vp]),
+        "mx_maddpg_set_num_updates": (C.c_int, [vp, i64]),
+        "mx_maddpg_ws_lookup": (C.c_int, [vp, C.c_char_p, C.POINTER(i64), C.POINTER(i64)]),
         "mx_maddpg_set_valid": (C.c_int, [vp, vp]),
         "mx_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, C.POINTER(vp)]),
         "mx_graph_launch": (C.c_int, [vp, vp]),

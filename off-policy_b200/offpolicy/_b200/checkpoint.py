@@ -8,7 +8,11 @@ restore path is broken (`restore_q` runs before the trainer exists, App. D-3).  
     load_checkpoint(path, trainer, buffer)     # PER trees, device MT19937), NumPy's and torch's host generators
 
 After `load_checkpoint` into freshly constructed objects the next learner steps are bit-identical to the uninterrupted run
-(tests/test_emu_checkpoint.py, tests/test_gpu_checkpoint.py).
+(tests/test_emu_checkpoint.py, tests/test_gpu_checkpoint.py, tests/test_{emu,gpu}_checkpoint_maddpg.py).
+
+Trainers: `QMix`, `VDN`, `M_QMix`, `M_VDN` (QMix.state_dict), `R_MADDPG`, `R_MATD3`, `MADDPG`, `MATD3` (shared or one policy per agent;
+offpolicy/_b200/maddpg_state.py).  Replays: `RecReplayBuffer`, `PrioritizedRecReplayBuffer`, `MlpReplayBuffer`,
+`PrioritizedMlpReplayBuffer`.  A checkpoint of another configuration is refused with ValueError.
 """
 import numpy as np
 import torch

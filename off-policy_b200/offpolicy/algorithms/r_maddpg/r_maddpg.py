@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from offpolicy._b200 import capi
+from offpolicy._b200.maddpg_state import MaddpgLearnerState
 from offpolicy.algorithms.r_maddpg.algorithm.rMADDPGPolicy import maddpg_cfg_struct, sample_gumbel
 from offpolicy.utils.rec_buffer import SampledBatch, DeviceArray
 
@@ -92,7 +93,7 @@ class _Engine(object):
             self.handle = None
 
 
-class R_MADDPG(object):
+class R_MADDPG(MaddpgLearnerState):
     def __init__(self, args, num_agents, policies, policy_mapping_fn, device=None, episode_length=None, actor_update_interval=1):
         self.args = args
         self.use_per = args.use_per

@@ -16,7 +16,7 @@ Several policies (`--share_policy` off, one policy per agent): one store per pol
 import numpy as np
 import torch
 
-from offpolicy.utils.rec_buffer import RecPolicyBuffer, _LazyField, sample_shared_uniform, share_indices
+from offpolicy.utils.rec_buffer import PolicyStoresState, RecPolicyBuffer, _LazyField, sample_shared_uniform, share_indices
 
 MLP_FIELDS = ("obs", "share_obs", "acts", "rewards", "next_obs", "next_share_obs", "dones", "dones_env", "valid_transition",
               "avail_acts", "next_avail_acts")
@@ -120,8 +120,20 @@ class MlpPolicyBuffer(object):
             out = v.reshape(B, 1)
         return out.contiguous().cpu().numpy()
 
+    # -- checkpoint / resume: the episode replay's persistent part + valid_transition -------------------------------------
+    def state_dict(self):
+        return {"rep": self.rep.state_dict(), "valid_transition": self.valid_transition.copy()}
 
-class MlpReplayBuffer(object):
+    def load_state_dict(self, sd):
+        valid = np.asarray(sd["valid_transition"], dtype=np.float32)
+        if valid.shape != self.valid_transition.shape:
+            raise ValueError("replay checkpoint has valid_transition of shape %s, this buffer %s" % (valid.shape, self.valid_transition.shape))
+        self.rep.load_state_dict(sd["rep"])          # checks capacity, agents and widths
+        self.valid_transition[...] = valid
+        self.valid_dev.copy_(torch.from_numpy(valid[:, :, 0]).to(self.valid_dev.device))     # in place: learners keep its pointer
+
+
+class MlpReplayBuffer(PolicyStoresState):
     def __init__(self, policy_info, policy_agents, buffer_size, use_same_share_obs, use_avail_acts, use_reward_normalization=False,
                  rng="numpy", max_batch=None, _per_alpha=None):
         self.policy_info = policy_info

@@ -171,6 +171,10 @@ class RecPolicyBuffer(object):
 
     def __del__(self):
         try:
+            for f in (getattr(self, "_stage_evt", None) or []) + (getattr(self, "_idx_ring_evt", None) or []):
+                if f is not None and f >= 0:
+                    capi.lib().mx_host_fence_release(f)      # the process-wide pool is bounded: a resumed run builds fresh buffers
+            self._stage_evt = self._idx_ring_evt = None
             if getattr(self, "handle", None):
                 capi.lib().mx_replay_destroy(self.handle)
                 self.handle = None
@@ -451,7 +455,22 @@ def sample_shared_uniform(stores, first, batch_size, rng, n):
     return inds
 
 
-class RecReplayBuffer(object):
+class PolicyStoresState(object):
+    """Checkpoint / resume of a replay made of one store per policy (`policy_buffers`) and an index-stream mode (`rng`): the episode
+    replays here and the transition replays of utils/mlp_buffer.py."""
+
+    def state_dict(self):
+        return {"rng": self.rng, "policy_buffers": {p: b.state_dict() for p, b in self.policy_buffers.items()}}
+
+    def load_state_dict(self, sd):
+        if sorted(sd["policy_buffers"]) != sorted(self.policy_buffers):
+            raise ValueError("replay checkpoint holds policies %s, this buffer %s" % (sorted(sd["policy_buffers"]), sorted(self.policy_buffers)))
+        self.rng = sd["rng"]
+        for p, b in self.policy_buffers.items():
+            b.load_state_dict(sd["policy_buffers"][p])
+
+
+class RecReplayBuffer(PolicyStoresState):
     """Uniform episode replay (rec_buffer.py:10-82)."""
 
     def __init__(self, policy_info, policy_agents, buffer_size, episode_length, use_same_share_obs, use_avail_acts,
@@ -483,14 +502,6 @@ class RecReplayBuffer(object):
         self.rng = "device"
         for b in self.policy_buffers.values():
             b.seed_device_rng(seed)
-
-    def state_dict(self):
-        return {"rng": self.rng, "policy_buffers": {p: b.state_dict() for p, b in self.policy_buffers.items()}}
-
-    def load_state_dict(self, sd):
-        self.rng = sd["rng"]
-        for p, b in self.policy_buffers.items():
-            b.load_state_dict(sd["policy_buffers"][p])
 
     def adopt_numpy_rng(self):
         self.rng = "device"
