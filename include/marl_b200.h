@@ -16,7 +16,8 @@
  *     on that forked branch, ordered against the caller's stream by events -- parallel graph branches
  *     under stream capture.)
  *   - every launch is ordered on the cudaStream_t given (as void*), is asynchronous and never synchronises,
- *     except the calls documented as synchronising (mx_replay_restore, mx_replay_get_rng_state, mx_profile_end).
+ *     except the calls documented as synchronising (mx_replay_restore, mx_replay_get_rng_state, mx_trng_seed / set_state /
+ *     get_state, mx_profile_end).
  *     Host pointers given to *_async calls must stay valid until the stream reaches that point
  *     (cudaMemcpyAsync rules); use pinned memory for real asynchrony.
  *   - all floating-point data is fp32 unless stated; PER trees are fp64 like the reference
@@ -40,8 +41,8 @@ typedef struct mx_qmix mx_qmix;       /* recurrent QMIX / VDN learner (QMix trai
 const char* mx_last_error(void);
 int mx_abi_version(void);
 /* sizeof() of a public struct by its C name ("mx_batch", "mx_replay_cfg", "mx_replay_layout", "mx_qmix_cfg", "mx_maddpg_cfg",
- * "mx_param_entry", "mx_policy_step_args", "mx_episodes"); -1 for an unknown name.  Lets a binding written in another language verify its
- * struct mirrors at load time. */
+ * "mx_param_entry", "mx_policy_step_args", "mx_episodes", "mx_trng_draw"); -1 for an unknown name.  Lets a binding written in another
+ * language verify its struct mirrors at load time. */
 int64_t mx_sizeof(const char* struct_name);
 /* Host fences for pinned staging buffers a binding reuses: alloc once (id >= 0, -1 on error); record after enqueueing the copy that reads
  * the buffer; wait before rewriting it (returns at once if never recorded); release when the buffer is dropped (waits for its last
@@ -325,6 +326,39 @@ int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* src_batch, const f
 struct mx_graph;
 int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                             const float* actor_noise_dev, int32_t update_actor, void* stream, struct mx_graph** out);
+
+/* torch's CPU generator on the device (the mt19937 behind torch.manual_seed / uniform_ / normal_): the noise draws of an update
+ * without host work.  The state is caller-owned device memory of MX_TRNG_WORDS uint32: key[624], then torch's `left` and `next`
+ * (the next word read is key[625 - left], after a twist when that is 624).  One fill reproduces one torch call on a contiguous float
+ * tensor of shape (T, rows_n * rows_b, cols) -- it consumes exactly the words torch would, the uniforms are bit-identical, the Gumbel
+ * and normal transforms agree with torch's to a few ulps -- and writes value (t, n * rows_b + b, c) to
+ * dst[t * ld_t + n * ld_n + b * ld_b + c].  Kinds: uniform_; uniform_ then -log(-log(u + 1e-20) + 1e-20) (sample_gumbel,
+ * utils/util.py:127-130); normal_(0, std) of >= 16 values (torch's Box-Muller over blocks of 16 with the redrawn tail block; a smaller
+ * normal draw takes torch's scalar path and is refused). */
+#define MX_TRNG_WORDS 640
+#define MX_TRNG_UNIFORM 0
+#define MX_TRNG_GUMBEL 1
+#define MX_TRNG_NORMAL 2
+typedef struct mx_trng_draw {
+  int32_t kind;
+  int32_t T, rows_n, rows_b, cols;   /* source shape (T, rows_n * rows_b, cols), rows agent-major: row = n * rows_b + b */
+  float std;                         /* MX_TRNG_NORMAL */
+  float* dst;                        /* device fp32, first column of the destination block */
+  int64_t ld_t, ld_n, ld_b;          /* destination strides in floats */
+} mx_trng_draw;
+int mx_trng_seed(uint32_t* state_dev, uint64_t seed, void* stream);      /* torch.manual_seed(seed); synchronises */
+int mx_trng_set_state(uint32_t* state_dev, const uint32_t key[624], int32_t left, int32_t next, void* stream);   /* synchronises */
+int mx_trng_get_state(const uint32_t* state_dev, uint32_t key[624], int32_t* left, int32_t* next, void* stream); /* synchronises */
+/* MT19937 words the fill consumes (the scratch it needs), or -1 and mx_last_error for a bad fill */
+int64_t mx_trng_words(const mx_trng_draw* f);
+/* Enqueue one fill on `stream` (two launches); advances the device state.  scratch_dev: device uint32[scratch_words >= mx_trng_words]. */
+int mx_trng_fill(uint32_t* state_dev, const mx_trng_draw* f, uint32_t* scratch_dev, int64_t scratch_words, void* stream);
+/* mx_maddpg_graph_capture with the update's noise draws at the head of the graph: the n_fills fills (in the order torch's calls would
+ * make them, into target_noise_dev / actor_noise_dev) run from state_dev before the sample, so one mx_graph_launch is the whole update.
+ * The fills share the scratch, which must hold the largest of them. */
+int mx_maddpg_graph_capture_ex(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
+                               const float* actor_noise_dev, int32_t update_actor, uint32_t* state_dev, const mx_trng_draw* fills,
+                               int32_t n_fills, uint32_t* scratch_dev, int64_t scratch_words, void* stream, struct mx_graph** out);
 /* cfg.mlp: valid_transition of the transition store, device fp32 [rows][n_agents] (mlp_buffer.py:156).  The actor loss of a batch
  * reads row batch->idx[b] (row b when the batch has no indices); NULL: every transition is valid.  The pointer is kept, so a
  * captured graph reads the store as it is at replay time. */

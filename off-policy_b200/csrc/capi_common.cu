@@ -116,7 +116,7 @@ extern "C" int64_t mx_sizeof(const char* n) {
   if (!n) return -1;
 #define MX_SZ(T) if (!strcmp(n, #T)) return (int64_t)sizeof(T)
   MX_SZ(mx_batch); MX_SZ(mx_replay_cfg); MX_SZ(mx_replay_layout); MX_SZ(mx_qmix_cfg); MX_SZ(mx_maddpg_cfg); MX_SZ(mx_param_entry);
-  MX_SZ(mx_policy_step_args); MX_SZ(mx_episodes);
+  MX_SZ(mx_policy_step_args); MX_SZ(mx_episodes); MX_SZ(mx_trng_draw);
 #undef MX_SZ
   return -1;
 }

@@ -1139,14 +1139,32 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
 // the update counter asks for; the noise buffers are fixed device buffers the caller refills before each launch.
 extern "C" int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                                        const float* actor_noise_dev, int32_t update_actor, void* stream, mx_graph** out) {
+  return mx_maddpg_graph_capture_ex(r, h, B, beta, flags, target_noise_dev, actor_noise_dev, update_actor, nullptr, nullptr, 0, nullptr, 0,
+                                    stream, out);
+}
+// The same graph headed by the update's noise fills (torch_rng.cu): no host draw and no copy per replay.
+extern "C" int mx_maddpg_graph_capture_ex(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
+                                          const float* actor_noise_dev, int32_t update_actor, uint32_t* state_dev, const mx_trng_draw* fills,
+                                          int32_t n_fills, uint32_t* scratch_dev, int64_t scratch_words, void* stream, mx_graph** out) {
   if (!r || !h || !out) { mx_set_error("mx_maddpg_graph_capture: null argument"); return 1; }
   if (h->cfg.mlp && h->cfg.cent_act_dim > 0) {      // the graph would replay the step without the other policies' contributions
     mx_set_error("mx_maddpg_graph_capture: an MLP learner with several policies (cent_act_dim > 0) cannot be captured: its step needs "
                  "mx_maddpg_cent_contribute from every policy first; run it eagerly");
     return 1;
   }
+  if (n_fills < 0 || (n_fills > 0 && (!fills || !state_dev || !scratch_dev))) {
+    mx_set_error("mx_maddpg_graph_capture_ex: %d fills need the fills, the generator state and the scratch", n_fills); return 1;
+  }
+  std::vector<mx_trng_draw> fl(fills, fills + n_fills);
+  for (const mx_trng_draw& f : fl) {              // refused here rather than half-way through the capture
+    const int64_t w = mx_trng_words(&f);
+    if (w < 0) return 1;
+    if (w > scratch_words) { mx_set_error("mx_maddpg_graph_capture_ex: scratch of %lld words, a fill consumes %lld", (long long)scratch_words, (long long)w); return 1; }
+  }
   if ((flags & 2u) && mx_replay_set_beta(r, beta, stream)) return 1;
   auto seq = [=](void* st) -> int {
+    for (const mx_trng_draw& f : fl)
+      if (mx_trng_fill(state_dev, &f, scratch_dev, scratch_words, st)) return 1;
     if (flags & 1u) { if (mx_replay_sample_uniform(r, B, st)) return 1; }
     else if (flags & 2u) { if (mx_replay_sample_per_state_beta(r, B, st)) return 1; }      // exponent: device scalar (mx_replay_set_beta)
     mx_batch b;

@@ -10,6 +10,7 @@
 #include <string.h>
 
 #include "mx_internal.h"
+#include "mx_mt19937.cuh"
 
 // =====================================================================================================
 // layout
@@ -205,41 +206,8 @@ __global__ void k_tree_update(TreeUpd u) {
 }
 
 // =====================================================================================================
-// NumPy legacy MT19937 on the device (SURVEY.md App. C; oracle/mt19937.py is the CPU restatement)
+// NumPy legacy MT19937 on the device (SURVEY.md App. C; oracle/mt19937.py is the CPU restatement; generator core: mx_mt19937.cuh)
 // =====================================================================================================
-#define MT_N 624
-#define MT_M 397
-
-MX_DEVINL uint32_t mt_temper(uint32_t y) {
-  y ^= y >> 11;
-  y ^= (y << 7) & 0x9D2C5680u;
-  y ^= (y << 15) & 0xEFC60000u;
-  y ^= y >> 18;
-  return y;
-}
-MX_DEVINL uint32_t mt_mix(uint32_t cur, uint32_t nxt, uint32_t far) {
-  uint32_t y = (cur & 0x80000000u) | (nxt & 0x7FFFFFFFu);
-  return far ^ (y >> 1) ^ ((y & 1u) ? 0x9908B0DFu : 0u);
-}
-// In-place regeneration of all 624 words by the whole CTA (>= 256 threads): three dependency-free phases.
-MX_DEVINL void mt_twist_cta(uint32_t* key) {
-  const int tid = threadIdx.x;
-  const int lo[3] = {0, 227, 454}, hi[3] = {227, 454, 624};
-  for (int ph = 0; ph < 3; ++ph) {
-    uint32_t v = 0;
-    const int i = lo[ph] + tid;
-    const bool act = i < hi[ph];
-    if (act) {
-      uint32_t nxt = key[(i + 1) % MT_N];
-      uint32_t far = key[(i + MT_M) % MT_N];
-      v = mt_mix(key[i], nxt, far);
-    }
-    __syncthreads();
-    if (act) key[i] = v;   // i == 623 reads key[0], already regenerated in phase 0, exactly like the serial loop
-    __syncthreads();
-  }
-}
-
 struct DrawArgs {
   uint32_t* rng;               // key[624]
   MxReplayState* state;

@@ -75,6 +75,15 @@ class PolicyStepArgs(C.Structure):
                 [(n, C.c_void_p) for n in ("x", "h_in", "h_out", "out", "avail", "greedy", "greedy_q", "h_copy")] + [("mlp", C.c_int32), ("no_feature_norm", C.c_int32), ("use_tanh", C.c_int32)])
 
 
+TRNG_WORDS = 640      # MX_TRNG_WORDS: the device copy of torch's CPU generator (key[624], left, next)
+TRNG_UNIFORM, TRNG_GUMBEL, TRNG_NORMAL = 0, 1, 2
+
+
+class TrngDraw(C.Structure):
+    _fields_ = ([(n, C.c_int32) for n in ("kind", "T", "rows_n", "rows_b", "cols")] + [("std", C.c_float), ("dst", C.c_void_p)] +
+                [(n, C.c_int64) for n in ("ld_t", "ld_n", "ld_b")])
+
+
 class MxError(RuntimeError):
     pass
 
@@ -151,6 +160,13 @@ def _declare(lib):
         "mx_set_option": (C.c_int, [C.c_char_p, i32]),
         "mx_tc_linear_probe": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, i32, vp]),
         "mx_maddpg_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(vp)]),
+        "mx_maddpg_graph_capture_ex": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(TrngDraw), i32, vp, i64, vp,
+                                                 C.POINTER(vp)]),
+        "mx_trng_seed": (C.c_int, [vp, C.c_uint64, vp]),
+        "mx_trng_set_state": (C.c_int, [vp, C.POINTER(u32), i32, i32, vp]),
+        "mx_trng_get_state": (C.c_int, [vp, C.POINTER(u32), C.POINTER(i32), C.POINTER(i32), vp]),
+        "mx_trng_words": (i64, [C.POINTER(TrngDraw)]),
+        "mx_trng_fill": (C.c_int, [vp, C.POINTER(TrngDraw), vp, i64, vp]),
         "mx_maddpg_num_updates": (i64, [vp]),
         "mx_maddpg_set_num_updates": (C.c_int, [vp, i64]),
         "mx_maddpg_ws_lookup": (C.c_int, [vp, C.c_char_p, C.POINTER(i64), C.POINTER(i64)]),

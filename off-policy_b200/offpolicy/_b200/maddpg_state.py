@@ -3,8 +3,9 @@
 Per policy the learner is its eight flat vectors (actor and critic: live, target, Adam m, Adam v; the MLP critic's frozen live and
 target heads sit in the critic vectors past the trunk), the two Adam step counters in its workspace (fp64 words) and the update count,
 kept twice: the host `num_updates[p_id]` the trainer and the graph helpers read, and the handle's own count that picks the actor
-phase of an eager step.  Loading writes every value in place, so the mx_maddpg handles, the `mx_maddpg_set_valid` pointers and any
-captured whole-update graph stay valid."""
+phase of an eager step.  A trainer in device noise mode (`use_device_noise`) also saves its generator's key and position
+("device_noise"); a host-mode checkpoint has no such entry and keeps the earlier format.  Loading writes every value in place, so the
+mx_maddpg handles, the `mx_maddpg_set_valid` pointers, the generator's device state and any captured whole-update graph stay valid."""
 import ctypes as C
 
 import torch
@@ -57,7 +58,10 @@ class MaddpgLearnerState(object):
                         "num_updates": int(self.num_updates[p]), "engine_updates": int(lib.mx_maddpg_num_updates(e.handle))}
             for name in ADAM_COUNTERS:
                 state[p][name] = self.ws_view(name, p, torch.float64).cpu().clone()
-        return {"config": self._config_key(), "state": state}
+        sd = {"config": self._config_key(), "state": state}
+        if getattr(self, "noise_gen", None) is not None:
+            sd["device_noise"] = self.noise_gen.state_dict()
+        return sd
 
     def load_state_dict(self, sd):
         want = self._config_key()
@@ -74,6 +78,10 @@ class MaddpgLearnerState(object):
             for key in w:
                 if g.get(key) != w[key]:
                     raise ValueError("learner checkpoint of policy %s was written for a different %s" % (p, key))
+        gen = getattr(self, "noise_gen", None)
+        if (gen is not None) != ("device_noise" in sd):
+            raise ValueError("learner checkpoint was written in %s noise mode, this trainer draws its noise on the %s"
+                             % ("device" if "device_noise" in sd else "host", "device" if gen is not None else "host"))
         lib = capi.lib()
         for p in self.policy_ids:
             e, st = self._eng[p], sd["state"][p]
@@ -83,5 +91,7 @@ class MaddpgLearnerState(object):
                 self.ws_view(name, p, torch.float64).copy_(torch.as_tensor(st[name]).to(self.dev))
             capi.check(lib.mx_maddpg_set_num_updates(e.handle, int(st["engine_updates"])))
             self.num_updates[p] = int(st["num_updates"])
+        if gen is not None:
+            gen.load_state_dict(sd["device_noise"])
         if self.dev.type == "cuda":
             torch.cuda.synchronize(self.dev)      # the next step may be a graph replay on another stream

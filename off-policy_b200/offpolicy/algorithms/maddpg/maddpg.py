@@ -19,7 +19,10 @@ in id order, which is also the order of the reference's target-noise draws.  Onl
 
 MultiDiscrete policies (`act_dim` an ndarray of sub-space widths) occupy `output_dim` columns of every action vector; the learner gets
 the sub-space widths (cfg.act_seg) and transforms each one-hot block on its own.  Their Gumbel draws are one `sample_gumbel` call per
-sub-space, in sub-space order, as the reference's per-block `gumbel_softmax` calls make them (MADDPGPolicy.py:73-89)."""
+sub-space, in sub-space order, as the reference's per-block `gumbel_softmax` calls make them (MADDPGPolicy.py:73-89).
+
+`use_device_noise(gen)` makes the same torch calls on the device, one fill each, straight into the learner's noise rows
+(offpolicy/_b200/torch_rng.py)."""
 import ctypes as C
 
 import numpy as np
@@ -27,6 +30,7 @@ import torch
 
 from offpolicy._b200 import capi
 from offpolicy._b200.maddpg_state import MaddpgLearnerState
+from offpolicy._b200.torch_rng import DeviceNoise, draw
 from offpolicy.algorithms.r_maddpg.algorithm.rMADDPGPolicy import maddpg_cfg_struct, sample_gumbel
 from offpolicy.utils.mlp_buffer import MlpSampledBatch
 from offpolicy.utils.rec_buffer import DeviceArray
@@ -118,7 +122,7 @@ class _Engine(object):
             self.handle = None
 
 
-class MADDPG(MaddpgLearnerState):
+class MADDPG(MaddpgLearnerState, DeviceNoise):
     def __init__(self, args, num_agents, policies, policy_mapping_fn, device=None, actor_update_interval=1):
         self.args = args
         self.use_per = args.use_per
@@ -195,6 +199,35 @@ class MADDPG(MaddpgLearnerState):
         ours[:, step] = draw.view(N, B, A).permute(1, 0, 2)
         return ours.to(self.dev, non_blocking=True)
 
+    _noise_steps = 2
+
+    def _noise_cols(self, p_id):
+        return self._eng[p_id].pol.output_dim
+
+    def _noise_draws(self, B, p_id, which, buf):
+        """Device mode: the torch calls of draw_target_noise (step 1) / draw_actor_noise (step 0) as fills into [b][step][n][A], one
+        per MultiDiscrete sub-space at its columns."""
+        e = self._eng[p_id]
+        pol, N, A = e.pol, e.n_agents, e.pol.output_dim
+        col = (1 if which == "target" else 0) * N * A
+        ld = (0, A, 2 * N * A)
+        if which == "target" and not pol.discrete:
+            return [draw(capi.TRNG_NORMAL, 1, N, B, A, buf, col, *ld, std=float(pol.target_noise))]
+        out = []
+        for n in (pol.act_segs if pol.act_segs is not None else [pol.act_dim]):
+            out.append(draw(capi.TRNG_GUMBEL, 1, N, B, int(n), buf, col, *ld))
+            col += int(n)
+        return out
+
+    def _noise(self, B, p_id, which):
+        """One policy's target ('target') or actor-update ('actor') noise rows on the device, or None when its update takes none."""
+        pol = self._eng[p_id].pol
+        if self.noise_gen is not None:
+            return self._device_noise(B, p_id, which) if (pol.td3 if which == "target" else pol.discrete) else None
+        if which == "target":
+            return self._rows(self.draw_target_noise(B, p_id), B, 1, p_id)
+        return self._rows(self.draw_actor_noise(B, p_id), B, 0, p_id)
+
     def _device_batch(self, batch, p_id):
         lib = capi.lib()
         e = self._eng[p_id]
@@ -231,15 +264,15 @@ class MADDPG(MaddpgLearnerState):
             keep = []
             for q in self.policy_ids:
                 bq = b if q == update_policy_id else self._device_batch(batch, q)
-                nq = self._rows(self.draw_target_noise(b.B, q), b.B, 1, q)
+                nq = self._noise(b.B, q, "target")
                 keep.append((bq, nq))
                 if q == update_policy_id:
                     self._noise_dev = nq
                 capi.check(lib.mx_maddpg_cent_contribute(self._eng[q].handle, C.byref(bq), capi.ptr(nq), e.handle, stream))
             self._keep = keep
         else:
-            self._noise_dev = self._rows(self.draw_target_noise(b.B, update_policy_id), b.B, 1, update_policy_id)
-        self._actor_noise_dev = self._rows(self.draw_actor_noise(b.B, update_policy_id), b.B, 0, update_policy_id)
+            self._noise_dev = self._noise(b.B, update_policy_id, "target")
+        self._actor_noise_dev = self._noise(b.B, update_policy_id, "actor")
         upd = C.c_int32()
         capi.check(lib.mx_maddpg_step_ex(e.handle, C.byref(b), capi.ptr(self._noise_dev), capi.ptr(self._actor_noise_dev), C.byref(upd),
                                          stream))

@@ -5,7 +5,8 @@ branch steps, TD target, critic loss/backward/Adam, then (every `actor_update_in
 the updated critic -- all on the device.  MATD3's Gaussian target-action noise is drawn on the host with the reference's
 own call (`torch.empty(shape).normal_`, utils/util.py:217-218) so a seeded run consumes torch's CPU RNG identically; for
 Discrete actors the Gumbel draws of the target actions (MATD3) and of the actor update (`use_gumbel=True`, r_maddpg.py:277) are
-drawn the same way (utils/util.py:127-130), in the reference's order.
+drawn the same way (utils/util.py:127-130), in the reference's order.  `use_device_noise(gen)` makes the same draws on the device instead
+(offpolicy/_b200/torch_rng.py).
 `cent_train_policy_on_batch` (per-agent centralised observations) is unusable in the reference (SURVEY.md App. D-7) and is not built."""
 import ctypes as C
 
@@ -14,6 +15,7 @@ import torch
 
 from offpolicy._b200 import capi
 from offpolicy._b200.maddpg_state import MaddpgLearnerState
+from offpolicy._b200.torch_rng import DeviceNoise, draw
 from offpolicy.algorithms.r_maddpg.algorithm.rMADDPGPolicy import maddpg_cfg_struct, sample_gumbel
 from offpolicy.utils.rec_buffer import SampledBatch, DeviceArray
 
@@ -93,7 +95,7 @@ class _Engine(object):
             self.handle = None
 
 
-class R_MADDPG(MaddpgLearnerState):
+class R_MADDPG(MaddpgLearnerState, DeviceNoise):
     def __init__(self, args, num_agents, policies, policy_mapping_fn, device=None, episode_length=None, actor_update_interval=1):
         self.args = args
         self.use_per = args.use_per
@@ -170,11 +172,32 @@ class R_MADDPG(MaddpgLearnerState):
         e = self._eng[p_id or self.policy_ids[0]]
         return sample_gumbel((self.episode_length, e.n_agents * B, e.pol.act_dim))
 
+    @property
+    def _noise_steps(self):
+        return self.episode_length + 1
+
+    def _noise_cols(self, p_id):
+        return self._eng[p_id].pol.act_dim
+
+    def _noise_draws(self, B, p_id, which, buf):
+        """Device mode: the torch call of draw_target_noise / draw_actor_noise as a fill into [b][t][n][Ac]."""
+        e = self._eng[p_id]
+        T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
+        ld = (N * Ac, Ac, (T + 1) * N * Ac)
+        if which == "target":
+            kind = capi.TRNG_GUMBEL if e.pol.discrete else capi.TRNG_NORMAL
+            return [draw(kind, T + 1, N, B, Ac, buf, 0, *ld, std=float(e.pol.target_noise or 0.0))]
+        return [draw(capi.TRNG_GUMBEL, T, N, B, Ac, buf, 0, *ld)]
+
     def _target_noise(self, B, p_id=None):
         """N(0, target_noise) / Gumbel draws for every target action, in batch row order on the device."""
         e = self._eng[p_id or self.policy_ids[0]]
         if not e.pol.td3:
             return None
+        if self.noise_gen is not None:
+            e.noise_dev = self._device_noise(B, p_id or self.policy_ids[0], "target")
+            self._noise_dev = e.noise_dev
+            return e.noise_dev
         T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
         noise = self.draw_target_noise(B, p_id)
         ours = noise.view(T + 1, N, B, Ac).permute(2, 0, 1, 3).contiguous()                      # -> [b][t][n][Ac]
@@ -185,6 +208,10 @@ class R_MADDPG(MaddpgLearnerState):
     def _actor_noise(self, B, p_id=None):
         """Gumbel draws of the actor update's `get_actions(..., use_gumbel=True)` over obs[:-1] (r_maddpg.py:277), padded to T+1 steps."""
         e = self._eng[p_id or self.policy_ids[0]]
+        if self.noise_gen is not None:
+            e.actor_noise_dev = self._device_noise(B, p_id or self.policy_ids[0], "actor")
+            self._actor_noise_dev = e.actor_noise_dev
+            return e.actor_noise_dev
         T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
         g = self.draw_actor_noise(B, p_id)
         ours = torch.zeros(B, T + 1, N, Ac)
