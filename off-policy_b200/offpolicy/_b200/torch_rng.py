@@ -3,8 +3,8 @@
 The reference draws the noise of every MADDPG / MATD3 / R-MADDPG / R-MATD3 update from torch's CPU generator: the Gumbel draws of
 the actor update and of MATD3's target actions (`sample_gumbel`, utils/util.py:127-130) and MATD3's N(0, std) target-action noise
 (util.py:217-218).  `DeviceTorchGenerator` holds a copy of that generator in device memory; a trainer switched to it with
-`trainer.use_device_noise(gen)` makes each of those torch calls as one fill on the device, written straight into the learner's noise
-layout, so an update (or a captured whole-update graph) needs no host draw and no copy.
+`trainer.use_device_noise(gen)` (offpolicy/_b200/maddpg_trainer.py) makes each of those torch calls as one fill on the device, written
+straight into the learner's noise layout, so an update (or a captured whole-update graph) needs no host draw and no copy.
 
 The fills consume exactly the words torch's calls would, and their uniforms are bit-identical to torch's.  The Gumbel and normal
 transforms agree with torch's to a few ulps, not bit for bit (torch's vectorised log / sin / cos differ from the device's in the last
@@ -103,31 +103,3 @@ def draw(kind, T, rows_n, rows_b, cols, dst, col, ld_t, ld_n, ld_b, std=0.0):
     return capi.TrngDraw(kind, int(T), int(rows_n), int(rows_b), int(cols), float(std), dst.data_ptr() + 4 * int(col), int(ld_t), int(ld_n),
                          int(ld_b))
 
-
-class DeviceNoise(object):
-    """Mixin of the MADDPG-family trainers: the device noise mode.  The trainer supplies `_noise_draws(B, p_id, which, buf)` (the torch
-    calls of its target ('target') or actor ('actor') noise, in the reference's order, into `buf`) and `_noise_steps` (the step axis of
-    its noise layout [B][steps][N][A])."""
-
-    noise_gen = None
-
-    def use_device_noise(self, gen):
-        """Draw every update's noise from `gen` (a DeviceTorchGenerator) on the device instead of from torch's CPU generator; None
-        goes back to the host draws."""
-        self.noise_gen = gen
-        self._noise_bufs = {}
-
-    def _noise_buffer(self, p_id, which, B):
-        """The fixed device buffer a policy's draws land in, zero outside the draws (the host path's padding)."""
-        key = (p_id, which, B)
-        if key not in self._noise_bufs:
-            e = self._eng[p_id]
-            self._noise_bufs[key] = torch.zeros(B, self._noise_steps, e.n_agents, self._noise_cols(p_id), dtype=torch.float32,
-                                                device=self.dev)
-        return self._noise_bufs[key]
-
-    def _device_noise(self, B, p_id, which):
-        buf = self._noise_buffer(p_id, which, B)
-        for d in self._noise_draws(B, p_id, which, buf):
-            self.noise_gen.fill(d)
-        return buf

@@ -102,6 +102,8 @@ def _init_net(mod, in_dim, hidden, out_specs, gain, use_orthogonal, use_relu=Tru
 
 
 class R_MADDPGPolicy(object):
+    act_segs = None             # one action block (MultiDiscrete is not built)
+
     def __init__(self, config, policy_config, target_noise=None, td3=False, train=True):
         self.config = config
         self.device = config["device"]

@@ -8,16 +8,13 @@ Discrete actors the Gumbel draws of the target actions (MATD3) and of the actor 
 drawn the same way (utils/util.py:127-130), in the reference's order.  `use_device_noise(gen)` makes the same draws on the device instead
 (offpolicy/_b200/torch_rng.py).
 `cent_train_policy_on_batch` (per-agent centralised observations) is unusable in the reference (SURVEY.md App. D-7) and is not built."""
-import ctypes as C
-
 import numpy as np
 import torch
 
 from offpolicy._b200 import capi
-from offpolicy._b200.maddpg_state import MaddpgLearnerState
-from offpolicy._b200.torch_rng import DeviceNoise, draw
+from offpolicy._b200.maddpg_trainer import MaddpgTrainer
 from offpolicy.algorithms.r_maddpg.algorithm.rMADDPGPolicy import maddpg_cfg_struct, sample_gumbel
-from offpolicy.utils.rec_buffer import SampledBatch, DeviceArray
+from offpolicy.utils.rec_buffer import SampledBatch
 
 
 class _HostBatchC(object):
@@ -62,90 +59,21 @@ class _HostBatchC(object):
         return b
 
 
-class _Engine(object):
-    """One policy's learner: its mx_maddpg handle + workspace views."""
+class R_MADDPG(MaddpgTrainer):
+    _popart_msg = "B200 R-MADDPG path: --use_popart is not implemented (the reference's PopArt target is used only there)"
+    _cent_msg = "cent_train_policy_on_batch is unusable in the reference (missing train_info['update_actor']) and is not built"
+    _idx_field = 8
 
-    def __init__(self, args, pol, n_agents, episode_length, max_batch, actor_update_interval, cent_act_dim, act_offset):
-        lib = capi.lib()
-        self.dev = capi.device()
-        self.pol, self.n_agents = pol, n_agents
-        self.cfg = maddpg_cfg_struct(args, n_agents, pol.obs_dim, pol.act_dim, pol.central_obs_dim, episode_length, max_batch,
-                                     pol.td3, pol.target_noise if pol.td3 else 0.0, actor_update_interval, pol.discrete,
-                                     cent_act_dim=cent_act_dim, act_offset=act_offset)
-        nbytes = int(lib.mx_maddpg_workspace_bytes(C.byref(self.cfg)))
-        if nbytes < 0:
-            raise capi.MxError(lib.mx_last_error().decode())
-        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=self.dev)
-        av = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.actor_vecs])
-        cv = (C.c_void_p * 4)(*[v.data_ptr() for v in pol.critic_vecs])
-        h = C.c_void_p()
-        capi.check(lib.mx_maddpg_create(C.byref(self.cfg), av, cv, capi.ptr(self.workspace), nbytes, C.byref(h)))
-        self.handle = h
-        ip = lib.mx_maddpg_info(self.handle) - self.workspace.data_ptr()
-        self.info = self.workspace[ip:ip + 32].view(torch.float32)
-        pp = lib.mx_maddpg_priorities(self.handle) - self.workspace.data_ptr()
-        self.prio = self.workspace[pp:pp + 4 * max_batch].view(torch.float32)
-        self.host_batch = None
-        self.noise_dev = None
-        self.actor_noise_dev = None
-
-    def close(self):
-        if self.handle:
-            capi.lib().mx_maddpg_destroy(self.handle)
-            self.handle = None
-
-
-class R_MADDPG(MaddpgLearnerState, DeviceNoise):
     def __init__(self, args, num_agents, policies, policy_mapping_fn, device=None, episode_length=None, actor_update_interval=1):
-        self.args = args
-        self.use_per = args.use_per
-        if getattr(args, "use_popart", False):
-            raise NotImplementedError("B200 R-MADDPG path: --use_popart is not implemented (the reference's PopArt target is used only there)")
-        self.num_agents = num_agents
-        self.policies = policies
-        self.policy_mapping_fn = policy_mapping_fn
-        self.policy_ids = sorted(list(self.policies.keys()))
-        self.policy_agents = {p: sorted(a for a in range(num_agents) if policy_mapping_fn(a) == p) for p in self.policies}
-        self.episode_length = args.episode_length if episode_length is None else episode_length
-        self.actor_update_interval = actor_update_interval
-        self.num_updates = {p: 0 for p in self.policy_ids}
-        self.use_same_share_obs = getattr(args, "use_same_share_obs", True)
-        self.max_batch = int(getattr(args, "batch_size", 32))
-        self.dev = capi.device()
-        # one shared policy ('policy_0' for every agent): the single-learner layout; several policies (config.py:61 share_policy False,
-        # train/train_mpe.py:139-150): one learner per policy, the centralised action vector is ordered like r_maddpg.py:62-105 walks
-        # the policies (sorted ids, each policy's agents in order)
-        self.multi = len(self.policy_ids) > 1
-        self._eng = {}
-        off = 0
-        total = sum(len(self.policy_agents[p]) * self.policies[p].act_dim for p in self.policy_ids)
-        for p in self.policy_ids:
-            pol, n_p = self.policies[p], len(self.policy_agents[p])
-            if self.multi and pol.central_act_dim != total:
-                raise ValueError("policy %s: cent_act_dim %d != total action width %d of all agents" % (p, pol.central_act_dim, total))
-            self._eng[p] = _Engine(args, pol, n_p, self.episode_length, self.max_batch, actor_update_interval,
-                                   total if self.multi else 0, off if self.multi else 0)
-            pol._trainer, pol._handle = self, self._eng[p].handle
-            off += n_p * pol.act_dim
-        first = self._eng[self.policy_ids[0]]
-        # single-policy attributes kept for the graph helpers / tests
-        self.cfg, self.workspace, self.handle, self._info, self._prio = first.cfg, first.workspace, first.handle, first.info, first.prio
+        self.episode_length = T = args.episode_length if episode_length is None else episode_length
+        # noise rows [B][T+1][N][A]: the target actions' draws cover every step, the actor update's obs[:-1]
+        self.noise_steps, self.noise_rows = T + 1, {"target": (0, T + 1), "actor": (0, T)}
+        MaddpgTrainer.__init__(self, args, num_agents, policies, policy_mapping_fn, device, actor_update_interval)
 
-    def __del__(self):
-        try:
-            for e in getattr(self, "_eng", {}).values():
-                e.close()
-            self.handle = None
-        except Exception:
-            pass
-
-    def grad_views(self, p_id=None):
-        """Numerator gradients (actor, critic) as flat views, for the parity tests."""
-        e = self._eng[p_id or self.policy_ids[0]]
-        a, c = C.c_int64(), C.c_int64()
-        capi.lib().mx_maddpg_grad_views(e.handle, C.byref(a), C.byref(c))
-        return (e.workspace[a.value:a.value + 4 * (e.pol.Pa + 4)].view(torch.float32),
-                e.workspace[c.value:c.value + 4 * (e.pol.Pc + 4)].view(torch.float32))
+    def _cfg(self, pol, n_agents, cent_act_dim, act_offset):
+        return maddpg_cfg_struct(self.args, n_agents, pol.obs_dim, pol.act_dim, pol.central_obs_dim, self.episode_length, self.max_batch,
+                                 pol.td3, pol.target_noise if pol.td3 else 0.0, self.actor_update_interval, pol.discrete,
+                                 cent_act_dim=cent_act_dim, act_offset=act_offset)
 
     def _device_batch(self, batch, p_id="policy_0"):
         if isinstance(batch, SampledBatch):
@@ -171,97 +99,3 @@ class R_MADDPG(MaddpgLearnerState, DeviceNoise):
         """Gumbel draws of the actor update's `get_actions(..., use_gumbel=True)` over obs[:-1] (r_maddpg.py:277): (T, N_p*B, Ac)."""
         e = self._eng[p_id or self.policy_ids[0]]
         return sample_gumbel((self.episode_length, e.n_agents * B, e.pol.act_dim))
-
-    @property
-    def _noise_steps(self):
-        return self.episode_length + 1
-
-    def _noise_cols(self, p_id):
-        return self._eng[p_id].pol.act_dim
-
-    def _noise_draws(self, B, p_id, which, buf):
-        """Device mode: the torch call of draw_target_noise / draw_actor_noise as a fill into [b][t][n][Ac]."""
-        e = self._eng[p_id]
-        T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
-        ld = (N * Ac, Ac, (T + 1) * N * Ac)
-        if which == "target":
-            kind = capi.TRNG_GUMBEL if e.pol.discrete else capi.TRNG_NORMAL
-            return [draw(kind, T + 1, N, B, Ac, buf, 0, *ld, std=float(e.pol.target_noise or 0.0))]
-        return [draw(capi.TRNG_GUMBEL, T, N, B, Ac, buf, 0, *ld)]
-
-    def _target_noise(self, B, p_id=None):
-        """N(0, target_noise) / Gumbel draws for every target action, in batch row order on the device."""
-        e = self._eng[p_id or self.policy_ids[0]]
-        if not e.pol.td3:
-            return None
-        if self.noise_gen is not None:
-            e.noise_dev = self._device_noise(B, p_id or self.policy_ids[0], "target")
-            self._noise_dev = e.noise_dev
-            return e.noise_dev
-        T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
-        noise = self.draw_target_noise(B, p_id)
-        ours = noise.view(T + 1, N, B, Ac).permute(2, 0, 1, 3).contiguous()                      # -> [b][t][n][Ac]
-        e.noise_dev = ours.to(self.dev, non_blocking=True)
-        self._noise_dev = e.noise_dev
-        return e.noise_dev
-
-    def _actor_noise(self, B, p_id=None):
-        """Gumbel draws of the actor update's `get_actions(..., use_gumbel=True)` over obs[:-1] (r_maddpg.py:277), padded to T+1 steps."""
-        e = self._eng[p_id or self.policy_ids[0]]
-        if self.noise_gen is not None:
-            e.actor_noise_dev = self._device_noise(B, p_id or self.policy_ids[0], "actor")
-            self._actor_noise_dev = e.actor_noise_dev
-            return e.actor_noise_dev
-        T, N, Ac = self.episode_length, e.n_agents, e.pol.act_dim
-        g = self.draw_actor_noise(B, p_id)
-        ours = torch.zeros(B, T + 1, N, Ac)
-        ours[:, :T] = g.view(T, N, B, Ac).permute(2, 0, 1, 3)
-        e.actor_noise_dev = ours.to(self.dev, non_blocking=True)
-        self._actor_noise_dev = e.actor_noise_dev
-        return e.actor_noise_dev
-
-    def train_policy_on_batch(self, update_policy_id, batch):
-        if self.use_same_share_obs:
-            return self.shared_train_policy_on_batch(update_policy_id, batch)
-        return self.cent_train_policy_on_batch(update_policy_id, batch)
-
-    def cent_train_policy_on_batch(self, update_policy_id, batch):
-        raise NotImplementedError("cent_train_policy_on_batch is unusable in the reference (missing train_info['update_actor']) and is not built")
-
-    def shared_train_policy_on_batch(self, update_policy_id, batch):
-        lib, stream = capi.lib(), capi.stream_ptr()
-        e = self._eng[update_policy_id]
-        b = self._device_batch(batch, update_policy_id)
-        if self.multi:
-            # r_maddpg.py:40-105 (get_update_info): every policy's buffer actions and TARGET-actor next actions, policy by policy in
-            # id order -- the target-noise draws (MATD3) consume torch's CPU generator in that same order
-            noise = None
-            keep = []
-            for q in self.policy_ids:
-                bq = b if q == update_policy_id else self._device_batch(batch, q)
-                nq = self._target_noise(b.B, q)
-                keep.append((bq, nq))
-                if q == update_policy_id:
-                    noise = nq
-                capi.check(lib.mx_maddpg_cent_contribute(self._eng[q].handle, C.byref(bq), capi.ptr(nq), e.handle, stream))
-            self._keep = keep
-        else:
-            noise = self._target_noise(b.B, update_policy_id)
-        will_update_actor = self.num_updates[update_policy_id] % self.actor_update_interval == 0
-        actor_noise = self._actor_noise(b.B, update_policy_id) if (e.pol.discrete and will_update_actor) else None
-        upd = C.c_int32()
-        capi.check(lib.mx_maddpg_step_ex(e.handle, C.byref(b), capi.ptr(noise), capi.ptr(actor_noise), C.byref(upd), stream))
-        info = e.info
-        train_info = {"critic_loss": info[0], "critic_grad_norm": info[1]}
-        if upd.value:
-            train_info["actor_loss"], train_info["actor_grad_norm"] = info[4], info[5]
-        train_info["update_actor"] = bool(upd.value)
-        self.num_updates[update_policy_id] += 1
-        new_priorities = DeviceArray(e.prio[:b.B]) if self.use_per else None
-        return train_info, new_priorities, batch[8]
-
-    def prep_training(self):
-        pass
-
-    def prep_rollout(self):
-        pass

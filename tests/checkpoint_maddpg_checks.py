@@ -6,7 +6,6 @@ A `Case` describes one trainer + replay configuration.  One round = insert a few
 checkpoint), sample, train every policy, write PER priorities back, soft-update; it returns what a caller can see of that round:
 sampled indices, every train_info scalar, the new priorities."""
 import contextlib
-import ctypes as C
 import os
 import tempfile
 
@@ -262,9 +261,9 @@ def _info_record(case, tr, buf, upd):
 
 
 def check_graph_resume(case, k=3):
-    """As check_resume, but the restored objects run the k rounds through the captured whole-update graph (R_MADDPG / R_MATD3:
-    MaddpgStepGraph; shared MADDPG / MATD3: mx_maddpg_graph_capture), against the uninterrupted run's eager rounds.  The graph samples
-    from the device RNG and inserts nothing, so neither do the rounds after the checkpoint here."""
+    """As check_resume, but the restored objects run the k rounds through the captured whole-update graph (MaddpgStepGraph), against
+    the uninterrupted run's eager rounds.  The graph samples from the device RNG and inserts nothing, so neither do the rounds after the
+    checkpoint here."""
     assert case.rng == "device" and not case.per and len(case.specs) == 1
     tr, buf, pols, rs = _prefix(case, k)
     with tempfile.TemporaryDirectory() as d:
@@ -282,30 +281,13 @@ def check_graph_resume(case, k=3):
     got = []
     ctx, side = _stream_ctx()
     with ctx:
-        if case.kind == "rec":
-            from offpolicy._b200.graph import MaddpgStepGraph
-            g = MaddpgStepGraph(buf2, tr2, case.B)
-            for _ in range(k):
-                upd = g.launch()
-                g.synchronize()
-                got.append(_info_record(case, tr2, buf2, upd))
-            g.close()
-        else:
-            lib, B = capi.lib(), case.B
-            n, _, a = case.specs[0]
-            dev = capi.device()
-            tn, an = torch.zeros(B, 2, n, fx.act_width(a), device=dev), torch.zeros(B, 2, n, fx.act_width(a), device=dev)
-            capi.check(lib.mx_maddpg_set_valid(tr2.handle, capi.ptr(buf2.policy_buffers["policy_0"].valid_dev)))
-            g = C.c_void_p()
-            capi.check(lib.mx_maddpg_graph_capture(case.first_store(buf2).handle, tr2.handle, B, 0.0, 1 | 4, capi.ptr(tn), capi.ptr(an), 1,
-                                                   capi.stream_ptr(), C.byref(g)))
-            for _ in range(k):
-                for dst, draw, step in ((tn, tr2.draw_target_noise(B), 1), (an, tr2.draw_actor_noise(B), 0)):
-                    if draw is not None:
-                        dst.copy_(tr2._rows(draw, B, step))
-                capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
-                got.append(_info_record(case, tr2, buf2, True))
-            lib.mx_graph_destroy(g)
+        from offpolicy._b200.graph import MaddpgStepGraph
+        g = MaddpgStepGraph(buf2, tr2, case.B)
+        for _ in range(k):
+            upd = g.launch()
+            g.synchronize()
+            got.append(_info_record(case, tr2, buf2, upd))
+        g.close()
     assert_same(got, want, "rounds")
     assert_same(snapshot(tr2, buf2), want_snap)
 

@@ -143,16 +143,13 @@ def check_layout(case, B=None):
     torch.manual_seed(31)
     host = {}
     for q, which in _draw_plan(tr):
-        if case.kind == "rec":
-            host[(q, which)] = (tr._target_noise if which == "target" else tr._actor_noise)(B, q).cpu().clone()
-        else:
-            host[(q, which)] = tr._noise(B, q, which).cpu().clone()
+        host[(q, which)] = tr._noise(B, q, which).cpu().clone()
     want_state = torch.get_rng_state().clone()
     torch.manual_seed(31)
     gen = DeviceTorchGenerator()
     tr.use_device_noise(gen)
     for q, which in _draw_plan(tr):
-        got = tr._device_noise(B, q, which)
+        got = tr._noise(B, q, which)
         _sync()
         got, want = got.cpu(), host[(q, which)]
         assert got.shape == want.shape, (q, which)
@@ -165,13 +162,11 @@ def check_layout(case, B=None):
 def _feed_device_values(tr, gen2):
     """Host-mode trainer whose draw_target_noise / draw_actor_noise return what gen2 (a twin of the device-mode generator) draws, in
     torch's layout: the host path then permutes and copies them in."""
-    dummy = torch.zeros(1, device=capi.device())
 
     def values(B, p_id, which):
-        ds = tr._noise_draws(B, p_id, which, dummy)
+        ds = tr._noise_draws(B, p_id, which)
         parts = [torch_layout(d.kind, d.T, d.rows_n, d.rows_b, d.cols, d.std, gen=gen2) for d in ds]
-        x = torch.cat(parts, -1)
-        return x[0] if not hasattr(tr, "episode_length") else x
+        return torch.cat(parts, -1)
 
     orig_t, orig_a = tr.draw_target_noise, tr.draw_actor_noise
 
@@ -246,8 +241,6 @@ def check_graph(case, n=4):
                     r = case.round(tr, buf, pols, None, insert=False)
                     rec.append((r[0], dict(r[1])["critic_loss"], dict(r[1])["update_actor"]))
             else:
-                if case.kind == "mlp":
-                    capi.check(capi.lib().mx_maddpg_set_valid(tr.handle, capi.ptr(buf.policy_buffers["policy_0"].valid_dev)))
                 g = MaddpgStepGraph(buf, tr, case.B)
                 for _ in range(n):
                     upd = g.launch()

@@ -1,7 +1,6 @@
 """Transition-level MADDPG / MATD3 on the real sm_90a kernels: lock-step against oracle/maddpg_mlp.py at small and at
 scripts/train_mpe_maddpg.sh sizes (B = 1000 drawn from a replay of 100 000 transitions), and the captured whole-update graph against
 eager steps."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -80,10 +79,10 @@ def test_lockstep_train_mpe_maddpg_sizes(gpu_engine, discrete, td3):
 
 @pytest.mark.parametrize("discrete,td3", [(True, False), (True, True), (False, False), (False, True)])
 def test_graph_replay_equals_eager(gpu_engine, discrete, td3):
-    """mx_maddpg_graph_capture (device uniform sample -> step -> soft update) replayed = the same updates run eagerly, bit for bit."""
-    from offpolicy._b200 import capi
+    """MaddpgStepGraph (device uniform sample -> step -> soft update) replayed = the same updates run eagerly, bit for bit."""
     from offpolicy._b200.factory import build_mlp_maddpg
-    B, lib = 256, capi.lib()
+    from offpolicy._b200.graph import MaddpgStepGraph
+    B = 256
     runs = []
     side = torch.cuda.Stream()                 # a capture needs a non-default stream; eager steps run on the same one
     for mode in ("eager", "graph"):
@@ -92,14 +91,8 @@ def test_graph_replay_equals_eager(gpu_engine, discrete, td3):
             args, pol, tr = build_mlp_maddpg(N, O, A, S, B, discrete=discrete, td3=td3)
             buf = _filled_buffer(B, 4096, discrete, 22)
             buf.seed_device_rng(23)
-            rep = buf.policy_buffers["policy_0"].rep
-            capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(buf.policy_buffers["policy_0"].valid_dev)))
-            tn_buf = torch.zeros(B, 2, N, A, device="cuda")
-            an_buf = torch.zeros(B, 2, N, A, device="cuda")
-            g = C.c_void_p()
             if mode == "graph":
-                capi.check(lib.mx_maddpg_graph_capture(rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn_buf), capi.ptr(an_buf), 1,
-                                                       capi.stream_ptr(), C.byref(g)))
+                g = MaddpgStepGraph(buf, tr, B)
             infos = []
             for k in range(3):
                 torch.manual_seed(100 + k)
@@ -108,10 +101,7 @@ def test_graph_replay_equals_eager(gpu_engine, discrete, td3):
                     info, _, _ = tr.shared_train_policy_on_batch("policy_0", batch)
                     pol.soft_target_updates()
                 else:
-                    for dst, draw, step in ((tn_buf, tr.draw_target_noise(B), 1), (an_buf, tr.draw_actor_noise(B), 0)):
-                        if draw is not None:
-                            dst.copy_(tr._rows(draw, B, step))
-                    capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
+                    g.launch()
                     info = tr._info
                 torch.cuda.synchronize()
                 infos.append([float(info[i]) for i in ("critic_loss", "critic_grad_norm", "actor_loss", "actor_grad_norm")] if mode == "eager"

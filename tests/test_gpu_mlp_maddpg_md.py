@@ -1,7 +1,6 @@
 """Transition-level MADDPG / MATD3 with MultiDiscrete action spaces on the real sm_90a kernels: the fixtures of the unmodified reference,
 lock-step against oracle/maddpg_mlp_md.py at small sizes and at simple_reference shapes (B = 1000 drawn from a replay of 100 000
 transitions), and the captured whole-update graph of a shared MultiDiscrete learner against eager steps."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -76,11 +75,11 @@ def test_lockstep_simple_reference_sizes(gpu_engine, td3):
 
 @pytest.mark.parametrize("td3", [False, True])
 def test_graph_replay_equals_eager(gpu_engine, td3):
-    """mx_maddpg_graph_capture (device uniform sample -> step -> soft update) of a shared MultiDiscrete learner replayed = the same
+    """MaddpgStepGraph (device uniform sample -> step -> soft update) of a shared MultiDiscrete learner replayed = the same
     updates run eagerly, bit for bit."""
-    from offpolicy._b200 import capi
     from offpolicy._b200.factory import build_mlp_maddpg
-    B, lib, A = 256, capi.lib(), sum(SEGS)
+    from offpolicy._b200.graph import MaddpgStepGraph
+    B = 256
     runs = []
     side = torch.cuda.Stream()                 # a capture needs a non-default stream; eager steps run on the same one
     for mode in ("eager", "graph"):
@@ -89,14 +88,8 @@ def test_graph_replay_equals_eager(gpu_engine, td3):
             args, pol, tr = build_mlp_maddpg(N, O, SEGS, S, B, td3=td3)
             buf = _filled_buffer(B, 4096, 22)
             buf.seed_device_rng(23)
-            rep = buf.policy_buffers["policy_0"].rep
-            capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(buf.policy_buffers["policy_0"].valid_dev)))
-            tn_buf = torch.zeros(B, 2, N, A, device="cuda")
-            an_buf = torch.zeros(B, 2, N, A, device="cuda")
-            g = C.c_void_p()
             if mode == "graph":
-                capi.check(lib.mx_maddpg_graph_capture(rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn_buf), capi.ptr(an_buf), 1,
-                                                       capi.stream_ptr(), C.byref(g)))
+                g = MaddpgStepGraph(buf, tr, B)
             infos = []
             for k in range(3):
                 torch.manual_seed(100 + k)
@@ -106,10 +99,7 @@ def test_graph_replay_equals_eager(gpu_engine, td3):
                     torch.cuda.synchronize()
                     infos.append([float(info[i]) for i in ("critic_loss", "critic_grad_norm", "actor_loss", "actor_grad_norm")])
                 else:
-                    for dst, draw, step in ((tn_buf, tr.draw_target_noise(B), 1), (an_buf, tr.draw_actor_noise(B), 0)):
-                        if draw is not None:
-                            dst.copy_(tr._rows(draw, B, step))
-                    capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
+                    g.launch()
                     torch.cuda.synchronize()
                     infos.append([float(tr._info[i]) for i in (0, 1, 4, 5)])
             runs.append((infos, [v.clone() for v in pol.actor_vecs + pol.critic_vecs]))

@@ -1,6 +1,6 @@
-"""Grad-steps/s of the MADDPG-family whole-update graphs with the update noise drawn on the host (torch's CPU generator, permuted and
-copied in before every replay) against drawn on the device (trainer.use_device_noise: the fills at the head of the graph, one launch
-per update).  Shapes:
+"""Grad-steps/s of the MADDPG-family whole-update graphs (MaddpgStepGraph) with the update noise drawn on the host (torch's CPU
+generator, placed in the graph's pinned staging ring and copied in before every replay) against drawn on the device
+(trainer.use_device_noise: the fills at the head of the graph, one launch per update).  Shapes:
 
     maddpg_spread / matd3_spread        MLP MADDPG / MATD3, simple_spread (3 agents, obs 18, Discrete(5), shared observation 54)
     maddpg_reference / matd3_reference  MLP MADDPG / MATD3, simple_reference (2 agents, obs 21, MultiDiscrete 5 + 10, shared obs 42)
@@ -16,7 +16,6 @@ limit and maximum SM clock read in the same call.  Needs a CUDA device.
 """
 import argparse
 import contextlib
-import ctypes as C
 import json
 import os
 import subprocess
@@ -56,44 +55,17 @@ def timed(one, steps, warmup):
     return steps / (time.perf_counter() - t0)
 
 
-def host_arm(case, tr, buf):
-    """The whole-update graph replayed after the host draws and copies the noise in (MaddpgStepGraph; for the MLP trainer the same
-    sequence as tools/bench_mlp_maddpg.py)."""
-    from offpolicy._b200 import capi
+def graph_arm(tr, buf, B):
+    """The whole-update graph (MaddpgStepGraph): in host noise mode the host draws the noise and copies it in through the graph's
+    pinned ring before every replay; in device noise mode the fills run at the head of the graph."""
     from offpolicy._b200.graph import MaddpgStepGraph
-    if case.kind == "rec":
-        g = MaddpgStepGraph(buf, tr, case.B)
-        return g.launch, g
-    lib, B = capi.lib(), case.B
-    pb = buf.policy_buffers["policy_0"]
-    capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(pb.valid_dev)))
-    n, A = tr._eng["policy_0"].n_agents, tr._eng["policy_0"].pol.output_dim
-    tn, an = torch.zeros(B, 2, n, A, device="cuda"), torch.zeros(B, 2, n, A, device="cuda")
-    g = C.c_void_p()
-    capi.check(lib.mx_maddpg_graph_capture(pb.rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn), capi.ptr(an), 1, capi.stream_ptr(), C.byref(g)))
-
-    def one():
-        for dst, d, step in ((tn, tr.draw_target_noise(B), 1), (an, tr.draw_actor_noise(B), 0)):
-            if d is not None:
-                dst.copy_(tr._rows(d, B, step))
-        capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
-    return one, (tn, an, g)
-
-
-def device_arm(case, tr, buf):
-    from offpolicy._b200 import capi
-    from offpolicy._b200.graph import MaddpgStepGraph
-    if case.kind == "mlp":
-        capi.check(capi.lib().mx_maddpg_set_valid(tr.handle, capi.ptr(buf.policy_buffers["policy_0"].valid_dev)))
-    g = MaddpgStepGraph(buf, tr, case.B)
+    g = MaddpgStepGraph(buf, tr, B)
     return g.launch, g
 
 
 def fill_ms(tr, B, reps):
     """Device time of one update's fills (every draw of an actor-updating update), from CUDA events; and the MT19937 words they use."""
-    pol = tr._eng["policy_0"].pol
-    draws = (tr._noise_draws(B, "policy_0", "target", tr._noise_buffer("policy_0", "target", B)) if pol.td3 else []) + \
-            (tr._noise_draws(B, "policy_0", "actor", tr._noise_buffer("policy_0", "actor", B)) if pol.discrete else [])
+    draws = tr._noise_draws(B, "policy_0", "target") + tr._noise_draws(B, "policy_0", "actor")
     gen = tr.noise_gen
     for d in draws:
         gen.fill(d)
@@ -133,7 +105,7 @@ def main():
             case.fill(buf, np.random.RandomState(2), case.E)
             tr_d, _, _ = case.build(1)
             tr_d.use_device_noise(DeviceTorchGenerator(seed=3))
-            arms = {"host": host_arm(case, tr_h, buf), "device": device_arm(case, tr_d, buf)}
+            arms = {"host": graph_arm(tr_h, buf, case.B), "device": graph_arm(tr_d, buf, case.B)}
             rates = {"host": [], "device": []}
             for _ in range(a.reps):
                 for arm in ("host", "device"):

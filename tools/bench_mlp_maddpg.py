@@ -3,8 +3,9 @@ obs 18, Discrete(5), shared observation 54), B = 1 000 transitions drawn from a 
 scripts/train_mpe_matd3.sh instead: simple_reference (2 agents, obs 21, shared observation 42, MultiDiscrete actions of sub-spaces 5 and
 10).
 
-GPU arm: the whole-update CUDA graph (device uniform draw + gather -> mx_maddpg step -> soft target update), the per-update noise drawn
-on the host from torch's CPU generator exactly as the reference draws it and copied into the graph's fixed buffers before each replay;
+GPU arm: the whole-update CUDA graph (MaddpgStepGraph: device uniform draw + gather -> mx_maddpg step -> soft target update), the
+per-update noise drawn on the host from torch's CPU generator exactly as the reference draws it and copied into the graph's fixed
+buffers through its pinned staging ring before each replay;
 timed over `--steps` replays after `--warmup`, ending in a device synchronise.  CPU arm: oracle/maddpg_mlp.py (the reference's
 update restated in eager PyTorch) on the same host and shapes, with its thread count and the host's core count.
 Prints one JSON line per algorithm.  Needs a CUDA device; it never falls back to the CPU for the GPU arm.
@@ -13,7 +14,6 @@ Prints one JSON line per algorithm.  Needs a CUDA device; it never falls back to
     python tools/bench_mlp_maddpg.py --shape reference --steps 500 --warmup 50
 """
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -55,10 +55,9 @@ def fill(buf, B, size, rng):
 
 
 def gpu_arm(td3, B, size, steps, warmup):
-    from offpolicy._b200 import capi
     from offpolicy._b200.factory import build_mlp_maddpg, act_space, Box
+    from offpolicy._b200.graph import MaddpgStepGraph
     from offpolicy.utils.mlp_buffer import MlpReplayBuffer
-    lib = capi.lib()
     side = torch.cuda.Stream()
     with torch.cuda.stream(side):
         torch.manual_seed(1)
@@ -68,24 +67,13 @@ def gpu_arm(td3, B, size, steps, warmup):
         buf = MlpReplayBuffer(info, {"policy_0": list(range(N))}, size, True, False, max_batch=B)
         fill(buf, B, size, np.random.default_rng(2))
         buf.seed_device_rng(3)
-        pb = buf.policy_buffers["policy_0"]
-        capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(pb.valid_dev)))
-        tn, an = torch.zeros(B, 2, N, A, device="cuda"), torch.zeros(B, 2, N, A, device="cuda")
-        g = C.c_void_p()
-        capi.check(lib.mx_maddpg_graph_capture(pb.rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn), capi.ptr(an), 1, capi.stream_ptr(),
-                                               C.byref(g)))
-
-        def one():
-            for dst, draw, step in ((tn, tr.draw_target_noise(B), 1), (an, tr.draw_actor_noise(B), 0)):
-                if draw is not None:
-                    dst.copy_(tr._rows(draw, B, step))
-            capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
+        g = MaddpgStepGraph(buf, tr, B)
         for _ in range(warmup):
-            one()
+            g.launch()
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         for _ in range(steps):
-            one()
+            g.launch()
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
         loss = float(tr._info[0])
@@ -138,7 +126,7 @@ def main():
         cpu = cpu_arm(td3, a.batch, a.cpu_steps)
         rec = {"metric": "grad-steps/s", "algo": algo, "value": rate, "unit": "steps/s", "batch": a.batch, "buffer": a.buffer,
                "steps": a.steps, "warmup": a.warmup, "path": "CUDA graph: device draw + gather + mx_maddpg step (mlp) + soft update; "
-               "host noise draws copied in per step", "last_critic_loss": loss, "gpu": q,
+               "host noise draws copied in per step through a pinned ring", "last_critic_loss": loss, "gpu": q,
                "cpu_oracle": {"value": cpu, "unit": "steps/s", "torch_threads": torch.get_num_threads(), "host_cores": os.cpu_count(),
                               "steps": a.cpu_steps, "kind": "oracle/maddpg_mlp.py (eager PyTorch restatement of the reference update)"},
                "speedup_vs_cpu_oracle": rate / cpu}

@@ -1,12 +1,11 @@
 """Where the time of a tools/bench_mlp_maddpg.py update goes, for both shapes (simple_spread, simple_reference) and both algorithms,
 alternating the shapes and repeating three times in one process: `graph_ms` is the captured whole-update graph replayed alone (noise
-buffers left as they are), `host_ms` the host noise draws from torch's CPU generator and their copies alone, `full_ms` both, as the
-benchmark runs them.  Then a per-kernel breakdown of eager MADDPG steps under torch.profiler (a separate, traced run).  Needs a CUDA
-device; prints JSON lines.
+buffers left as they are), `host_ms` the host noise draws from torch's CPU generator and their copies through the graph's pinned ring
+alone, `full_ms` both (MaddpgStepGraph.launch), as the benchmark runs them.  Then a per-kernel breakdown of eager MADDPG steps under
+torch.profiler (a separate, traced run).  Needs a CUDA device; prints JSON lines.
 
     python tools/bench_mlp_maddpg_split.py
 """
-import ctypes as C
 import json
 import os
 import sys
@@ -21,10 +20,9 @@ import bench_mlp_maddpg as bm
 
 def setup(shape, td3, B=1000, size=500_000):
     bm.set_shape(shape)
-    from offpolicy._b200 import capi
     from offpolicy._b200.factory import build_mlp_maddpg, act_space, Box
+    from offpolicy._b200.graph import MaddpgStepGraph
     from offpolicy.utils.mlp_buffer import MlpReplayBuffer
-    lib = capi.lib()
     torch.manual_seed(1)
     act = bm.A if bm.SEGS is None else bm.SEGS
     args, pol, tr = build_mlp_maddpg(bm.N, bm.O, act, bm.S, B, discrete=True, td3=td3)
@@ -32,12 +30,7 @@ def setup(shape, td3, B=1000, size=500_000):
     buf = MlpReplayBuffer(info, {"policy_0": list(range(bm.N))}, size, True, False, max_batch=B)
     bm.fill(buf, B, size, np.random.default_rng(2))
     buf.seed_device_rng(3)
-    pb = buf.policy_buffers["policy_0"]
-    capi.check(lib.mx_maddpg_set_valid(tr.handle, capi.ptr(pb.valid_dev)))
-    tn, an = torch.zeros(B, 2, bm.N, bm.A, device="cuda"), torch.zeros(B, 2, bm.N, bm.A, device="cuda")
-    g = C.c_void_p()
-    capi.check(lib.mx_maddpg_graph_capture(pb.rep.handle, tr.handle, B, 0.0, 1 | 4, capi.ptr(tn), capi.ptr(an), 1, capi.stream_ptr(), C.byref(g)))
-    return lib, capi, tr, tn, an, g, buf
+    return tr, MaddpgStepGraph(buf, tr, B), buf
 
 
 def timed(fn, n):
@@ -52,6 +45,7 @@ def timed(fn, n):
 def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_mlp_maddpg_split: needs a CUDA device")
+    from offpolicy._b200 import capi
     B = 1000
     side = torch.cuda.Stream()
     with torch.cuda.stream(side):
@@ -64,26 +58,19 @@ def main():
         for rep in range(3):
             for shape in ("spread", "reference"):
                 for td3 in (False, True):
-                    (lib, capi, tr, tn, an, g, buf), dims = ctx[(shape, td3)]
+                    (tr, g, buf), dims = ctx[(shape, td3)]
                     bm.N, bm.O, bm.A, bm.S, bm.SEGS = dims
-                    launch = lambda: capi.check(lib.mx_graph_launch(g, capi.stream_ptr()))
-
-                    def host():
-                        for dst, draw, step in ((tn, tr.draw_target_noise(B), 1), (an, tr.draw_actor_noise(B), 0)):
-                            if draw is not None:
-                                dst.copy_(tr._rows(draw, B, step))
-
-                    def full():
-                        host(); launch()
+                    launch = lambda: capi.check(g.lib.mx_graph_launch(g.graphs[1], g._sp))
+                    host = lambda: g._stage_noise(1)
                     for _ in range(50):
-                        full()
+                        g.launch()
                     r = dict(rep=rep, shape=shape, algo="matd3" if td3 else "maddpg", graph_ms=timed(launch, 500), host_ms=timed(host, 200),
-                             full_ms=timed(full, 500))
+                             full_ms=timed(g.launch, 500))
                     print(json.dumps(r), flush=True)
         # per-kernel breakdown of one replay batch each, eager step under the profiler
         from torch.profiler import profile, ProfilerActivity
         for shape in ("spread", "reference"):
-            (lib, capi, tr, tn, an, g, buf), dims = ctx[(shape, False)]
+            (tr, g, buf), dims = ctx[(shape, False)]
             bm.N, bm.O, bm.A, bm.S, bm.SEGS = dims
             for _ in range(5):
                 tr.shared_train_policy_on_batch("policy_0", buf.sample(B))
