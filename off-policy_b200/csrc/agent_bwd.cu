@@ -786,31 +786,15 @@ __global__ void __launch_bounds__(MX_TILE_THREADS, 2) k_gru_wgrad(FrontBwdArgs a
 // =====================================================================================================
 // launchers
 // =====================================================================================================
-template <int APL>
-static int qhead_bwd_launch(const QHeadBwdArgs& a, int grid, cudaStream_t s) {
-  const size_t smem = qhead_bwd_smem(a.A, APL);
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > 48 * 1024 && smem > configured) {
-    if (cudaFuncSetAttribute(k_qhead_bwd<APL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("qhead_bwd: smem %zu too large", smem); return 1; }
-    configured = smem;
-  }
-#endif
-  MX_LAUNCH_PDL(k_qhead_bwd<APL>, dim3(grid), dim3(256), smem, s, a);
-  return 0;
-}
-
 int mx_launch_qhead_bwd(const QHeadBwdArgs& a, int* nparts_used, cudaStream_t s) {
   if (a.A > 64) { mx_set_error("qhead_bwd: act_dim %d > 64 unsupported", a.A); return 1; }
   int grid = mx_ceil_div(a.M, 8 * 4);   // ~4 rows per warp
   const int cap = mx_num_sms();
   if (grid > cap) grid = cap;
   if (grid < 1) grid = 1;
-  if (a.A > 32 ? qhead_bwd_launch<2>(a, grid, s) : qhead_bwd_launch<1>(a, grid, s)) return 1;
-  MX_COUNT();
-  MX_MARK("k_qhead_bwd", s);
+  const int apl = a.A > 32 ? 2 : 1;
   *nparts_used = grid;
-  return MX_CHECK_LAUNCH("qhead_bwd");
+  return mx_launch("k_qhead_bwd", apl == 2 ? k_qhead_bwd<2> : k_qhead_bwd<1>, dim3(grid), dim3(256), qhead_bwd_smem(a.A, apl), s, MX_STEP, a);
 }
 
 // MLP variant: gradient w.r.t. the "gi" rows = the Q-head outputs: only the taken action of the step-0 rows receives dL/dq
@@ -835,10 +819,7 @@ int mx_launch_mlp_dgi(const float* dq_taken, const int32_t* act_idx, int ld_tn, 
   int grid = (int)((total + 255) / 256);
   const int cap = mx_num_sms() * 8;
   if (grid > cap) grid = cap;
-  MX_LAUNCH_PDL(k_mlp_dgi, dim3(grid), dim3(256), 0, s, dq_taken, act_idx, ld_tn, dgi, B, N);
-  MX_COUNT();
-  MX_MARK("k_mlp_dgi", s);
-  return MX_CHECK_LAUNCH("mlp_dgi");
+  return mx_launch("k_mlp_dgi", k_mlp_dgi, dim3(grid), dim3(256), 0, s, MX_STEP, dq_taken, act_idx, ld_tn, dgi, B, N);
 }
 
 int mx_launch_gru_bwd(const GruBwdArgs& a, cudaStream_t s) {
@@ -846,19 +827,9 @@ int mx_launch_gru_bwd(const GruBwdArgs& a, cudaStream_t s) {
   int rpc = 1;
   while (rpc < 4 && mx_ceil_div(a.R, rpc) > 2 * sms) rpc *= 2;
   // sequences: the 128-thread kernel, one row per CTA (r02 sweeps)
-  if (a.T >= 8) {
-    MX_LAUNCH_PDL(k_gru_bwd2<1>, dim3(a.R), dim3(BWD2_THREADS), 0, s, a);
-    MX_COUNT();
-    MX_MARK("k_gru_bwd", s);
-    return MX_CHECK_LAUNCH("gru_bwd2");
-  }
-  dim3 grid(mx_ceil_div(a.R, rpc));
-  if (rpc == 1) MX_LAUNCH_PDL(k_gru_bwd<1>, grid, dim3(BWD_THREADS), 0, s, a);
-  else if (rpc == 2) MX_LAUNCH_PDL(k_gru_bwd<2>, grid, dim3(BWD_THREADS), 0, s, a);
-  else MX_LAUNCH_PDL(k_gru_bwd<4>, grid, dim3(BWD_THREADS), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_gru_bwd", s);
-  return MX_CHECK_LAUNCH("gru_bwd");
+  if (a.T >= 8) return mx_launch("k_gru_bwd", k_gru_bwd2<1>, dim3(a.R), dim3(BWD2_THREADS), 0, s, MX_STEP, a);
+  auto kern = rpc == 1 ? k_gru_bwd<1> : rpc == 2 ? k_gru_bwd<2> : k_gru_bwd<4>;
+  return mx_launch("k_gru_bwd", kern, dim3(mx_ceil_div(a.R, rpc)), dim3(BWD_THREADS), 0, s, MX_STEP, a);
 }
 
 // Tile height: the grid is one persistent CTA per SM, so the kernel takes `waves` tile-times; pick the 16*RM rows per tile that
@@ -868,7 +839,7 @@ static int front_bwd_pick_rm(int M, int in_dim, int sms, bool gru_ext) {
   double best_cost = 1e30;
   for (int rm = 2; rm <= 4; ++rm) {
     FrontBwdSmem sm = front_bwd_smem(in_dim, 16 * rm, gru_ext);
-    if ((size_t)sm.total * sizeof(float) + 16 > 227 * 1024) continue;
+    if ((size_t)sm.total * sizeof(float) + 16 > MX_SMEM_OPTIN_MAX) continue;
     const int tiles = mx_ceil_div(M, 16 * rm);
     const double cost = (double)mx_ceil_div(tiles, sms) * (1.0 + rm);
     if (cost < best_cost - 1e-9) { best_cost = cost; best = rm; }
@@ -879,29 +850,23 @@ static int front_bwd_pick_rm(int M, int in_dim, int sms, bool gru_ext) {
 // The 32-row tile (RM 2, front_bwd_pick_rm's fallback) must fit; its input tiles are round_up(in_dim, 64) wide.
 int mx_front_bwd_max_in_dim(bool gru_ext) {
   int w = 0;
-  while ((size_t)front_bwd_smem(w + 64, 32, gru_ext).total * sizeof(float) + 16 <= 227 * 1024) w += 64;
+  while ((size_t)front_bwd_smem(w + 64, 32, gru_ext).total * sizeof(float) + 16 <= MX_SMEM_OPTIN_MAX) w += 64;
   return w;
 }
 
-template <int RM>
-static int front_bwd_launch(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s) {
-  const int TM = 16 * RM;
+static int front_bwd_launch(const FrontBwdArgs& a, int rm, int* nparts_used, cudaStream_t s) {
+  const int TM = 16 * rm;
   FrontBwdSmem sm = front_bwd_smem(a.L.in_dim, TM, a.gru_wgrad_ext != 0);
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   const int ntiles = mx_ceil_div(a.M, TM);
   int grid = mx_num_sms();
   if (grid > ntiles) grid = ntiles;
-  auto kern = k_front_bwd<RM>;
 #if !MX_EMU
-  if (smem > 227 * 1024) { mx_set_error("front_bwd: %zu bytes of shared memory needed (obs_dim too large)", smem); return 1; }
-  static size_t configured = 0;
-  if (smem > configured) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); configured = smem; }
+  if (smem > MX_SMEM_OPTIN_MAX) { mx_set_error("front_bwd: %zu bytes of shared memory needed (obs_dim too large)", smem); return 1; }
 #endif
-  MX_LAUNCH_PDL(kern, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_front_bwd", s);
+  auto kern = rm == 3 ? k_front_bwd<3> : rm == 4 ? k_front_bwd<4> : k_front_bwd<2>;
   *nparts_used = grid;
-  return MX_CHECK_LAUNCH("front_bwd");
+  return mx_launch("k_front_bwd", kern, dim3(grid), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a, sm);
 }
 
 bool mx_front_bwd_tc_usable(const FrontBwdArgs& a);
@@ -911,10 +876,7 @@ int mx_launch_front_bwd(const FrontBwdArgs& a_in, int* nparts_used, cudaStream_t
   FrontBwdArgs a = a_in;
   a.wgrad_external = mx_wgrad_tc_usable(a) ? 1 : 0;
   const int rm = front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), a.gru_wgrad_ext != 0);
-  int rc;
-  if (rm == 3) rc = front_bwd_launch<3>(a, nparts_used, s);
-  else if (rm == 4) rc = front_bwd_launch<4>(a, nparts_used, s);
-  else rc = front_bwd_launch<2>(a, nparts_used, s);
+  const int rc = front_bwd_launch(a, rm, nparts_used, s);
   if (rc || !a.wgrad_external) return rc;
   return mx_launch_wgrad_tc(a, *nparts_used, s);      // one gradient partial per k_front_bwd CTA: the same rows of gpart
 }
@@ -925,28 +887,16 @@ bool mx_gru_wgrad_split_usable(const FrontBwdArgs& a) {
   if (a.no_gru || a.skip_wgrad) return false;
   return !mx_front_bwd_tc_usable(a) && !mx_wgrad_tc_usable(a);
 }
-template <int RM>
-static int gru_wgrad_launch(const FrontBwdArgs& a, cudaStream_t s) {
-  const int TM = 16 * RM;
+// `a` must be the arguments the following mx_launch_front_bwd call gets (gru_wgrad_ext = 1): same tile height, same grid, so CTA b
+// of both kernels writes gradient partial b
+int mx_launch_gru_wgrad(const FrontBwdArgs& a, cudaStream_t s) {
+  const int rm = front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), true);
+  const int TM = 16 * rm;
   GruWgradSmem sm = gru_wgrad_smem(TM);
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   const int ntiles = mx_ceil_div(a.M, TM);
   int grid = mx_num_sms();
   if (grid > ntiles) grid = ntiles;
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > configured) { cudaFuncSetAttribute(k_gru_wgrad<RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); configured = smem; }
-#endif
-  MX_LAUNCH_PDL(k_gru_wgrad<RM>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_gru_wgrad", s);
-  return MX_CHECK_LAUNCH("gru_wgrad");
-}
-// `a` must be the arguments the following mx_launch_front_bwd call gets (gru_wgrad_ext = 1): same tile height, same grid, so CTA b
-// of both kernels writes gradient partial b
-int mx_launch_gru_wgrad(const FrontBwdArgs& a, cudaStream_t s) {
-  const int rm = front_bwd_pick_rm(a.M, a.L.in_dim, mx_num_sms(), true);
-  if (rm == 3) return gru_wgrad_launch<3>(a, s);
-  if (rm == 4) return gru_wgrad_launch<4>(a, s);
-  return gru_wgrad_launch<2>(a, s);
+  auto kern = rm == 3 ? k_gru_wgrad<3> : rm == 4 ? k_gru_wgrad<4> : k_gru_wgrad<2>;
+  return mx_launch("k_gru_wgrad", kern, dim3(grid), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a, sm);
 }

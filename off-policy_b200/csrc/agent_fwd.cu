@@ -512,10 +512,7 @@ __global__ void __launch_bounds__(256) k_mlp_qselect(MlpQSelArgs a) {
 int mx_launch_mlp_qselect(const MlpQSelArgs& a, cudaStream_t s) {
   int grid = mx_ceil_div(a.B * a.N, 256);
   if (grid > mx_num_sms() * 4) grid = mx_num_sms() * 4;
-  MX_LAUNCH_PDL(k_mlp_qselect, dim3(grid), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_mlp_qselect", s);
-  return MX_CHECK_LAUNCH("mlp_qselect");
+  return mx_launch("k_mlp_qselect", k_mlp_qselect, dim3(grid), dim3(256), 0, s, MX_STEP, a);
 }
 
 // =====================================================================================================
@@ -545,10 +542,7 @@ int mx_launch_pack_prev_act(const float* obs, int obs_ld, const float* acts, int
   int grid = (int)((total + 255) / 256);
   const int cap = mx_num_sms() * 8;
   if (grid > cap) grid = cap;
-  MX_LAUNCH_PDL(k_pack_prev_act, dim3(grid), dim3(256), 0, s, obs, obs_ld, acts, act_ld, X, ldx, B, T, N, O, A);
-  MX_COUNT();
-  MX_MARK("k_pack_prev_act", s);
-  return MX_CHECK_LAUNCH("pack_prev_act");
+  return mx_launch("k_pack_prev_act", k_pack_prev_act, dim3(grid), dim3(256), 0, s, MX_STEP, obs, obs_ld, acts, act_ld, X, ldx, B, T, N, O, A);
 }
 
 // =====================================================================================================
@@ -572,18 +566,7 @@ int mx_launch_front_fwd(const FrontFwdArgs& a, int nets, cudaStream_t s) {
   if (gx < 1) gx = 1;
   if (gx > ntiles) gx = ntiles;
   const size_t smem = mx_front_fwd_smem(a.L.in_dim, RM);
-  auto kern = k_front_fwd<2>;
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("front_fwd: smem %zu too large", smem); return 1; }
-    configured = smem;
-  }
-#endif
-  MX_LAUNCH_PDL(kern, dim3(gx, nets), dim3(MX_TILE_THREADS), smem, s, a);
-  MX_COUNT();
-  MX_MARK("k_front_fwd", s);
-  return MX_CHECK_LAUNCH("front_fwd");
+  return mx_launch("k_front_fwd", k_front_fwd<RM>, dim3(gx, nets), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a);
 }
 
 int mx_launch_gru_fwd(const GruFwdArgs& a, int nets, cudaStream_t s) {
@@ -592,19 +575,9 @@ int mx_launch_gru_fwd(const GruFwdArgs& a, int nets, cudaStream_t s) {
   while (rpc < 4 && mx_ceil_div(a.R, rpc) * nets > 2 * sms) rpc *= 2;   // two CTAs fit per SM (<= 128 registers): co-resident CTAs hide each other's latencies
   // sequences: the 128-thread kernel, one row per CTA (r02 sweeps: 3m 174 vs 188 us, 2s3z 555 vs 619, 8m 1408 vs 1494).  The one-step
   // "branch" calls of R-MADDPG keep the multi-row CTAs: a CTA per row would spend its time loading W_hh
-  if (a.T + 1 >= 8) {
-    MX_LAUNCH_PDL(k_gru_fwd2<1>, dim3(a.R, nets), dim3(GRU2_THREADS), 0, s, a);
-    MX_COUNT();
-    MX_MARK("k_gru_fwd", s);
-    return MX_CHECK_LAUNCH("gru_fwd2");
-  }
-  dim3 grid(mx_ceil_div(a.R, rpc), nets);
-  if (rpc == 1) MX_LAUNCH_PDL(k_gru_fwd<1>, grid, dim3(GRU_THREADS), 0, s, a);
-  else if (rpc == 2) MX_LAUNCH_PDL(k_gru_fwd<2>, grid, dim3(GRU_THREADS), 0, s, a);
-  else MX_LAUNCH_PDL(k_gru_fwd<4>, grid, dim3(GRU_THREADS), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_gru_fwd", s);
-  return MX_CHECK_LAUNCH("gru_fwd");
+  if (a.T + 1 >= 8) return mx_launch("k_gru_fwd", k_gru_fwd2<1>, dim3(a.R, nets), dim3(GRU2_THREADS), 0, s, MX_STEP, a);
+  auto kern = rpc == 1 ? k_gru_fwd<1> : rpc == 2 ? k_gru_fwd<2> : k_gru_fwd<4>;
+  return mx_launch("k_gru_fwd", kern, dim3(mx_ceil_div(a.R, rpc), nets), dim3(GRU_THREADS), 0, s, MX_STEP, a);
 }
 
 int mx_launch_qhead(const QHeadArgs& a, cudaStream_t s) {
@@ -612,9 +585,5 @@ int mx_launch_qhead(const QHeadArgs& a, cudaStream_t s) {
   int grid = mx_ceil_div(a.M, 8);
   const int cap = mx_num_sms() * 4;
   if (grid > cap) grid = cap;
-  if (a.A > 32) MX_LAUNCH_PDL(k_qhead<2>, dim3(grid), dim3(256), 0, s, a);
-  else MX_LAUNCH_PDL(k_qhead<1>, dim3(grid), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_qhead", s);
-  return MX_CHECK_LAUNCH("qhead");
+  return mx_launch("k_qhead", a.A > 32 ? k_qhead<2> : k_qhead<1>, dim3(grid), dim3(256), 0, s, MX_STEP, a);
 }

@@ -1,7 +1,10 @@
 // Error reporting, launch accounting and device queries shared by every entry point.
+#include <limits.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
+
+#include <unordered_map>
 
 #include "mx_internal.h"
 
@@ -201,13 +204,43 @@ extern "C" int mx_profile_end(void* stream, char* names_buf, int32_t buf_len, fl
 
 #if !MX_EMU
 int g_mx_smem_carveout = 100;
-void mx_prefer_carveout(const void* kern) {
-  static const void* seen[128];
-  static int nseen = 0, applied = -2;
-  if (applied != g_mx_smem_carveout) { nseen = 0; applied = g_mx_smem_carveout; }      // option changed: re-apply to every kernel
-  for (int i = 0; i < nseen; ++i) if (seen[i] == kern) return;
-  if (nseen < 128) seen[nseen++] = kern;
-  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, g_mx_smem_carveout < 0 ? -1 : g_mx_smem_carveout);
+
+// What each kernel launched so far has been configured for: its dynamic shared-memory limit and the carveout option it was given.
+struct MxKernelConfig {
+  size_t smem = 0;
+  int carveout = INT_MIN;
+};
+static std::unordered_map<const void*, MxKernelConfig> g_kernel_config;
+
+int mx_launch_config(const char* name, const void* kern, size_t smem, MxLaunchKind kind, cudaLaunchConfig_t* cfg) {
+  if (kind == MX_PLAIN && smem == 0) return 0;
+  MxKernelConfig& k = g_kernel_config[kern];
+  if (smem > k.smem) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+      cudaGetLastError();
+      mx_set_error("%s: %zu bytes of shared memory are more than the kernel can be configured for", name, smem);
+      return MX_ERR_SMEM;
+    }
+    k.smem = smem;
+  }
+  if (kind == MX_STEP) {
+    if (k.carveout != g_mx_smem_carveout) {
+      cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, g_mx_smem_carveout < 0 ? -1 : g_mx_smem_carveout);
+      k.carveout = g_mx_smem_carveout;
+    }
+    if ((g_mx_pdl > 0 || (g_mx_pdl < 0 && g_mx_pdl_auto)) && !g_mx_pdl_skip_next) {
+      cfg->attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      cfg->attrs[0].val.programmaticStreamSerializationAllowed = 1;
+      cfg->numAttrs = 1;
+    }
+    g_mx_pdl_skip_next = 0;
+  }
+  return 0;
+}
+int mx_launch_done(const char* name, cudaStream_t s) {
+  ++g_mx_launches;
+  MX_MARK(name, s);
+  return mx_check_launch(name);
 }
 int mx_num_sms() {
   static int sms = 0;

@@ -226,15 +226,8 @@ int mx_launch_gather_tma(void* p, const int64_t* idx_dev, int B, cudaStream_t s)
   if (grid > sms * 3) grid = sms * 3;                          // three resident CTAs (64 KB of stages each) per SM
   else if (grid > sms) grid = grid / sms * sms;
   const size_t smem = (size_t)GT_WARPS * GT_STAGES * GT_ROWS * GT_BOX * 4;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(k_gather_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return -1; }
-    configured = true;
-  }
-  MX_LAUNCH_PDL(k_gather_tma, dim3(grid), dim3(GT_WARPS * 32), smem, s, g->maps, a);
-  MX_COUNT();
-  MX_MARK("k_gather", s);
-  return MX_CHECK_LAUNCH("gather_tma");
+  const int rc = mx_launch("k_gather", k_gather_tma, dim3(grid), dim3(GT_WARPS * 32), smem, s, MX_STEP, g->maps, a);
+  return rc == MX_ERR_SMEM ? -1 : rc;      // no room for the stages: the vectorised gather instead
 }
 #else
 void* mx_gather_tma_create(mx_replay*) { return nullptr; }

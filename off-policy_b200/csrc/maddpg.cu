@@ -692,14 +692,6 @@ static int launch1d(long long work) {
   return (int)g;
 }
 
-// one launch of a file-local kernel, counted and marked for the profiler
-#define MX_RUN(kern, grid, block, s, ...)             \
-  do {                                                \
-    MX_LAUNCH(kern, grid, block, 0, s, __VA_ARGS__);  \
-    MX_COUNT();                                       \
-    MX_MARK(#kern, s);                                \
-  } while (0)
-
 // kernel that only publishes the two loss scalars in the layout k_adam expects: grad[P+0] = denominator, [P+1] = loss numerator
 __global__ void k_set_scalars(float* grad_tail, const float* scal) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -732,7 +724,9 @@ static int optimise(mx_maddpg* h, bool actor, int front_parts, int head_parts, c
   o.lr = c.lr; o.beta1 = c.adam_beta1; o.beta2 = c.adam_beta2; o.eps = c.adam_eps; o.max_grad_norm = c.max_grad_norm; o.tau = c.tau;
   o.weight_decay = c.weight_decay;
   if (mx_launch_grad_reduce(o, s)) return 1;     // (its scalar block bumps the Adam step count; the loss scalars come from the loss kernel)
-  MX_RUN(k_set_scalars, dim3(1), dim3(32), s, o.grad + o.P, (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c)));
+  if (mx_launch("k_set_scalars", k_set_scalars, dim3(1), dim3(32), 0, s, MX_PLAIN, o.grad + o.P,
+                (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c))))
+    return 1;
   return mx_launch_adam(o, s);
 }
 
@@ -807,7 +801,7 @@ struct Step {               // one call of learner h over batch b on stream s
   }
 
   // head of copy `sel` (LIVE or TARGET) of net n over the M rows of pass p (+ noise) into its out slot and / or the minimum into out_min
-  void head_fwd(Net n, const MxPassWs& p, int sel, int M, const float* noise, float* out_min) const {
+  int head_fwd(Net n, const MxPassWs& p, int sel, int M, const float* noise, float* out_min) const {
     const int k = sel == TARGET ? 1 : 0;
     HeadArgs a;
     memset(&a, 0, sizeof(a));
@@ -815,11 +809,11 @@ struct Step {               // one call of learner h over batch b on stream s
     a.theta = net(n).th[k]; a.h = ws + p.h[k]; a.M = M;
     if (k == 0) a.sto = ws + p.sto;
     a.noise = noise; a.out = ws + p.out[k]; a.out_min = out_min;
-    MX_RUN(k_head_fwd, dim3(launch1d((long long)M * 32)), dim3(256), s, a);
+    return mx_launch("k_head_fwd", k_head_fwd, dim3(launch1d((long long)M * 32)), dim3(256), 0, s, MX_PLAIN, a);
   }
 
   // back through the live head of net n over pass p, p.dout -> p.dh; parts: the gradient partials written, or null for a frozen head
-  void head_bwd(Net n, const MxPassWs& p, int M, int* parts) const {
+  int head_bwd(Net n, const MxPassWs& p, int M, int* parts) const {
     const NetRef nr = net(n);
     const int grid = mx_imin_host(mx_num_sms(), mx_ceil_div(M, 32));
     HeadBwdArgs a;
@@ -828,7 +822,7 @@ struct Step {               // one call of learner h over batch b on stream s
     a.theta = nr.th[0]; a.h = ws + p.h[0]; a.sto = ws + p.sto; a.dout = ws + p.dout; a.M = M; a.dh_out = ws + p.dh;
     a.gpart = parts ? nr.gpart : nullptr; a.P = nr.P;
     if (parts) *parts = grid;
-    MX_RUN(k_head_bwd, dim3(grid), dim3(256), s, a);
+    return mx_launch("k_head_bwd", k_head_bwd, dim3(grid), dim3(256), 0, s, MX_PLAIN, a);
   }
 
   // back through the live GRU of net n over pass p, p.dh -> p.dgi (R, T, N, T1, h0 as GruBwdArgs)
@@ -866,7 +860,7 @@ struct Step {               // one call of learner h over batch b on stream s
 
   // the critic's input rows [s | actions] of one pass: mode 0 the buffer actions into c.x, 1 the target actions at the next step into
   // t.x, 2 the agent-replaced copies into r.x (the recurrent learner: with the critic state before each step)
-  void pack_critic_in(int mode) const {
+  int pack_critic_in(int mode) const {
     PackArgs pk;
     memset(&pk, 0, sizeof(pk));
     pk.mode = mode; pk.B = b->B; pk.T = c.episode_len; pk.N = c.n_agents; pk.S = c.state_dim; pk.Ac = c.act_dim;
@@ -884,39 +878,41 @@ struct Step {               // one call of learner h over batch b on stream s
       if (!c.mlp) { pk.hseq = ws + W.c.h[0]; pk.h0 = ws + W.r.h0; }
       rows *= c.n_agents;
     }
-    MX_RUN(k_pack_critic_in, dim3(launch1d(rows * pk.ldx)), dim3(256), s, pk);
+    return mx_launch("k_pack_critic_in", k_pack_critic_in, dim3(launch1d(rows * pk.ldx)), dim3(256), 0, s, MX_PLAIN, pk);
   }
 
   // Discrete actions of the actor rows: mode 0 arg-max one-hot, 1 hard Gumbel-softmax of logits (+ gumbel).  MultiDiscrete (n_act_seg
   // > 0, one segment included) takes no available-action mask (MADDPGPolicy.py:73-89); maddpg_check allows it on the MLP learner only
-  void act_transform(int mode, const float* logits, const float* gumbel, float* out, float* soft) const {
+  int act_transform(int mode, const float* logits, const float* gumbel, float* out, float* soft) const {
     ActXformArgs ax;
     memset(&ax, 0, sizeof(ax));
     ax.M = Ma(); ax.Ac = c.act_dim; ax.mode = mode; ax.sg = act_segs(&c);
     ax.avail = c.n_act_seg > 0 ? nullptr : b->avail; ax.avail_ld = b->act_ld;
     ax.logits = logits; ax.gumbel = gumbel; ax.out = out; ax.soft = soft;
-    MX_RUN(k_act_transform, dim3(launch1d(Ma())), dim3(256), s, ax);
+    return mx_launch("k_act_transform", k_act_transform, dim3(launch1d(Ma())), dim3(256), 0, s, MX_PLAIN, ax);
   }
 
   // d(critic input) of the agent-replaced copies -> the actor's head outputs: a.dout, or the MLP actor's "gi" gradient rows a.dgi
-  void scatter_actor_grad() const {
-    MX_RUN(k_scatter_actor_grad, dim3(launch1d(Ma())), dim3(256), s, (const float*)(ws + W.r.dx), ldc(), b->B, c.episode_len, c.n_agents,
-           c.state_dim, c.act_dim, (const float*)(c.discrete ? ws + W.a.soft : nullptr), ws + (c.mlp ? W.a.dgi : W.a.dout), c.act_offset,
+  int scatter_actor_grad() const {
+    return mx_launch("k_scatter_actor_grad", k_scatter_actor_grad, dim3(launch1d(Ma())), dim3(256), 0, s, MX_PLAIN, (const float*)(ws + W.r.dx),
+                     ldc(), b->B, c.episode_len, c.n_agents, c.state_dim, c.act_dim, (const float*)(c.discrete ? ws + W.a.soft : nullptr), ws + (c.mlp ? W.a.dgi : W.a.dout), c.act_offset,
            c.mlp ? (int)MX_G : c.act_dim, act_segs(&c));
   }
 
   // cfg.mlp: the head outputs in columns [0, OD) of the "gi" rows at offset gi (+ noise) into out and / or their minimum into out_min
-  void mlp_head_cols(int64_t gi, int M, int OD, const float* noise, float* out, float* out_min) const {
-    MX_RUN(k_mlp_head_cols, dim3(launch1d(M)), dim3(256), s, (const float*)(ws + gi), M, OD, noise, out, out_min);
+  int mlp_head_cols(int64_t gi, int M, int OD, const float* noise, float* out, float* out_min) const {
+    return mx_launch("k_mlp_head_cols", k_mlp_head_cols, dim3(launch1d(M)), dim3(256), 0, s, MX_PLAIN, (const float*)(ws + gi), M, OD, noise, out,
+                     out_min);
   }
 
   // cfg.mlp: the gradient at the critic's head outputs p.dout as the "gi" gradient rows p.dgi that k_front_bwd reads
-  void mlp_dgi_cols(const MxPassWs& p, int M) const {
-    MX_RUN(k_mlp_dgi_cols, dim3(launch1d((long long)M * MX_G)), dim3(256), s, (const float*)(ws + p.dout), c.num_q, M, ws + p.dgi);
+  int mlp_dgi_cols(const MxPassWs& p, int M) const {
+    return mx_launch("k_mlp_dgi_cols", k_mlp_dgi_cols, dim3(launch1d((long long)M * MX_G)), dim3(256), 0, s, MX_PLAIN, (const float*)(ws + p.dout),
+                     c.num_q, M, ws + p.dgi);
   }
 
   // TD target, critic loss, PER priorities: per sequence (recurrent) or the mean over the heads (MLP, maddpg.py:144: no per_nu)
-  void critic_loss() const {
+  int critic_loss() const {
     const int T = c.episode_len, N = c.n_agents;
     CriticLossArgs cl;
     memset(&cl, 0, sizeof(cl));
@@ -926,18 +922,18 @@ struct Step {               // one call of learner h over batch b on stream s
     if (c.mlp) cl.prio_mean_k = 1;
     else cl.per_nu = c.per_nu;
     cl.use_huber = c.use_huber; cl.dq = ws + W.c.dout; cl.err = ws + W.c.err; cl.scal = ws + W.scal_c; cl.prio = c.use_per ? ws + W.prio : nullptr;
-    MX_RUN(k_critic_loss, dim3(1), dim3(256), s, cl);
+    return mx_launch("k_critic_loss", k_critic_loss, dim3(1), dim3(256), 0, s, MX_PLAIN, cl);
   }
 
   // actor loss through critic head 0 on the agent-replaced copies, masked by the agents' dones or (MLP) by valid_transition
-  void actor_loss() const {
+  int actor_loss() const {
     const int T = c.episode_len, N = c.n_agents;
     ActorLossArgs al;
     memset(&al, 0, sizeof(al));
     al.B = b->B; al.T = T; al.N = N; al.K = c.num_q; al.ld_tn = b->ep_tn_ld > 0 ? b->ep_tn_ld : T * N; al.qa = ws + W.r.out[0]; al.dones = b->dones;
     if (c.mlp) { al.valid = h->valid; al.valid_idx = b->idx; }
     al.dout = ws + W.r.dout; al.scal = ws + W.scal_a;
-    MX_RUN(k_actor_loss, dim3(1), dim3(256), s, al);
+    return mx_launch("k_actor_loss", k_actor_loss, dim3(1), dim3(256), 0, s, MX_PLAIN, al);
   }
 
   // The actor's copies `sel` over its rows Ma = B*(T+1)*N; the target copy's head (+ MATD3 noise) gives the target actions a.out[1],
@@ -948,14 +944,14 @@ struct Step {               // one call of learner h over batch b on stream s
     if (front_fwd(ACTOR, W.a, Ma(), sel, (sel & LIVE) != 0)) return 1;
     if (!c.mlp) {
       if (gru_fwd(ACTOR, W.a, sel, B * N, T, N, nullptr)) return 1;
-      if (sel & LIVE) head_fwd(ACTOR, W.a, LIVE, Ma(), nullptr, nullptr);
+      if ((sel & LIVE) && head_fwd(ACTOR, W.a, LIVE, Ma(), nullptr, nullptr)) return 1;
     }
     if (!(sel & TARGET)) return 0;
     const float* noise = c.target_noise > 0.f ? target_noise_dev : nullptr;
     // cfg.mlp (maddpg.py:64-74): the head sits in the weight_ih slot; the noise rows are the step-1 (next-observation) rows [b][2][N][Ac]
-    if (c.mlp) mlp_head_cols(W.a.gi[1], Ma(), c.act_dim, noise, ws + W.a.out[1], nullptr);
-    else head_fwd(ACTOR, W.a, TARGET, Ma(), noise, nullptr);
-    if (c.discrete) act_transform(c.target_noise > 0.f ? 1 : 0, ws + W.a.out[1], nullptr, ws + W.a.out[1], nullptr);
+    if (c.mlp ? mlp_head_cols(W.a.gi[1], Ma(), c.act_dim, noise, ws + W.a.out[1], nullptr) : head_fwd(ACTOR, W.a, TARGET, Ma(), noise, nullptr))
+      return 1;
+    if (c.discrete) return act_transform(c.target_noise > 0.f ? 1 : 0, ws + W.a.out[1], nullptr, ws + W.a.out[1], nullptr);
     return 0;
   }
 };
@@ -971,23 +967,23 @@ static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const 
   if (st.actor_fwd(BOTH, target_noise_dev)) return 1;
 
   // ---------- B. critic over the buffer sequence (live + target) ----------
-  st.pack_critic_in(0);
+  if (st.pack_critic_in(0)) return 1;
   if (st.front_fwd(CRITIC, W.c, Mc, BOTH, true)) return 1;
   if (st.gru_fwd(CRITIC, W.c, BOTH, B, T - 1, 1, nullptr)) return 1;
-  st.head_fwd(CRITIC, W.c, LIVE, Mc, nullptr, nullptr);
+  if (st.head_fwd(CRITIC, W.c, LIVE, Mc, nullptr, nullptr)) return 1;
 
   // ---------- C. target Q: one branch step per (b,t) from the target critic's buffer state ----------
-  st.pack_critic_in(1);
+  if (st.pack_critic_in(1)) return 1;
   if (st.front_fwd(CRITIC, W.t, Mc, TARGET, false)) return 1;
   if (st.gru_fwd(CRITIC, W.t, TARGET, Mc, 0, 1, ws + W.c.h[1])) return 1;
-  st.head_fwd(CRITIC, W.t, TARGET, Mc, nullptr, ws + W.t.qmin);
+  if (st.head_fwd(CRITIC, W.t, TARGET, Mc, nullptr, ws + W.t.qmin)) return 1;
 
   // ---------- D. TD target, critic loss ----------
-  st.critic_loss();
+  if (st.critic_loss()) return 1;
 
   // ---------- E. critic backward + Adam ----------
   int head_parts = 0, parts = 0;
-  st.head_bwd(CRITIC, W.c, Mc, &head_parts);
+  if (st.head_bwd(CRITIC, W.c, Mc, &head_parts)) return 1;
   if (st.gru_bwd(CRITIC, W.c, B, T, 1, T, nullptr)) return 1;
   if (st.front_bwd(CRITIC, W.c, Mc, T, 1, T, nullptr, nullptr, &parts)) return 1;
   if (optimise(st.h, false, parts, head_parts, st.s)) return 1;
@@ -998,20 +994,20 @@ static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const 
   if (st.front_fwd(CRITIC, W.c, Mc, LIVE, false)) return 1;
   if (st.gru_fwd(CRITIC, W.c, LIVE, B, T - 1, 1, nullptr)) return 1;
   // the live actor's hard Gumbel-softmax sample (straight-through), r_maddpg.py:277
-  if (st.c.discrete) st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft);
-  st.pack_critic_in(2);
+  if (st.c.discrete && st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft)) return 1;
+  if (st.pack_critic_in(2)) return 1;
   if (st.front_fwd(CRITIC, W.r, Mr, LIVE, true)) return 1;
   if (st.gru_fwd(CRITIC, W.r, LIVE, Mr, 0, 1, ws + W.r.h0)) return 1;
-  st.head_fwd(CRITIC, W.r, LIVE, Mr, nullptr, nullptr);
-  st.actor_loss();
+  if (st.head_fwd(CRITIC, W.r, LIVE, Mr, nullptr, nullptr)) return 1;
+  if (st.actor_loss()) return 1;
   // back through the (frozen) critic to its action inputs
-  st.head_bwd(CRITIC, W.r, Mr, nullptr);
+  if (st.head_bwd(CRITIC, W.r, Mr, nullptr)) return 1;
   if (st.gru_bwd(CRITIC, W.r, Mr, 1, 1, 1, ws + W.r.h0)) return 1;
   if (st.front_bwd(CRITIC, W.r, Mr, 0, 1, 1, ws + W.r.h0, ws + W.r.dx, nullptr)) return 1;
-  st.scatter_actor_grad();
+  if (st.scatter_actor_grad()) return 1;
   // actor backward + Adam
   int ahead_parts = 0, aparts = 0;
-  st.head_bwd(ACTOR, W.a, Ma, &ahead_parts);
+  if (st.head_bwd(ACTOR, W.a, Ma, &ahead_parts)) return 1;
   if (st.gru_bwd(ACTOR, W.a, B * N, T, N, T + 1, nullptr)) return 1;
   if (st.front_bwd(ACTOR, W.a, Ma, T, N, 0, nullptr, nullptr, &aparts)) return 1;
   return optimise(st.h, true, aparts, ahead_parts, st.s);
@@ -1036,33 +1032,33 @@ static int maddpg_step_mlp(const Step& st, const float* target_noise_dev, const 
   if (st.actor_fwd(st.c.cent_act_dim > 0 ? LIVE : BOTH, target_noise_dev)) return 1;
 
   // ---------- B. live critic on (s, a), target critic on (s', a'); TD target, loss, priorities (maddpg.py:112-151) ----------
-  st.pack_critic_in(0);
-  st.pack_critic_in(1);
+  if (st.pack_critic_in(0)) return 1;
+  if (st.pack_critic_in(1)) return 1;
   if (st.front_fwd(CRITIC, W.c, Mc, LIVE, true)) return 1;
   if (st.front_fwd(CRITIC, W.t, Mc, TARGET, false)) return 1;
-  st.mlp_head_cols(W.c.gi[0], Mc, K, nullptr, ws + W.c.out[0], nullptr);
-  st.mlp_head_cols(W.t.gi[1], Mc, K, nullptr, nullptr, ws + W.t.qmin);
-  st.critic_loss();
+  if (st.mlp_head_cols(W.c.gi[0], Mc, K, nullptr, ws + W.c.out[0], nullptr)) return 1;
+  if (st.mlp_head_cols(W.t.gi[1], Mc, K, nullptr, nullptr, ws + W.t.qmin)) return 1;
+  if (st.critic_loss()) return 1;
 
   // ---------- C. critic backward through the frozen live heads into the trunk; clip + Adam over the trunk ----------
-  st.mlp_dgi_cols(W.c, Mc);
+  if (st.mlp_dgi_cols(W.c, Mc)) return 1;
   int parts = 0;
   if (st.front_bwd(CRITIC, W.c, Mc, 1, 1, 0, nullptr, nullptr, &parts)) return 1;
   if (optimise(st.h, false, parts, 0, st.s)) return 1;
   if (!update_actor) return 0;
 
   // ---------- D. actor loss through head 0 of the UPDATED critic on the agent-replaced copies, masked by valid_transition ----------
-  st.mlp_head_cols(W.a.gi[0], Ma, Ac, nullptr, ws + W.a.out[0], nullptr);
+  if (st.mlp_head_cols(W.a.gi[0], Ma, Ac, nullptr, ws + W.a.out[0], nullptr)) return 1;
   // get_actions(obs, avail, use_gumbel=True): hard Gumbel-softmax, straight-through (maddpg.py:209)
-  if (st.c.discrete) st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft);
-  st.pack_critic_in(2);
+  if (st.c.discrete && st.act_transform(1, ws + W.a.out[0], actor_noise_dev, ws + W.a.act, ws + W.a.soft)) return 1;
+  if (st.pack_critic_in(2)) return 1;
   if (st.front_fwd(CRITIC, W.r, Mr, LIVE, true)) return 1;
-  st.mlp_head_cols(W.r.gi[0], Mr, K, nullptr, ws + W.r.out[0], nullptr);
-  st.actor_loss();
+  if (st.mlp_head_cols(W.r.gi[0], Mr, K, nullptr, ws + W.r.out[0], nullptr)) return 1;
+  if (st.actor_loss()) return 1;
   // back through the frozen critic (trunk and live head 0) to its action inputs, then into the actor's head rows
-  st.mlp_dgi_cols(W.r, Mr);
+  if (st.mlp_dgi_cols(W.r, Mr)) return 1;
   if (st.front_bwd(CRITIC, W.r, Mr, 1, 1, 0, nullptr, ws + W.r.dx, nullptr)) return 1;
-  st.scatter_actor_grad();
+  if (st.scatter_actor_grad()) return 1;
   int aparts = 0;
   if (st.front_bwd(ACTOR, W.a, Ma, 1, N, 0, nullptr, nullptr, &aparts)) return 1;
   return optimise(st.h, true, aparts, 0, st.s);
@@ -1129,9 +1125,9 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
   if (Step(src, b, s).actor_fwd(TARGET, target_noise_dev)) return 1;
   // cfg.mlp: k_cent_scatter's row (b*(T+1)+t+1)*N+n with T = 1, t = 0 is the next-observation step the target actor ran on
   const int B = b->B, T = c.episode_len, N = c.n_agents, Ac = c.act_dim;
-  MX_RUN(k_cent_scatter, dim3(launch1d((long long)B * T * N * Ac)), dim3(256), s, (const float*)(src->ws + src->W.a.out[1]), b->acts, b->act_ld, B, T,
-         N, Ac, dst->ws + dst->W.cent_acts, dst->ws + dst->W.cent_nacts, mx_round_up(d.cent_act_dim, 4), c.act_offset);
-  return MX_CHECK_LAUNCH("cent_contribute");
+  return mx_launch("k_cent_scatter", k_cent_scatter, dim3(launch1d((long long)B * T * N * Ac)), dim3(256), 0, s, MX_PLAIN,
+                   (const float*)(src->ws + src->W.a.out[1]), b->acts, b->act_ld, B, T, N, Ac, dst->ws + dst->W.cent_acts, dst->ws + dst->W.cent_nacts,
+                   mx_round_up(d.cent_act_dim, 4), c.act_offset);
 }
 
 // [sample ->] shared_train_policy_on_batch [-> PER write-back] [-> soft update] as one CUDA graph.  The actor is updated only

@@ -380,36 +380,16 @@ int mx_mid_supported(const MidArgs& a) {
   return mid_pick_warps(a) != 0;          // the per-warp operand staging must fit
 }
 
-template <int W, int APL>
-static int mid_launch(const MidArgs& a, int* parts_used, cudaStream_t s) {
-  const int E = a.mix.B * a.T;
-  int grid = mx_ceil_div(E, W);
-  if (grid > mx_num_sms()) grid = mx_num_sms();
-  MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, W, APL);
-  const size_t bytes = (size_t)sm.total * sizeof(float) + 16;
-  auto kern = k_mid<W, APL>;
-#if !MX_EMU
-  static size_t configured = 0;
-  if (bytes > 48 * 1024 && bytes > configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) { mx_set_error("mid: smem %zu too large", bytes); return 1; }
-    configured = bytes;
-  }
-#endif
-  MX_LAUNCH_PDL(kern, dim3(grid), dim3(32 * W), bytes, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_mid", s);
-  *parts_used = grid;
-  return MX_CHECK_LAUNCH("mid");
-}
 int mx_launch_mid(const MidArgs& a, int* parts_used, cudaStream_t s) {
-  const int w = mid_pick_warps(a);
-  if (a.A <= 32) {
-    if (w == 16) return mid_launch<16, 1>(a, parts_used, s);
-    if (w == 8) return mid_launch<8, 1>(a, parts_used, s);
-  } else if (a.A <= 64) {
-    if (w == 16) return mid_launch<16, 2>(a, parts_used, s);
-    if (w == 8) return mid_launch<8, 2>(a, parts_used, s);
+  const int w = mid_pick_warps(a), apl = a.A <= 32 ? 1 : 2;
+  if (a.A > 64 || (w != 16 && w != 8)) {
+    mx_set_error("mid: configuration does not fit (N %d, A %d)", a.N, a.A);
+    return 1;
   }
-  mx_set_error("mid: configuration does not fit (N %d, A %d)", a.N, a.A);
-  return 1;
+  auto kern = w == 16 ? (apl == 1 ? k_mid<16, 1> : k_mid<16, 2>) : (apl == 1 ? k_mid<8, 1> : k_mid<8, 2>);
+  int grid = mx_ceil_div(a.mix.B * a.T, w);
+  if (grid > mx_num_sms()) grid = mx_num_sms();
+  MidSmem sm = mid_smem(a.A, a.N, a.mix.gP, a.mix.gM, w, apl);
+  *parts_used = grid;
+  return mx_launch("k_mid", kern, dim3(grid), dim3(32 * w), (size_t)sm.total * sizeof(float) + 16, s, MX_STEP, a, sm);
 }

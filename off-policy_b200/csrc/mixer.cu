@@ -40,7 +40,7 @@ static MixSmem mix_smem_layout(const MxMixLayout& L, int TE, bool wide = false) 
   return m;
 }
 
-bool mx_mix_wide_state(const MxMixLayout& L) { return (size_t)mix_smem_layout(L, 32).total * sizeof(float) + 16 > 227 * 1024; }
+bool mx_mix_wide_state(const MxMixLayout& L) { return (size_t)mix_smem_layout(L, 32).total * sizeof(float) + 16 > MX_SMEM_OPTIN_MAX; }
 
 void mx_mix_wide_layout(const MxMixLayout& L, MxMixWide* w) {
   memset(w, 0, sizeof(*w));
@@ -728,11 +728,8 @@ int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
   if (a.vdn) {
     int grid = mx_ceil_div(E, 256);
     if (grid > sms) grid = sms;
-    MX_LAUNCH_PDL(k_vdn_mix, dim3(grid), dim3(256), 0, s, a);
-    MX_COUNT();
-    MX_MARK("k_vdn_mix", s);
     *nparts_used = grid;
-    return MX_CHECK_LAUNCH("vdn_mix");
+    return mx_launch("k_vdn_mix", k_vdn_mix, dim3(grid), dim3(256), 0, s, MX_STEP, a);
   }
   if (a.L.N > 32) { mx_set_error("mixer: n_agents > 32 unsupported"); return 1; }
   const int RM = (E > 16 * sms) ? 2 : 1;
@@ -742,33 +739,16 @@ int mx_launch_mixer(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
   int grid = mx_ceil_div(E, TE);
   if (grid > sms) grid = sms;
 #if !MX_EMU
-  if (smem > 227 * 1024) { mx_set_error("mixer: %zu bytes of shared memory needed (state_dim / n_agents too large)", smem); return 1; }
-  static size_t conf1 = 0, conf2 = 0;
-  if (RM == 1 && smem > conf1) { cudaFuncSetAttribute(k_mixer<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); conf1 = smem; }
-  if (RM == 2 && smem > conf2) { cudaFuncSetAttribute(k_mixer<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); conf2 = smem; }
+  if (smem > MX_SMEM_OPTIN_MAX) { mx_set_error("mixer: %zu bytes of shared memory needed (state_dim / n_agents too large)", smem); return 1; }
 #endif
-  if (RM == 1) MX_LAUNCH_PDL(k_mixer<1>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm);
-  else MX_LAUNCH_PDL(k_mixer<2>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_mixer", s);
   *nparts_used = grid;
-  return MX_CHECK_LAUNCH("mixer");
+  return mx_launch("k_mixer", RM == 1 ? k_mixer<1> : k_mixer<2>, dim3(grid), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a, sm);
 }
 
 int mx_mixer_split_supported(const MxMixLayout& L) { return L.ME <= 32 * MX_MIX_MAXK && L.N <= 32; }
 
 static int mix_split_rm(int E) {
   return (E > 16 * mx_num_sms()) ? 2 : 1;
-}
-template <class K>
-static int mix_smem_attr(K kern, size_t smem, size_t* conf) {
-#if !MX_EMU
-  if (smem > 227 * 1024) { mx_set_error("mixer: %zu bytes of shared memory needed (state_dim / n_agents too large)", smem); return 1; }
-  if (smem > *conf) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); *conf = smem; }
-#else
-  (void)kern; (void)smem; (void)conf;
-#endif
-  return 0;
 }
 
 int mx_launch_mix_hyper_fwd(const MixerArgs& a, cudaStream_t s) {
@@ -778,32 +758,18 @@ int mx_launch_mix_hyper_fwd(const MixerArgs& a, cudaStream_t s) {
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   int grid = mx_ceil_div(E, TE);
   if (grid > mx_num_sms()) grid = mx_num_sms();
-  if (a.wide) {
-    if (mx_launch_mixw_state_fwd(a, s)) return 1;
-    static size_t w1 = 0, w2 = 0;
-    if (RM == 1) { if (mix_smem_attr(k_mix_hyper_fwd<1, true>, smem, &w1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<1, true>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-    else { if (mix_smem_attr(k_mix_hyper_fwd<2, true>, smem, &w2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<2, true>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-    MX_COUNT();
-    MX_MARK("k_mix_hyper_fwd_wide", s);
-    return MX_CHECK_LAUNCH("mix_hyper_fwd_wide");
-  }
-  static size_t c1 = 0, c2 = 0;
-  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_fwd<1, false>, smem, &c1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<1, false>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  else { if (mix_smem_attr(k_mix_hyper_fwd<2, false>, smem, &c2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_fwd<2, false>), dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  MX_COUNT();
-  MX_MARK("k_mix_hyper_fwd", s);
-  return MX_CHECK_LAUNCH("mix_hyper_fwd");
+  if (a.wide && mx_launch_mixw_state_fwd(a, s)) return 1;
+  auto kern = a.wide ? (RM == 1 ? k_mix_hyper_fwd<1, true> : k_mix_hyper_fwd<2, true>)
+                     : (RM == 1 ? k_mix_hyper_fwd<1, false> : k_mix_hyper_fwd<2, false>);
+  return mx_launch(a.wide ? "k_mix_hyper_fwd_wide" : "k_mix_hyper_fwd", kern, dim3(grid, 2), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a, sm);
 }
 
 int mx_launch_mix_core(const MixerArgs& a, int* scalar_parts_used, cudaStream_t s) {
   const int E = a.B * a.T;
   int grid = mx_ceil_div(E, 16);                  // one warp per element, 16 warps per CTA: 3m (1 920 elements) = 120 CTAs, one pass
   if (grid > mx_num_sms()) grid = mx_num_sms();   // (spart holds one scalar partial per SM)
-  MX_LAUNCH_PDL(k_mix_core, dim3(grid), dim3(512), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_mix_core", s);
   *scalar_parts_used = grid;
-  return MX_CHECK_LAUNCH("mix_core");
+  return mx_launch("k_mix_core", k_mix_core, dim3(grid), dim3(512), 0, s, MX_STEP, a);
 }
 
 int mx_launch_mix_hyper_bwd(const MixerArgs& a, int* nparts_used, cudaStream_t s) {
@@ -813,21 +779,10 @@ int mx_launch_mix_hyper_bwd(const MixerArgs& a, int* nparts_used, cudaStream_t s
   const size_t smem = (size_t)sm.total * sizeof(float) + 16;
   int grid = mx_ceil_div(E, TE);
   if (grid > mx_num_sms()) grid = mx_num_sms();
-  if (a.wide) {
-    static size_t w1 = 0, w2 = 0;
-    if (RM == 1) { if (mix_smem_attr(k_mix_hyper_bwd<1, true>, smem, &w1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<1, true>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-    else { if (mix_smem_attr(k_mix_hyper_bwd<2, true>, smem, &w2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<2, true>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-    MX_COUNT();
-    MX_MARK("k_mix_hyper_bwd_wide", s);
-    *nparts_used = grid;
-    if (MX_CHECK_LAUNCH("mix_hyper_bwd_wide")) return 1;
-    return mx_launch_mixw_state_wgrad(a, s);
-  }
-  static size_t c1 = 0, c2 = 0;
-  if (RM == 1) { if (mix_smem_attr(k_mix_hyper_bwd<1, false>, smem, &c1)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<1, false>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  else { if (mix_smem_attr(k_mix_hyper_bwd<2, false>, smem, &c2)) return 1; MX_LAUNCH_PDL((k_mix_hyper_bwd<2, false>), dim3(grid), dim3(MX_TILE_THREADS), smem, s, a, sm); }
-  MX_COUNT();
-  MX_MARK("k_mix_hyper_bwd", s);
+  auto kern = a.wide ? (RM == 1 ? k_mix_hyper_bwd<1, true> : k_mix_hyper_bwd<2, true>)
+                     : (RM == 1 ? k_mix_hyper_bwd<1, false> : k_mix_hyper_bwd<2, false>);
   *nparts_used = grid;
-  return MX_CHECK_LAUNCH("mix_hyper_bwd");
+  if (const int rc = mx_launch(a.wide ? "k_mix_hyper_bwd_wide" : "k_mix_hyper_bwd", kern, dim3(grid), dim3(MX_TILE_THREADS), smem, s, MX_STEP, a, sm))
+    return rc;
+  return a.wide ? mx_launch_mixw_state_wgrad(a, s) : 0;
 }

@@ -177,25 +177,13 @@ int mx_launch_mixw_state_fwd(const MixerArgs& a, cudaStream_t s) {
     const size_t n = (size_t)w.Cp * w.Sp + w.Cp;
     int grid = (int)((n + 255) / 256);
     if (grid > 4 * mx_num_sms()) grid = 4 * mx_num_sms();
-    MX_LAUNCH_PDL(k_mixw_prep, dim3(grid, 2), dim3(256), 0, s, a.theta, a.theta_tgt, w, a.L.S, a.wimg);
-    MX_COUNT();
-    MX_MARK("k_mixw_prep", s);
-    if (MX_CHECK_LAUNCH("mixw_prep")) return 1;
+    if (const int rc = mx_launch("k_mixw_prep", k_mixw_prep, dim3(grid, 2), dim3(256), 0, s, MX_STEP, a.theta, a.theta_tgt, w, a.L.S, a.wimg))
+      return rc;
   }
   const MixwFwdSmem sm = mixw_fwd_smem();
   const int R = a.B * (a.T + 1);
   const dim3 grid(mx_ceil_div(R, 128), 2 * mx_ceil_div(w.Cp, MXW_NB));
-#if !MX_EMU
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(k_mixw_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, sm.total) != cudaSuccess) { mx_set_error("mixw_fwd: smem %d too large", sm.total); return 1; }
-    configured = true;
-  }
-#endif
-  MX_LAUNCH_PDL(k_mixw_fwd, grid, dim3(128), (size_t)sm.total, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_mixw_fwd", s);
-  return MX_CHECK_LAUNCH("mixw_fwd");
+  return mx_launch("k_mixw_fwd", k_mixw_fwd, grid, dim3(128), (size_t)sm.total, s, MX_STEP, a, sm);
 }
 
 // ---- weight gradient -----------------------------------------------------------------------------------------------------------
@@ -314,15 +302,5 @@ int mx_launch_mixw_state_wgrad(const MixerArgs& a, cudaStream_t s) {
   if (!a.d_pre) { mx_set_error("mixer (wide state): d_pre region missing"); return 1; }
   const MixwGradSmem sm = mixw_grad_smem();
   const dim3 grid(mx_ceil_div(a.L.S, MXW_NS), mx_ceil_div(a.wl.Cp, 128));
-#if !MX_EMU
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(k_mixw_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, sm.total) != cudaSuccess) { mx_set_error("mixw_wgrad: smem %d too large", sm.total); return 1; }
-    configured = true;
-  }
-#endif
-  MX_LAUNCH_PDL(k_mixw_wgrad, grid, dim3(128), (size_t)sm.total, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_mixw_wgrad", s);
-  return MX_CHECK_LAUNCH("mixw_wgrad");
+  return mx_launch("k_mixw_wgrad", k_mixw_wgrad, grid, dim3(128), (size_t)sm.total, s, MX_STEP, a, sm);
 }

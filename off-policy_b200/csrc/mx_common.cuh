@@ -10,7 +10,6 @@
 #ifdef MARL_EMU
 #include "emu_runtime.h"
 #define MX_EMU 1
-#define MX_LAUNCH_PDL MX_LAUNCH
 #define MX_PDL_WAIT() ((void)0)
 #define MX_PDL_THETA_WRITTEN() ((void)0)
 #else
@@ -18,10 +17,7 @@
 #define MX_EMU 0
 #define MX_LAUNCH(kern, grid, block, smem, stream, ...) kern<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
 
-// Programmatic dependent launch (PDL).  A kernel launched with MX_LAUNCH_PDL may begin while its stream predecessor is still
-// running; everything it does before MX_PDL_WAIT() overlaps the predecessor's tail, so that part may only touch state the
-// predecessor does not write: its own shared memory / tensor-core accumulator and the parameter vectors theta / theta_target.  Those are written
-// only by the optimiser kernels, which call MX_PDL_THETA_WRITTEN() so that the NEXT launch is a plain, fully ordered one.
+// Programmatic dependent launch (mx_launch in mx_internal.h says which launches may overlap their predecessor).
 // MX_PDL_WAIT() = griddepcontrol.wait (returns at once in a plain launch) followed by launch_dependents, i.e. a dependent may
 // start as soon as every CTA of this grid is past its own wait -- never before this grid's predecessor has completed.
 extern int g_mx_pdl, g_mx_pdl_auto, g_mx_pdl_rows;      // option pdl: -1 automatic (per learner step, by size), 0 off, 1 on
@@ -32,26 +28,7 @@ extern int g_mx_pdl_skip_next;
     asm volatile("griddepcontrol.wait;" ::: "memory");                    \
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");       \
   } while (0)
-// Kernels of the two branches of a step only share an SM if the SM's L1 / shared-memory split, fixed while any CTA is resident, leaves
-// room for both: every step kernel asks for the largest shared-memory carveout once (option smem_carveout, percent; < 0 = driver default).
 extern int g_mx_smem_carveout;
-void mx_prefer_carveout(const void* kern);
-template <typename... KArgs, typename... Args>
-static inline void mx_launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
-  mx_prefer_carveout(reinterpret_cast<const void*>(kern));
-  cudaLaunchConfig_t cfg;
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  cfg.attrs = at; cfg.numAttrs = 0;
-  if ((g_mx_pdl > 0 || (g_mx_pdl < 0 && g_mx_pdl_auto)) && !g_mx_pdl_skip_next) {
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 1;
-  }
-  g_mx_pdl_skip_next = 0;
-  cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
-#define MX_LAUNCH_PDL(kern, grid, block, smem, stream, ...) mx_launch_pdl(kern, grid, block, smem, stream, __VA_ARGS__)
 #endif
 
 #define MX_H 64          // hidden size the kernels are specialised for (reference default, config.py:63)

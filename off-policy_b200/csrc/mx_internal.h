@@ -12,16 +12,57 @@ extern int g_mx_prof_on;
 void mx_prof_mark(const char* name, cudaStream_t s);
 extern int g_mx_mixer_split, g_mx_overlap, g_mx_overlap_rows, g_mx_mid_fused, g_mx_optim_fused, g_mx_p2p_ll, g_mx_p2p_timeout_ms;
 int mx_set_option_common(const char* name, int value);   // 0 when `name` was one of the build-independent options
-#define MX_COUNT() (++g_mx_launches)
 #define MX_MARK(name, s) do { if (g_mx_prof_on) mx_prof_mark((name), (s)); } while (0)
 
 #if MX_EMU
 static inline int mx_num_sms() { return 4; }
-#define MX_CHECK_LAUNCH(what) 0
+static inline int mx_check_launch(const char*) { return 0; }
 #else
 int mx_num_sms();
 int mx_check_launch(const char* what);
-#define MX_CHECK_LAUNCH(what) mx_check_launch(what)
+#endif
+
+// ---- launching a kernel ------------------------------------------------------------------------------------------------------------
+// Every kernel launch goes through mx_launch: it raises the kernel's dynamic shared-memory limit when `smem` needs it, applies the
+// launch policy of `kind`, launches, counts the launch (mx_launch_count), marks `name` for the profiler and returns the launch status:
+// 0, MX_ERR_SMEM when the kernel cannot be given `smem` bytes (mx_last_error says so), or mx_check_launch's code.
+//
+// MX_STEP launches are the learner-step kernels, whose device code calls MX_PDL_WAIT():
+//  * Programmatic dependent launch (PDL).  Such a kernel may begin while its stream predecessor is still running; everything it does
+//    before MX_PDL_WAIT() overlaps the predecessor's tail, so that part may only touch state the predecessor does not write: its own
+//    shared memory / tensor-core accumulator and the parameter vectors theta / theta_target.  Those are written only by the optimiser
+//    kernels, which call MX_PDL_THETA_WRITTEN() so that the NEXT launch is a plain, fully ordered one.
+//  * Kernels of the two branches of a step only share an SM if the SM's L1 / shared-memory split, fixed while any CTA is resident,
+//    leaves room for both: every step kernel asks for the largest shared-memory carveout (option smem_carveout, percent; < 0 = driver
+//    default), once per kernel and again after the option changes.
+// MX_PLAIN launches (replay, rollout, exchange, noise and actor-critic head kernels, the probe) are ordinary launches.
+enum MxLaunchKind { MX_PLAIN, MX_STEP };
+constexpr size_t MX_SMEM_OPTIN_MAX = 227 * 1024;   // dynamic shared memory one block may opt in to on sm_90
+constexpr int MX_ERR_SMEM = 1;
+
+#if MX_EMU
+template <typename... KArgs, typename... Args>
+static inline int mx_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, MxLaunchKind,
+                            Args&&... args) {
+  emu::launch(grid, block, smem, [&]() { kern(args...); });
+  ++g_mx_launches;
+  MX_MARK(name, s);
+  return 0;
+}
+#else
+int mx_launch_config(const char* name, const void* kern, size_t smem, MxLaunchKind kind, cudaLaunchConfig_t* cfg);   // opt-in, carveout, PDL
+int mx_launch_done(const char* name, cudaStream_t s);                                                              // count, mark, check
+template <typename... KArgs, typename... Args>
+static inline int mx_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, MxLaunchKind kind,
+                            Args&&... args) {
+  cudaLaunchAttribute at[1];
+  cudaLaunchConfig_t cfg;
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
+  cfg.attrs = at; cfg.numAttrs = 0;
+  if (const int rc = mx_launch_config(name, reinterpret_cast<const void*>(kern), smem, kind, &cfg)) return rc;
+  cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
+  return mx_launch_done(name, s);
+}
 #endif
 
 // whole-step CUDA graph (qmix.cu): the recorded launch sequence, kept for the emulated build which simply re-runs it

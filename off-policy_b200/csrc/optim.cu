@@ -444,10 +444,7 @@ __global__ void __launch_bounds__(256) k_polyak(float* __restrict__ tgt, const f
 
 int mx_launch_grad_reduce(const OptimArgs& a, cudaStream_t s) {
   const int grid = mx_grad_reduce_blocks(a.P) + 1;
-  MX_LAUNCH_PDL(k_grad_reduce, dim3(grid), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_grad_reduce", s);
-  return MX_CHECK_LAUNCH("grad_reduce");
+  return mx_launch("k_grad_reduce", k_grad_reduce, dim3(grid), dim3(256), 0, s, MX_STEP, a);
 }
 int g_mx_optim_fused = 1;
 int mx_launch_optim_fused(const OptimArgs& a, cudaStream_t s) {
@@ -459,34 +456,27 @@ int mx_launch_optim_fused(const OptimArgs& a, cudaStream_t s) {
   OptimArgs b = a;
   const int grid = mx_grad_reduce_blocks(a.P) + 1;
   b.phase = 1;
-  MX_LAUNCH(k_optim_fused, dim3(grid), dim3(256), 0, s, b);
+  MX_LAUNCH(k_optim_fused, dim3(grid), dim3(256), 0, s, b);      // uncounted: the two phases are one launch on the device
   b.phase = 2;
-  MX_LAUNCH(k_optim_fused, dim3(grid), dim3(256), 0, s, b);
-  MX_COUNT();
-  MX_MARK("k_optim_fused", s);
-  return 0;
+  return mx_launch("k_optim_fused", k_optim_fused, dim3(grid), dim3(256), 0, s, MX_PLAIN, b);
 #else
   if (!g_mx_optim_fused || !a.sync || !a.normpart) return -1;
   const int grid = mx_grad_reduce_blocks(a.P) + 1;
   static int per_sm = -1;
   if (per_sm < 0 && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_optim_fused, 256, 0) != cudaSuccess) per_sm = 0;
   if (grid > per_sm * mx_num_sms()) return -1;        // not all blocks co-resident: no grid barrier
-  MX_LAUNCH_PDL(k_optim_fused, dim3(grid), dim3(256), 0, s, a);
+  const int rc = mx_launch("k_optim_fused", k_optim_fused, dim3(grid), dim3(256), 0, s, MX_STEP, a);
   MX_PDL_THETA_WRITTEN();
-  MX_COUNT();
-  MX_MARK("k_optim_fused", s);
-  return MX_CHECK_LAUNCH("optim_fused");
+  return rc;
 #endif
 }
 int mx_launch_adam(const OptimArgs& a, cudaStream_t s) {
   int grid = (int)((a.P + 4095) / 4096);
   const int sms = mx_num_sms();
   if (grid > sms) grid = sms;
-  MX_LAUNCH_PDL(k_adam, dim3(grid), dim3(1024), 0, s, a);
+  const int rc = mx_launch("k_adam", k_adam, dim3(grid), dim3(1024), 0, s, MX_STEP, a);
   MX_PDL_THETA_WRITTEN();
-  MX_COUNT();
-  MX_MARK("k_adam", s);
-  return MX_CHECK_LAUNCH("adam");
+  return rc;
 }
 int mx_launch_polyak(float* tgt, const float* src, long long n, float tau, cudaStream_t s) {
   const long long n4 = n / 4;
@@ -494,9 +484,7 @@ int mx_launch_polyak(float* tgt, const float* src, long long n, float tau, cudaS
   const int sms = mx_num_sms();
   if (grid > sms) grid = sms;
   if (grid < 1) grid = 1;
-  MX_LAUNCH_PDL(k_polyak, dim3(grid), dim3(256), 0, s, tgt, src, n4, tau);
+  const int rc = mx_launch("k_polyak", k_polyak, dim3(grid), dim3(256), 0, s, MX_STEP, tgt, src, n4, tau);
   MX_PDL_THETA_WRITTEN();
-  MX_COUNT();
-  MX_MARK("k_polyak", s);
-  return MX_CHECK_LAUNCH("polyak");
+  return rc;
 }

@@ -146,18 +146,12 @@ extern "C" int mx_qmix_p2p_publish(mx_qmix* q, void* stream) {
   if (!q->p2p_world) { mx_set_error("mx_qmix_p2p_publish: mx_qmix_set_peers was not called"); return 1; }
   P2pArgs a = p2p_args(q);
   cudaStream_t s = (cudaStream_t)stream;
-  MX_LAUNCH(k_p2p_push, dim3(p2p_grid(a)), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_p2p_push", s);
-  return MX_CHECK_LAUNCH("p2p_publish");
+  return mx_launch("k_p2p_push", k_p2p_push, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
 }
 
 extern "C" int mx_qmix_p2p_reduce(mx_qmix* q, void* stream) {
   if (!q->p2p_world) { mx_set_error("mx_qmix_p2p_reduce: mx_qmix_set_peers was not called"); return 1; }
   P2pArgs a = p2p_args(q);
   cudaStream_t s = (cudaStream_t)stream;
-  MX_LAUNCH(k_p2p_sum, dim3(p2p_grid(a)), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_p2p_sum", s);
-  return MX_CHECK_LAUNCH("p2p_reduce");
+  return mx_launch("k_p2p_sum", k_p2p_sum, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
 }

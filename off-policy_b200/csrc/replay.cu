@@ -587,33 +587,26 @@ static int insert_staged(mx_replay* r, int32_t n_ep, int32_t* first_slot_out, cu
     rs.rew_stage = reinterpret_cast<const float*>(stage + sf[3].offset); rs.de_stage = reinterpret_cast<const float*>(stage + sf[5].offset);
     rs.T = T; rs.N = N; rs.n_ep = n_ep; rs.first_slot = first; rs.capacity = c.capacity; rs.filled_before = r->filled;
     rs.rstats = at<double>(r, L.off_rstats); rs.state = a.state;
-    MX_LAUNCH(k_reward_stats_update, dim3(1), dim3(256), 0, s, rs);
-    MX_COUNT();
-    MX_MARK("k_reward_stats_update", s);
+    if (const int rc = mx_launch("k_reward_stats_update", k_reward_stats_update, dim3(1), dim3(256), 0, s, MX_PLAIN, rs)) return rc;
   }
   int64_t work = a.f[0].count;
   int grid = (int)((work + 255) / 256);
   int maxg = mx_num_sms() * 8;
   if (grid > maxg) grid = maxg;
   if (grid < 1) grid = 1;
-  MX_LAUNCH(k_insert_scatter, dim3(grid), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_insert_scatter", s);
+  if (const int rc = mx_launch("k_insert_scatter", k_insert_scatter, dim3(grid), dim3(256), 0, s, MX_PLAIN, a)) return rc;
   if (c.use_per) {
     TreeUpd u;
     memset(&u, 0, sizeof(u));
     u.sum_tree = at<double>(r, L.off_sum_tree); u.min_tree = at<double>(r, L.off_min_tree);
     u.cap = L.tree_cap; u.n = n_ep; u.idx = nullptr; u.first_slot = first; u.capacity = c.capacity;
     u.alpha = c.per_alpha; u.prime_from_max = 1; u.state = a.state; u.update_max = 0;
-    int th = mx_round_up(n_ep, 32);
-    MX_LAUNCH(k_tree_update, dim3(1), dim3(th), 0, s, u);
-    MX_COUNT();
-    MX_MARK("k_tree_update", s);
+    if (const int rc = mx_launch("k_tree_update", k_tree_update, dim3(1), dim3(mx_round_up(n_ep, 32)), 0, s, MX_PLAIN, u)) return rc;
   }
   if (first_slot_out) *first_slot_out = first;
   r->cursor = a.new_cursor;
   r->filled = a.new_filled;
-  return MX_CHECK_LAUNCH("insert");
+  return 0;
 }
 
 static int check_insert(mx_replay* r, int32_t n_ep) {
@@ -725,10 +718,7 @@ static int launch_gather(mx_replay* r, const int64_t* idx_dev, int B, cudaStream
   int grid = (int)(want < 1 ? 1 : want);
   if (grid > sms * 8) grid = sms * 8;
   else if (grid > sms) grid = grid / sms * sms;
-  MX_LAUNCH_PDL(k_gather, dim3(grid), dim3(256), 0, s, g);
-  MX_COUNT();
-  MX_MARK("k_gather", s);
-  return MX_CHECK_LAUNCH("gather");
+  return mx_launch("k_gather", k_gather, dim3(grid), dim3(256), 0, s, MX_STEP, g);
 }
 
 static int check_sample(mx_replay* r, int B) {
@@ -746,9 +736,7 @@ extern "C" int mx_replay_sample_uniform(mx_replay* r, int32_t B, void* stream) {
   d.state = at<MxReplayState>(r, r->L.off_state);
   d.B = B; d.per = 0;
   d.idx_out = at<long long>(r, r->L.off_b_idx);
-  MX_LAUNCH(k_draw, dim3(1), dim3(256), 0, s, d);
-  MX_COUNT();
-  MX_MARK("k_draw", s);
+  if (const int rc = mx_launch("k_draw", k_draw, dim3(1), dim3(256), 0, s, MX_PLAIN, d)) return rc;
   return launch_gather(r, at<int64_t>(r, r->L.off_b_idx), B, s);
 }
 
@@ -775,8 +763,8 @@ __global__ void k_set_beta(MxReplayState* st, double beta) { st->per_beta = beta
 extern "C" int mx_replay_set_beta(mx_replay* r, double beta, void* stream) {
   if (!r || !r->cfg.use_per) { mx_set_error("mx_replay_set_beta: replay created without use_per"); return 1; }
   if (!(beta > 0)) { mx_set_error("mx_replay_set_beta: beta must be > 0"); return 1; }
-  MX_LAUNCH(k_set_beta, dim3(1), dim3(1), 0, (cudaStream_t)stream, at<MxReplayState>(r, r->L.off_state), beta);
-  return MX_CHECK_LAUNCH("set_beta");
+  MX_LAUNCH(k_set_beta, dim3(1), dim3(1), 0, (cudaStream_t)stream, at<MxReplayState>(r, r->L.off_state), beta);   // (not counted or marked)
+  return mx_check_launch("set_beta");
 }
 
 static int sample_per_impl(mx_replay* r, int32_t B, double beta, void* stream);
@@ -802,9 +790,7 @@ static int sample_per_impl(mx_replay* r, int32_t B, double beta, void* stream) {
   d.beta = beta;
   d.w_out = at<double>(r, r->L.off_b_weights);
   d.w32_out = at<float>(r, r->L.off_b_wf32);
-  MX_LAUNCH(k_draw, dim3(1), dim3(256), 0, s, d);
-  MX_COUNT();
-  MX_MARK("k_draw", s);
+  if (const int rc = mx_launch("k_draw", k_draw, dim3(1), dim3(256), 0, s, MX_PLAIN, d)) return rc;
   return launch_gather(r, at<int64_t>(r, r->L.off_b_idx), B, s);
 }
 
@@ -820,10 +806,7 @@ extern "C" int mx_replay_update_priorities(mx_replay* r, const int64_t* idx_dev,
   u.cap = r->L.tree_cap; u.n = B; u.idx = (const long long*)idx_dev; u.capacity = r->cfg.capacity;
   u.prio = prio_dev; u.leaves = leaves_f64_dev; u.alpha = r->cfg.per_alpha; u.prime_from_max = 0;
   u.state = at<MxReplayState>(r, r->L.off_state); u.update_max = 1;
-  MX_LAUNCH(k_tree_update, dim3(1), dim3(mx_round_up(B, 32)), 0, s, u);
-  MX_COUNT();
-  MX_MARK("k_tree_update", s);
-  return MX_CHECK_LAUNCH("tree_update");
+  return mx_launch("k_tree_update", k_tree_update, dim3(1), dim3(mx_round_up(B, 32)), 0, s, MX_PLAIN, u);
 }
 
 extern "C" int mx_replay_batch(const mx_replay* r, int32_t B, mx_batch* out) {

@@ -149,8 +149,5 @@ extern "C" int mx_policy_step(const mx_policy_step_args* p, void* stream) {
   const int cap = mx_num_sms() * 4;
   if (grid > cap) grid = cap;
   cudaStream_t s = (cudaStream_t)stream;
-  MX_LAUNCH(k_policy_step, dim3(grid), dim3(MX_ROLL_THREADS), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_policy_step", s);
-  return MX_CHECK_LAUNCH("policy_step");
+  return mx_launch("k_policy_step", k_policy_step, dim3(grid), dim3(MX_ROLL_THREADS), 0, s, MX_PLAIN, a);
 }

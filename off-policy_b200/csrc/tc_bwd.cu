@@ -350,17 +350,7 @@ static int launch_wgrad_tc(const FrontBwdArgs& a, int nparts, int ln_zero_from, 
   w.nchunks = mx_ceil_div(a.M, WG_ROWS);
   w.Kp16 = mx_round_up(a.L.in_dim, 16);
   WgradSmem sm = wgrad_smem(64 + w.Kp16);
-#if !MX_EMU
-  static int configured = 0;
-  if (sm.total > configured) {
-    if (cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, sm.total) != cudaSuccess) { mx_set_error("wgrad_tc: smem %d too large", sm.total); return 1; }
-    configured = sm.total;
-  }
-#endif
-  MX_LAUNCH_PDL(k_wgrad_tc, dim3(nparts), dim3(WG_THREADS), (size_t)sm.total, s, w, sm);
-  MX_COUNT();
-  MX_MARK("k_wgrad_tc", s);
-  return MX_CHECK_LAUNCH("wgrad_tc");
+  return mx_launch("k_wgrad_tc", k_wgrad_tc, dim3(nparts), dim3(WG_THREADS), (size_t)sm.total, s, MX_STEP, w, sm);
 }
 
 
@@ -636,10 +626,7 @@ bool mx_front_bwd_tc_usable(const FrontBwdArgs& a) {
 bool mx_tc_prep_T_wanted(int in_dim) { return wgrad_mode(in_dim) >= 2 && in_dim <= WG_MAX_IN; }
 int mx_launch_tc_prep_weights_T(const float* theta, const MxNetLayout& L, float* imgT, cudaStream_t s) {
   const int n = 3 * 4096 + 4096 + mx_round_up(L.in_dim, 16) * 64;
-  MX_LAUNCH_PDL(k_tc_prep_weights_T, dim3((n + 255) / 256), dim3(256), 0, s, theta, L, imgT);
-  MX_COUNT();
-  MX_MARK("k_tc_prep_weights_T", s);
-  return MX_CHECK_LAUNCH("tc_prep_weights_T");
+  return mx_launch("k_tc_prep_weights_T", k_tc_prep_weights_T, dim3((n + 255) / 256), dim3(256), 0, s, MX_STEP, theta, L, imgT);
 }
 
 int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t s) {
@@ -648,16 +635,9 @@ int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t
   // streamed (every weight operand through ONE chunk buffer, two CTAs per SM) when the caller gives the side array for the LayerNorm sums
   const bool stream = a.ln_part != nullptr;
   BwdTcSmem sm = bwd_tc_smem(Kp16, stream);
-#if !MX_EMU
-  static int configured = 0;
-  if (sm.total > configured) {
-    if (cudaFuncSetAttribute(k_front_bwd_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, sm.total) != cudaSuccess) { mx_set_error("front_bwd_tc: smem %d too large", sm.total); return 1; }
-    configured = sm.total;
-  }
-#endif
   const int ntiles = mx_ceil_div(a.M, 128), nchunks = mx_ceil_div(a.M, WG_ROWS);
   int ga = mx_num_sms(), gb = mx_num_sms();
-  if (stream && 2 * (sm.total + 2048) <= 227 * 1024) ga = 2 * mx_num_sms();      // two CTAs per SM fit
+  if (stream && 2 * (sm.total + 2048) <= (int)MX_SMEM_OPTIN_MAX) ga = 2 * mx_num_sms();      // two CTAs per SM fit
   if (ga > ntiles) ga = ntiles;
   if (gb > nchunks) gb = nchunks;
   if (!a.tc_acc || a.tc_acc_cols < 512) { mx_set_error("front_bwd_tc: accumulator region missing or too small"); return 1; }
@@ -666,10 +646,7 @@ int mx_launch_front_bwd_tc(const FrontBwdArgs& a, int* nparts_used, cudaStream_t
   FrontBwdArgs b = a;
   b.wgrad_external = 1;
   if (ga > a.ln_part_rows && stream) ga = a.ln_part_rows;
-  MX_LAUNCH_PDL(k_front_bwd_tc, dim3(ga), dim3(128), (size_t)sm.total, s, b, sm);
-  MX_COUNT();
-  MX_MARK("k_front_bwd_tc", s);
-  if (MX_CHECK_LAUNCH("front_bwd_tc")) return 1;
+  if (const int rc = mx_launch("k_front_bwd_tc", k_front_bwd_tc, dim3(ga), dim3(128), (size_t)sm.total, s, MX_STEP, b, sm)) return rc;
   *nparts_used = gb;
   if (stream) return launch_wgrad_tc(b, gb, -1, s, ga);
   return launch_wgrad_tc(b, gb, ga < gb ? ga : -1, s);

@@ -96,10 +96,7 @@ int mx_launch_tc_prep_weights(const float* const theta[2], const MxNetLayout& L,
   const int n = MX_H * mx_round_up(L.in_dim, 8) + MX_H * MX_H + MX_G * MX_H;
   TcPrepArgs p;
   for (int k = 0; k < 2; ++k) { p.th[k] = theta[k < nets ? k : 0]; p.img[k] = img[k < nets ? k : 0]; }
-  MX_LAUNCH_PDL(k_tc_prep_weights, dim3((n + 255) / 256, nets), dim3(256), 0, s, p, L);
-  MX_COUNT();
-  MX_MARK("k_tc_prep_weights", s);
-  return MX_CHECK_LAUNCH("tc_prep_weights");
+  return mx_launch("k_tc_prep_weights", k_tc_prep_weights, dim3((n + 255) / 256, nets), dim3(256), 0, s, MX_STEP, p, L);
 }
 
 // 64-term sums on 8 independent chains (a thread owns a whole row: no other warp hides FADD latency for it)
@@ -668,17 +665,7 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
     if (g2 > ntiles) g2 = ntiles;
     if (g2 * nets * 256 > a.tc_acc_cols) g2 = a.tc_acc_cols / (256 * nets);
     if (g2 < 1) g2 = 1;
-#if !MX_EMU
-    static bool configured_w2 = false;
-    if (!configured_w2) {
-      if (cudaFuncSetAttribute(k_front_fwd_tc_wide2, cudaFuncAttributeMaxDynamicSharedMemorySize, s2.total) != cudaSuccess) { mx_set_error("front_fwd_tc_wide2: smem %d too large", s2.total); return 1; }
-      configured_w2 = true;
-    }
-#endif
-    MX_LAUNCH_PDL(k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, a, s2);
-    MX_COUNT();
-    MX_MARK("k_front_fwd_tc_wide", s);
-    return MX_CHECK_LAUNCH("front_fwd_tc_wide2");
+    return mx_launch("k_front_fwd_tc_wide", k_front_fwd_tc_wide2, dim3(g2, nets), dim3(128), (size_t)s2.total, s, MX_STEP, a, s2);
   }
   FrontTcSmem sm = front_tc_smem(mx_round_up(a.L.in_dim, 8));
   const size_t smem = (size_t)sm.total;
@@ -686,31 +673,11 @@ int mx_launch_front_fwd_tc(const FrontFwdArgs& a, int nets, cudaStream_t s) {
   if (gx > ntiles) gx = ntiles;
   if (gx * nets * 256 > a.tc_acc_cols) gx = a.tc_acc_cols / (256 * nets);      // 256 accumulator columns per CTA
   if (gx < 1) gx = 1;
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > configured) {
-    if (cudaFuncSetAttribute(k_front_fwd_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("front_fwd_tc: smem %zu too large", smem); return 1; }
-    configured = smem;
-  }
-#endif
   // (inputs of 57..64 columns fill the 227 KB with operand tiles: the pair-exchange buffer of the 256-thread kernel no longer fits beside them)
-  if (smem + 5 * 1024 + 256 <= 227 * 1024) {
-#if !MX_EMU
-    static size_t configured2 = 0;
-    if (smem > configured2) {
-      if (cudaFuncSetAttribute(k_front_fwd_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { mx_set_error("front_fwd_tc2: smem %zu too large", smem); return 1; }
-      configured2 = smem;
-    }
-#endif
-    MX_LAUNCH_PDL(k_front_fwd_tc2, dim3(gx, nets), dim3(256), smem, s, a, sm);
-    MX_COUNT();
-    MX_MARK("k_front_fwd_tc", s);
-    return MX_CHECK_LAUNCH("front_fwd_tc2");
-  }
-  MX_LAUNCH_PDL(k_front_fwd_tc, dim3(gx, nets), dim3(128), smem, s, a, sm);
-  MX_COUNT();
-  MX_MARK("k_front_fwd_tc1", s);      // (its own name: tests pin which of the two variants ran)
-  return MX_CHECK_LAUNCH("front_fwd_tc");
+  if (smem + 5 * 1024 + 256 <= MX_SMEM_OPTIN_MAX)
+    return mx_launch("k_front_fwd_tc", k_front_fwd_tc2, dim3(gx, nets), dim3(256), smem, s, MX_STEP, a, sm);
+  // (its own name: tests pin which of the two variants ran)
+  return mx_launch("k_front_fwd_tc1", k_front_fwd_tc, dim3(gx, nets), dim3(128), smem, s, MX_STEP, a, sm);
 }
 
 extern "C" int mx_set_option(const char* name, int32_t value) {
@@ -783,11 +750,5 @@ extern "C" int mx_tc_linear_probe(const float* X, const float* W, float* Y, int3
   if (N % 16 || N < 16 || N > 256 || K % 8 || K < 8 || K > 64 || M < 1) { mx_set_error("tc probe: M >= 1, N %% 16, N <= 256, K %% 8, K <= 64 required"); return 1; }
   TcProbeArgs a{X, W, Y, M, N, K, passes, swap_ls};
   const size_t smem = (size_t)(2 * 128 + 2 * 64) * K * 4 + 64 * 128 * 4;
-#if !MX_EMU
-  static size_t configured = 0;
-  if (smem > configured) { cudaFuncSetAttribute(k_tc_linear_probe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); configured = smem; }
-#endif
-  MX_LAUNCH(k_tc_linear_probe, dim3((M + 127) / 128), dim3(128), smem, (cudaStream_t)stream, a);
-  MX_COUNT();
-  return MX_CHECK_LAUNCH("tc_linear_probe");
+  return mx_launch("k_tc_linear_probe", k_tc_linear_probe, dim3((M + 127) / 128), dim3(128), smem, (cudaStream_t)stream, MX_PLAIN, a);
 }

@@ -136,9 +136,7 @@ extern "C" int mx_trng_fill(uint32_t* state_dev, const mx_trng_draw* f, uint32_t
   if (!state_dev || !scratch_dev) { mx_set_error("mx_trng_fill: null state or scratch"); return 1; }
   if (scratch_words < words) { mx_set_error("mx_trng_fill: scratch of %lld words, the fill consumes %lld", (long long)scratch_words, (long long)words); return 1; }
   cudaStream_t s = (cudaStream_t)stream;
-  MX_LAUNCH(k_trng_twist, dim3(1), dim3(256), 0, s, state_dev, scratch_dev, (int)words);
-  MX_COUNT();
-  MX_MARK("k_trng_twist", s);
+  if (const int rc = mx_launch("k_trng_twist", k_trng_twist, dim3(1), dim3(256), 0, s, MX_PLAIN, state_dev, scratch_dev, (int)words)) return rc;
   TrngFillArgs a;
   a.words = scratch_dev;
   a.n = (int)((int64_t)f->T * f->rows_n * f->rows_b * f->cols);
@@ -151,8 +149,5 @@ extern "C" int mx_trng_fill(uint32_t* state_dev, const mx_trng_draw* f, uint32_t
   a.ld_t = f->ld_t; a.ld_n = f->ld_n; a.ld_b = f->ld_b;
   int grid = (a.n + 255) / 256;
   if (grid > mx_num_sms() * 4) grid = mx_num_sms() * 4;
-  MX_LAUNCH(k_trng_fill, dim3(grid), dim3(256), 0, s, a);
-  MX_COUNT();
-  MX_MARK("k_trng_fill", s);
-  return MX_CHECK_LAUNCH("trng_fill");
+  return mx_launch("k_trng_fill", k_trng_fill, dim3(grid), dim3(256), 0, s, MX_PLAIN, a);
 }
