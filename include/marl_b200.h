@@ -287,7 +287,8 @@ typedef struct mx_maddpg_cfg {
    * obs).  The critic's K Q heads are not trained (a plain list in the reference, SURVEY.md App. D-6): the live and the target heads
    * are two fixed initialisations kept behind the critic's trunk, outside the range Adam, clipping and the target updates touch.
    * The actor loss is masked by valid_transition (mx_maddpg_set_valid).  Several policies work as in the recurrent learner
-   * (cent_act_dim > 0, mx_maddpg_cent_contribute before every step); mx_maddpg_graph_capture takes one shared policy only. */
+   * (cent_act_dim > 0, mx_maddpg_cent_contribute before every step).  mx_maddpg_graph_capture(_ex) takes one shared policy only;
+   * several policies are captured together, a whole batch_train per graph, by mx_maddpg_batch_graph_capture (recurrent or mlp). */
   int32_t mlp;
   /* MultiDiscrete actions (envs/mpe/multi_discrete.py, act.py:15-17: one Linear head per sub-space): the action is n_act_seg one-hot
    * blocks of act_seg[i] columns, act_dim = their sum.  Arg-max, hard Gumbel-softmax and its straight-through gradient work per block,
@@ -322,7 +323,8 @@ int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* batch, const float* target_n
 int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* src_batch, const float* target_noise_dev, mx_maddpg* dst, void* stream);
 /* Whole-update CUDA graph (declared with mx_graph below): [sample ->] step [-> PER write-back] [-> soft update when the actor
  * was updated, base_runner.py:250-252]; flags as for mx_graph_capture.  One graph per variant (update_actor = 1 / 0); the two
- * noise pointers are fixed device buffers the caller refills before every mx_graph_launch. */
+ * noise pointers are fixed device buffers the caller refills before every mx_graph_launch.  A learner of several policies
+ * (cent_act_dim > 0) is refused: its step needs every policy's contribution first (mx_maddpg_batch_graph_capture). */
 struct mx_graph;
 int mx_maddpg_graph_capture(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                             const float* actor_noise_dev, int32_t update_actor, void* stream, struct mx_graph** out);
@@ -359,6 +361,18 @@ int mx_trng_fill(uint32_t* state_dev, const mx_trng_draw* f, uint32_t* scratch_d
 int mx_maddpg_graph_capture_ex(mx_replay* r, mx_maddpg* h, int32_t B, double beta, uint32_t flags, const float* target_noise_dev,
                                const float* actor_noise_dev, int32_t update_actor, uint32_t* state_dev, const mx_trng_draw* fills,
                                int32_t n_fills, uint32_t* scratch_dev, int64_t scratch_words, void* stream, struct mx_graph** out);
+/* Several policies (cent_act_dim > 0; mx_maddpg_graph_capture(_ex) refuses such a learner): one batch_train of the runner
+ * (runner/{rnn,mlp}/base_runner.py) as one CUDA graph.  stores / learners: the P >= 2 policies' replays and learners in policy-id order
+ * (act_offsets tiling cent_act_dim).  Per policy p: its fill_counts[p] fills (the next ones of `fills`, in the order torch's calls would
+ * make them: the target noise of every policy q in id order, then p's actor draws), the sample (flags bit0: one uniform draw on
+ * stores[uniform_store]; bit1: a PER draw from p's tree) gathered into every other store, mx_maddpg_cent_contribute of every q into p,
+ * the step of p, and (bit3) the write-back to p's tree; then (bit2) the soft updates of all P learners in the update_actor variant.
+ * target_noise_dev[p * P + q]: q's target noise in p's update; actor_noise_dev[p]: p's actor draws (NULL where none is taken; one
+ * buffer may serve every p when the fills write it inside the graph).  Each replay advances every learner's update count. */
+int mx_maddpg_batch_graph_capture(mx_replay* const* stores, mx_maddpg* const* learners, int32_t n_policies, int32_t uniform_store, int32_t B,
+                                  double beta, uint32_t flags, const float* const* target_noise_dev, const float* const* actor_noise_dev,
+                                  int32_t update_actor, uint32_t* state_dev, const mx_trng_draw* fills, const int32_t* fill_counts,
+                                  uint32_t* scratch_dev, int64_t scratch_words, void* stream, struct mx_graph** out);
 /* cfg.mlp: valid_transition of the transition store, device fp32 [rows][n_agents] (mlp_buffer.py:156).  The actor loss of a batch
  * reads row batch->idx[b] (row b when the batch has no indices); NULL: every transition is valid.  The pointer is kept, so a
  * captured graph reads the store as it is at replay time. */

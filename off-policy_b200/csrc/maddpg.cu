@@ -1130,6 +1130,20 @@ extern "C" int mx_maddpg_cent_contribute(mx_maddpg* src, const mx_batch* b, cons
                    mx_round_up(d.cent_act_dim, 4), c.act_offset);
 }
 
+// The noise fills a capture puts in its graph: refused before the capture rather than half-way through it.
+static int check_fills(const char* who, const uint32_t* state_dev, const mx_trng_draw* fills, int32_t n_fills, const uint32_t* scratch_dev,
+                       int64_t scratch_words) {
+  if (n_fills < 0 || (n_fills > 0 && (!fills || !state_dev || !scratch_dev))) {
+    mx_set_error("%s: %d fills need the fills, the generator state and the scratch", who, n_fills); return 1;
+  }
+  for (int32_t i = 0; i < n_fills; ++i) {
+    const int64_t w = mx_trng_words(&fills[i]);
+    if (w < 0) return 1;
+    if (w > scratch_words) { mx_set_error("%s: scratch of %lld words, fill %d consumes %lld", who, (long long)scratch_words, i, (long long)w); return 1; }
+  }
+  return 0;
+}
+
 // [sample ->] shared_train_policy_on_batch [-> PER write-back] [-> soft update] as one CUDA graph.  The actor is updated only
 // every actor_update_interval-th call, so the caller records one graph per variant (update_actor = 1 / 0) and replays the one
 // the update counter asks for; the noise buffers are fixed device buffers the caller refills before each launch.
@@ -1143,20 +1157,13 @@ extern "C" int mx_maddpg_graph_capture_ex(mx_replay* r, mx_maddpg* h, int32_t B,
                                           const float* actor_noise_dev, int32_t update_actor, uint32_t* state_dev, const mx_trng_draw* fills,
                                           int32_t n_fills, uint32_t* scratch_dev, int64_t scratch_words, void* stream, mx_graph** out) {
   if (!r || !h || !out) { mx_set_error("mx_maddpg_graph_capture: null argument"); return 1; }
-  if (h->cfg.mlp && h->cfg.cent_act_dim > 0) {      // the graph would replay the step without the other policies' contributions
-    mx_set_error("mx_maddpg_graph_capture: an MLP learner with several policies (cent_act_dim > 0) cannot be captured: its step needs "
-                 "mx_maddpg_cent_contribute from every policy first; run it eagerly");
+  if (h->cfg.cent_act_dim > 0) {      // the graph would replay the step without the other policies' contributions
+    mx_set_error("mx_maddpg_graph_capture: a learner of several policies (cent_act_dim > 0) cannot be captured alone: its step needs "
+                 "mx_maddpg_cent_contribute from every policy first; capture the whole batch_train with mx_maddpg_batch_graph_capture");
     return 1;
   }
-  if (n_fills < 0 || (n_fills > 0 && (!fills || !state_dev || !scratch_dev))) {
-    mx_set_error("mx_maddpg_graph_capture_ex: %d fills need the fills, the generator state and the scratch", n_fills); return 1;
-  }
+  if (check_fills("mx_maddpg_graph_capture_ex", state_dev, fills, n_fills, scratch_dev, scratch_words)) return 1;
   std::vector<mx_trng_draw> fl(fills, fills + n_fills);
-  for (const mx_trng_draw& f : fl) {              // refused here rather than half-way through the capture
-    const int64_t w = mx_trng_words(&f);
-    if (w < 0) return 1;
-    if (w > scratch_words) { mx_set_error("mx_maddpg_graph_capture_ex: scratch of %lld words, a fill consumes %lld", (long long)scratch_words, (long long)w); return 1; }
-  }
   if ((flags & 2u) && mx_replay_set_beta(r, beta, stream)) return 1;
   auto seq = [=](void* st) -> int {
     for (const mx_trng_draw& f : fl)
@@ -1174,6 +1181,93 @@ extern "C" int mx_maddpg_graph_capture_ex(mx_replay* r, mx_maddpg* h, int32_t B,
     return 0;
   };
   return mx_graph_capture_seq(seq, [h]() { h->num_updates += 1; }, stream, out);
+}
+
+// Several policies: one batch_train of the runner (runner/{rnn,mlp}/base_runner.py batch_train) as one CUDA graph.  Per policy p in id
+// order: p's noise fills; the sample (uniform: one draw on stores[uniform_store], PER: p's tree) gathered into every other store;
+// mx_maddpg_cent_contribute of every policy q into p; the step of p; the write-back to p's tree.  Then, when the actor was updated,
+// the soft updates of all P policies.  The eager trainer does the same launches in the same order (MaddpgTrainer
+// .shared_train_policy_on_batch), so a replay computes what an eager batch_train computes, bit for bit.
+extern "C" int mx_maddpg_batch_graph_capture(mx_replay* const* stores, mx_maddpg* const* learners, int32_t P, int32_t uniform_store, int32_t B,
+                                             double beta, uint32_t flags, const float* const* target_noise_dev,
+                                             const float* const* actor_noise_dev, int32_t update_actor, uint32_t* state_dev,
+                                             const mx_trng_draw* fills, const int32_t* fill_counts, uint32_t* scratch_dev,
+                                             int64_t scratch_words, void* stream, mx_graph** out) {
+  static const char* who = "mx_maddpg_batch_graph_capture";
+  if (!stores || !learners || !target_noise_dev || !actor_noise_dev || !out) { mx_set_error("%s: null argument", who); return 1; }
+  if (P < 2) { mx_set_error("%s: %d policies; one shared policy is captured by mx_maddpg_graph_capture_ex", who, P); return 1; }
+  if ((flags & 1u) && (uniform_store < 0 || uniform_store >= P)) { mx_set_error("%s: uniform_store %d outside [0, %d)", who, uniform_store, P); return 1; }
+  for (int32_t p = 0; p < P; ++p)
+    if (!stores[p] || !learners[p]) { mx_set_error("%s: store or learner %d is null", who, p); return 1; }
+  // the learners form one policy set: same centralised action width, episode length and kind, act_offsets tiling cent_act_dim in order
+  const mx_maddpg_cfg& c0 = learners[0]->cfg;
+  int32_t off = 0;
+  for (int32_t p = 0; p < P; ++p) {
+    const mx_maddpg_cfg& c = learners[p]->cfg;
+    if (c.cent_act_dim <= 0 || c.cent_act_dim != c0.cent_act_dim || c.episode_len != c0.episode_len || c.mlp != c0.mlp) {
+      mx_set_error("%s: learner %d (cent_act_dim %d, episode length %d, mlp %d) is not of one policy set with learner 0 (%d, %d, %d; "
+                   "cent_act_dim > 0)", who, p, c.cent_act_dim, c.episode_len, c.mlp, c0.cent_act_dim, c0.episode_len, c0.mlp);
+      return 1;
+    }
+    if (B <= 0 || B > c.max_batch) { mx_set_error("%s: batch size %d outside [1, max_batch=%d] of learner %d", who, B, c.max_batch, p); return 1; }
+    if (c.act_offset != off) {
+      mx_set_error("%s: learner %d has act_offset %d, expected %d: the learners are not in policy-id order or not one policy set", who, p,
+                   c.act_offset, off);
+      return 1;
+    }
+    off += c.n_agents * c.act_dim;
+    const mx_replay_cfg& r = stores[p]->cfg;
+    if (r.n_agents != c.n_agents || r.obs_dim != c.obs_dim || r.act_dim != c.act_dim || r.share_dim != c.state_dim || r.episode_len != c.episode_len) {
+      mx_set_error("%s: store %d (agents %d, obs %d, act %d, share %d, episode %d) does not hold the batches of learner %d (%d, %d, %d, %d, %d)",
+                   who, p, r.n_agents, r.obs_dim, r.act_dim, r.share_dim, r.episode_len, p, c.n_agents, c.obs_dim, c.act_dim, c.state_dim,
+                   c.episode_len);
+      return 1;
+    }
+    if (B > r.max_batch) { mx_set_error("%s: batch size %d > max_batch=%d of store %d", who, B, r.max_batch, p); return 1; }
+    if ((flags & 2u) && (!r.use_per || !c.use_per)) { mx_set_error("%s: PER sampling needs use_per in store and learner %d", who, p); return 1; }
+  }
+  if (off != c0.cent_act_dim) { mx_set_error("%s: the %d learners' action widths sum to %d, cent_act_dim is %d", who, P, off, c0.cent_act_dim); return 1; }
+  std::vector<std::vector<mx_trng_draw>> fl(P);
+  for (int32_t p = 0, first = 0; p < P; first += fl[p].size(), ++p) {
+    const int32_t n = fill_counts ? fill_counts[p] : 0;
+    if (check_fills(who, state_dev, fills + first, n, scratch_dev, scratch_words)) return 1;
+    fl[p].assign(fills + first, fills + first + n);
+  }
+  const std::vector<mx_replay*> R(stores, stores + P);
+  const std::vector<mx_maddpg*> H(learners, learners + P);
+  const std::vector<const float*> tn(target_noise_dev, target_noise_dev + (size_t)P * P), an(actor_noise_dev, actor_noise_dev + P);
+  if (flags & 2u)
+    for (mx_replay* r : R)
+      if (mx_replay_set_beta(r, beta, stream)) return 1;
+  auto seq = [=](void* st) -> int {
+    std::vector<mx_batch> b(P);
+    for (int32_t p = 0; p < P; ++p) {
+      for (const mx_trng_draw& f : fl[p])
+        if (mx_trng_fill(state_dev, &f, scratch_dev, scratch_words, st)) return 1;
+      if (flags & 3u) {      // one index set for every store (rec_buffer.py:76-80,291-299, mlp_buffer.py:100-106,288-296)
+        mx_replay* src = (flags & 1u) ? R[uniform_store] : R[p];
+        if ((flags & 1u) ? mx_replay_sample_uniform(src, B, st) : mx_replay_sample_per_state_beta(src, B, st)) return 1;
+        mx_batch sb;
+        if (mx_replay_batch(src, B, &sb)) return 1;
+        for (mx_replay* r : R)
+          if (r != src && mx_replay_gather(r, sb.idx, B, st)) return 1;
+      }
+      for (int32_t q = 0; q < P; ++q)
+        if (mx_replay_batch(R[q], B, &b[q])) return 1;
+      for (int32_t q = 0; q < P; ++q)
+        if (mx_maddpg_cent_contribute(H[q], &b[q], tn[(size_t)p * P + q], H[p], st)) return 1;
+      H[p]->force_update_actor = update_actor ? 1 : 0;
+      const int rc = mx_maddpg_step_ex(H[p], &b[p], tn[(size_t)p * P + p], an[p], nullptr, st);
+      H[p]->force_update_actor = -1;
+      if (rc) return 1;
+      if (flags & 8u) { if (mx_replay_update_priorities(R[p], b[p].idx, mx_maddpg_priorities(H[p]), nullptr, nullptr, B, st)) return 1; }
+    }
+    if ((flags & 4u) && update_actor)       // base_runner.py batch_train: after the P updates
+      for (mx_maddpg* h : H)
+        if (mx_maddpg_soft_update(h, st)) return 1;
+    return 0;
+  };
+  return mx_graph_capture_seq(seq, [H]() { for (mx_maddpg* h : H) h->num_updates += 1; }, stream, out);
 }
 extern "C" int64_t mx_maddpg_num_updates(const mx_maddpg* h) { return h->num_updates; }
 extern "C" int mx_maddpg_set_num_updates(mx_maddpg* h, int64_t n) {

@@ -162,6 +162,8 @@ def _declare(lib):
         "mx_maddpg_graph_capture": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(vp)]),
         "mx_maddpg_graph_capture_ex": (C.c_int, [vp, vp, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(TrngDraw), i32, vp, i64, vp,
                                                  C.POINTER(vp)]),
+        "mx_maddpg_batch_graph_capture": (C.c_int, [vp, vp, i32, i32, i32, dbl, u32, vp, vp, i32, vp, C.POINTER(TrngDraw), vp, vp, i64,
+                                                    vp, C.POINTER(vp)]),
         "mx_trng_seed": (C.c_int, [vp, C.c_uint64, vp]),
         "mx_trng_set_state": (C.c_int, [vp, C.POINTER(u32), i32, i32, vp]),
         "mx_trng_get_state": (C.c_int, [vp, C.POINTER(u32), C.POINTER(i32), C.POINTER(i32), vp]),
