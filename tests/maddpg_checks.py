@@ -286,3 +286,57 @@ def check_multi_golden(name, through_buffer=False):
                 if err > 5e-3 * lr * rounds + 1e-7:
                     problems.append("final p%d %s.%s err %.3e" % (i, tag, k, err))
     assert not problems, "\n".join(problems[:40])
+
+
+def check_oracle_lockstep(cfg, B, T, steps=3, seed=40):
+    """R-MADDPG / R-MATD3 whole updates at (B, T) in lock-step with the fp32 oracle, from the randomised state of
+    row_coverage_checks.maddpg_pair: per update the losses, grad norms and every clipped critic / actor gradient tensor within 1e-4,
+    the draws taken from torch's CPU generator in the trainer's order (R-MATD3's target noise, then the Discrete actor's Gumbel draws on
+    the updates that train the actor), soft updates after each actor update; the parameters after the last one within 5e-3 lr per
+    update.  Returns the worst gradient error relative to its bound."""
+    import row_coverage_checks as rc
+    from oracle.maddpg import MaddpgLearner, sample_gumbel, synth_batch_cont, synth_batch_disc
+    L64, pol, tr = rc.maddpg_pair(cfg, B, T)
+    L = MaddpgLearner(cfg, dtype=torch.float32)
+    for dst, src in ((L.actor, pol.actor), (L.critic, pol.critic), (L.tgt_actor, pol.target_actor), (L.tgt_critic, pol.target_critic)):
+        dst.load_state_dict({k: v.cpu() for k, v in src.state_dict().items()})
+    N, problems, worst = cfg.n_agents, [], 0.0
+    for s in range(steps):
+        batch = (synth_batch_disc if cfg.discrete else synth_batch_cont)(cfg, B, T, seed=seed + s)
+        w = np.random.RandomState(seed + 100 + s).rand(B).astype(np.float32) * 0.9 + 0.1
+        batch = tuple(batch) + (w if cfg.use_per else None, np.arange(B) if cfg.use_per else None)
+        update = tr.num_updates["policy_0"] % tr.actor_update_interval == 0
+        torch.manual_seed(1000 + s)
+        tnoise = tr.draw_target_noise(B).numpy() if cfg.td3 else None
+        anoise = sample_gumbel((T, N * B, cfg.act_dim)).numpy() if cfg.discrete and update else None
+        torch.manual_seed(1000 + s)
+        info, _, _ = tr.shared_train_policy_on_batch("policy_0", ref_tuple(batch))
+        ref, _ = L.step(batch, tnoise, anoise)
+        ga, gc = tr.grad_views()
+        assert bool(info["update_actor"]) == bool(ref["update_actor"]) == update, (s, info["update_actor"], ref["update_actor"])
+        keys = ("critic_loss", "critic_grad_norm") + (("actor_loss", "actor_grad_norm") if update else ())
+        for key in keys:
+            e = rel_err(info[key].cpu(), ref[key])
+            if e > 1e-4:
+                problems.append("step %d %s rel err %.3e" % (s, key, e))
+        nets = [(gc, pol.Pc, pol._c_entries, L.critic_grads, ref["critic_grad_norm"])]
+        if update:
+            nets.append((ga, pol.Pa, pol._a_entries, L.actor_grads, ref["actor_grad_norm"]))
+        for flat, P, entries, grads, gn in nets:
+            coef = min(1.0, cfg.max_grad_norm / (float(gn) + 1e-6))
+            views = named_views(flat, entries)
+            for k, gr in grads.items():
+                ok, err, lim = close(views[k] / flat[P] * coef, gr, 1e-4)
+                worst = max(worst, err / lim)
+                if not ok:
+                    problems.append("step %d grad %s err %.3e > %.3e" % (s, k, err, lim))
+        if update:
+            pol.soft_target_updates()
+            L.soft_update()
+    for mod, ref_mod in ((pol.actor, L.actor), (pol.critic, L.critic), (pol.target_actor, L.tgt_actor), (pol.target_critic, L.tgt_critic)):
+        for k, v in mod.state_dict().items():
+            err = float((v.cpu() - ref_mod.state_dict()[k]).abs().max())
+            if err > 5e-3 * cfg.lr * steps + 1e-7:
+                problems.append("final %s err %.3e" % (k, err))
+    assert not problems, "\n".join(problems[:40])
+    return worst

@@ -36,6 +36,14 @@ from oracle.maddpg_mlp_md import MlpMaddpgMD, draw_noise_multi_md, step_multi_md
 DECISION_MARGIN = 1e-3
 SOFTMAX_SLACK = 0.05
 MAX_REDRAWS = 40
+# An isolated row whose gradient the fp32 oracle itself gets wrong by more than this share of GRAD_TOL is ill-conditioned, not a tile
+# edge: above 128 critic columns the actor row's gradient is the critic's input-LayerNorm backward at the agent's action columns,
+# rstd (d0 g - mean(d0 g) - xh mean(d0 g xh)), whose terms can cancel to a small share of their size.  Measured on the emulator at
+# simple_spread N = 6 (critic 246): one copy row in four where the fp32 oracle is 8.4e-6 off float64 (4e-7 on the other three) and the
+# engine 2.5e-5.  Such a transition is redrawn like a near-tie and counted (stats["ill_conditioned"], printed per case), never absorbed
+# into a wider bound.  The rule applies only to critics wider than FP32_COND_MIN_CRITIC columns; narrower cases are checked as drawn.
+FP32_COND_SHARE = 0.25
+FP32_COND_MIN_CRITIC = 128
 
 
 # ---- the learner pair ------------------------------------------------------------------------------------------------------
@@ -60,13 +68,13 @@ def build_pair(specs, S, B, discrete=True, td3=False, seed=11, **over):
     return args, pols, tr, oracles64(args, pols)
 
 
-def oracles64(args, pols):
+def oracles64(args, pols, dtype=torch.float64):
     cpu = lambda m: {k: v.cpu() for k, v in m.state_dict().items()}
     return {p: MlpMaddpgMD(cpu(pol.actor), cpu(pol.critic), cpu(pol.critic_heads), cpu(pol.target_actor), cpu(pol.target_critic),
                            cpu(pol.target_critic_heads), pol.discrete, pol.td3, gamma=args.gamma, lr=args.lr, eps=args.opti_eps,
                            weight_decay=args.weight_decay, max_grad_norm=args.max_grad_norm, tau=args.tau, huber=args.use_huber_loss,
                            huber_delta=args.huber_delta, use_per=args.use_per, per_eps=args.per_eps, relu=bool(args.use_ReLU),
-                           feature_norm=bool(args.use_feature_normalization), segs=pol.act_segs, dtype=torch.float64)
+                           feature_norm=bool(args.use_feature_normalization), segs=pol.act_segs, dtype=dtype)
             for p, pol in pols.items()}
 
 
@@ -232,14 +240,16 @@ def settle(tr, L64, p, batch, checks, seed, rng, stats, slack=True):
 # ---- tile rules of the MLP step ----------------------------------------------------------------------------------------------
 def row_tiles(rules, M, in_dim, data_grad=False):
     """(kernel, rows per tile, tiles) of the backward that owns an M-row space of width in_dim on the MLP path.  No recurrence:
-    k_front_bwd picks its tile height without the k_gru_wgrad extension.  Above 64 columns the weight gradient runs on k_wgrad_tc's
+    k_front_bwd picks its tile height without the k_gru_wgrad extension.  At 65-128 columns the weight gradient runs on k_wgrad_tc's
     64-row chunks (after k_front_bwd_tc) -- except for a data-gradient launch (the agent-replaced copies: dX set, skip_wgrad), which
-    neither tensor-core kernel takes (tc_bwd.cu mx_wgrad_tc_usable / mx_front_bwd_tc_usable): FFMA k_front_bwd at every width."""
-    if in_dim > 64 and not data_grad:
-        TM, nt, _ = rules.agent_rows(M, in_dim)["k_wgrad_tc"]
-        return "k_wgrad_tc", TM, nt
-    TM = 16 * rules.front_bwd_rm(M, in_dim, False)
-    return "k_front_bwd", TM, -(-M // TM)
+    neither tensor-core kernel takes (tc_bwd.cu mx_wgrad_tc_usable / mx_front_bwd_tc_usable).  Up to 64 and above 128 columns
+    (WG_MAX_IN), and for the copies at every width: FFMA k_front_bwd, on 32-row tiles only above 128."""
+    kern = "k_front_bwd" if data_grad else rules.row_kernel(in_dim)
+    if kern == "k_front_bwd":
+        TM = 16 * rules.front_bwd_rm(M, in_dim, False)
+        return kern, TM, -(-M // TM)
+    TM, nt, _ = rules.agent_rows(M, in_dim, gru_ext=False)[kern]
+    return kern, TM, nt
 
 
 def spaces(rules, B, N, O, cin):
@@ -349,13 +359,39 @@ def owner_launches(names):
     return {"critic": names[d[0] + 1:red[0]], "copies": names[d[1] + 1:sc], "actor": names[sc + 1:red[1]]}
 
 
-def assert_row_kernels(names, sp, n_policies=1):
+def forward_launches(names):
+    """The forward launches of one MLP step by the nets they run: a critic forward (live and target on the buffer rows, live on the
+    agent-replaced copies) directly follows the k_pack_critic_in that built its input; every other k_front_fwd* launch is an actor's."""
+    out = {"critic": [], "actor": []}
+    after_pack = False
+    for k in names:
+        if k.startswith("k_front_fwd"):
+            out["critic" if after_pack else "actor"].append(k)
+        else:
+            after_pack = k == "k_pack_critic_in"
+    return out
+
+
+# above WG_MAX_IN (128) input columns every net runs FFMA: k_front_fwd<2> forward (no tensor-core image), k_front_bwd backward
+TC_KERNELS = ("k_front_fwd_tc", "k_front_fwd_tc1", "k_front_fwd_tc_wide", "k_front_bwd_tc", "k_wgrad_tc", "k_tc_prep_weights_T")
+
+
+def assert_row_kernels(names, sp, n_policies=1, widths=None):
     """Each space's row kernel ran in the launch that owns that space; the copies' backward is exactly one k_front_bwd; every policy's
-    cent_contribute ran (k_cent_scatter) when there are several."""
+    cent_contribute ran (k_cent_scatter) when there are several.  widths {"critic": cin, "actor": obs}: a net above 128 columns ran
+    only k_front_fwd forwards and only k_front_bwd in each of its spaces' own launches."""
     own = owner_launches(names)
     for name, (M, kern, TM, nt) in sp.items():
         assert kern in own[name], (name, kern, "did not run in its own launch", own[name])
     assert own["copies"] == ["k_front_bwd"], own["copies"]
+    fwd = forward_launches(names)
+    for net, w in (widths or {}).items():
+        if w <= 128:
+            continue
+        assert fwd[net] and set(fwd[net]) == {"k_front_fwd"}, (net, w, "forward launches", fwd[net], names)
+        for name in ("critic", "copies") if net == "critic" else ("actor",):
+            assert own[name] == ["k_front_bwd"], (name, w, "backward launches", own[name])
+        assert not any(k in TC_KERNELS for k in own["critic" if net == "critic" else "actor"]), (net, own)
     for k in ("k_mlp_head_cols", "k_critic_loss", "k_actor_loss", "k_pack_critic_in"):
         assert k in names, (k, "did not run")
     if n_policies > 1:
@@ -382,7 +418,22 @@ def grad_errs(ours, ref, tol, tag):
     return errs
 
 
-def isolated(tr, pols, L64, p, batch, pairs, sp, seed, rng, stats, tol=GRAD_TOL):
+def fp32_oracle_error(L32, L64, p, batch, tn, an):
+    """The fp32 oracle's worst relative gradient error against float64 on `batch` (its conditioning, FP32_COND_SHARE).  Both steps run on
+    copies, so neither oracle's Adam state moves."""
+    import copy
+    _, _, g32 = step_multi_md(copy.deepcopy(L32), p, batch, tn, an, dtype=torch.float32)
+    _, _, g64 = step_multi_md(copy.deepcopy(L64), p, batch, tn, an, dtype=torch.float64)
+    worst = 0.0
+    for net, d in g64.items():
+        for k, r in d.items():
+            scale = float(r.detach().abs().max())
+            if scale > 0.0:
+                worst = max(worst, float((g32[net][k].detach().double() - r.detach()).abs().max()) / scale)
+    return worst
+
+
+def isolated(tr, pols, L64, p, batch, pairs, sp, seed, rng, stats, tol=GRAD_TOL, L32=None):
     """For each (n, b, tiles) of `pairs` (pinned_pairs): one engine step of policy p with PER weights one-hot on b and valid_transition
     one-hot on (n, b), against the float64 step: every critic and actor tensor within tol x max|ref|, and the isolated copy's actor_loss
     within ROW_TOL of its scale; the decisions settled first.  The pair's critic, actor and copy rows must sit in `tiles`.  Returns the
@@ -390,18 +441,30 @@ def isolated(tr, pols, L64, p, batch, pairs, sp, seed, rng, stats, tol=GRAD_TOL)
     B = np.asarray(batch[0][p]).shape[1]
     Np = np.asarray(batch[0][p]).shape[0]
     worst = {}
+    cond = pols[p].central_obs_dim + pols[p].central_act_dim > FP32_COND_MIN_CRITIC
+    if cond and L32 is None:
+        L32 = oracles64(tr.args, pols, torch.float32)
+    stats.setdefault("ill_conditioned", 0)
     for i, (n, b, tiles) in enumerate(pairs):
         for name, t in tiles.items():
             assert space_row(name, n, b, B, Np) // sp[name][2] == t, (name, n, b, t)
         s = seed + 17 * i
-        bt = settle(tr, L64, p, batch, [("critic", b), ("actor", (n, b))], s, rng, stats)
-        bt = far_td_error(L64, p, bt, b, *noise_at(tr, p, B, s))
-        w = np.zeros(B, np.float32)
-        w[b] = 1.0
-        valid = {q: np.array(v, copy=True) for q, v in bt[8].items()}
-        valid[p][:] = 0.0
-        valid[p][n, b] = 1.0
-        bt = tuple(bt[:8]) + (valid,) + tuple(bt[9:11]) + (w, np.arange(B))
+        for _ in range(MAX_REDRAWS + 1):
+            bt = settle(tr, L64, p, batch, [("critic", b), ("actor", (n, b))], s, rng, stats)
+            bt = far_td_error(L64, p, bt, b, *noise_at(tr, p, B, s))
+            w = np.zeros(B, np.float32)
+            w[b] = 1.0
+            valid = {q: np.array(v, copy=True) for q, v in bt[8].items()}
+            valid[p][:] = 0.0
+            valid[p][n, b] = 1.0
+            bt = tuple(bt[:8]) + (valid,) + tuple(bt[9:11]) + (w, np.arange(B))
+            if not cond or fp32_oracle_error(L32, L64, p, bt, *noise_at(tr, p, B, s)) <= FP32_COND_SHARE * tol:
+                break
+            batch = redraw(batch, rng, b)
+            stats["redraws"] = stats.get("redraws", 0) + 1
+            stats["ill_conditioned"] += 1
+        else:
+            raise AssertionError("transition %d: no draw the fp32 oracle gets within %.0e of float64" % (b, FP32_COND_SHARE * tol))
         qscale = float(margins(L64, p, bt, *noise_at(tr, p, B, s))["qscale"][n, b])
         info, _, ref, _, grads = step_both(tr, L64, p, bt, s)
         errs = grad_errs(mc.engine_grads(tr, pols[p], p), grads, tol, "transition %d (agent %d) of %d" % (b, n, B))
@@ -466,7 +529,8 @@ def batch_size_sequence(args, tr, pols, L64, p, make, Bs, seed, rng, stats, rule
         res = []
         names = kernels_run(engine.lib(), stream, lambda: res.append(step_both(tr, L64, p, batch, seed + s)))
         pol = pols[p]
-        assert_row_kernels(names, spaces(rules, B, N, pol.obs_dim, pol.central_obs_dim + pol.central_act_dim), len(pols))
+        cin = pol.central_obs_dim + pol.central_act_dim
+        assert_row_kernels(names, spaces(rules, B, N, pol.obs_dim, cin), len(pols), {"critic": cin, "actor": pol.obs_dim})
         info, prio, ref, rprio, grads = res[0]
         errs = grad_errs(mc.clipped_engine_grads(tr, pols[p], ref, args.max_grad_norm, p), grads, tol, "step %d at B = %d" % (s, B))
         worst = max([worst] + list(errs.values()))
@@ -520,7 +584,7 @@ def run_case(engine, stream, rules, specs, S, discrete, td3, Bs, p="policy_0", a
         ulps = []
         names = kernels_run(engine.lib(), stream, lambda: ulps.append(per_transition_forward(tr, L64, p, batch, seed + B, rng, stats)))
         worst["td_ulps"] = max(worst["td_ulps"], ulps[0])
-        assert_row_kernels(names, sp, len(pols))
+        assert_row_kernels(names, sp, len(pols), {"critic": cin, "actor": O})
         if discrete:
             assert "k_act_transform" in names
         errs = isolated(tr, pols, L64, p, batch, pairs, sp, seed + 7 * B, rng, stats)

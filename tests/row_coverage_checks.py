@@ -84,6 +84,25 @@ def _front_bwd_smem_floats(in_dim, TM, gru_ext):         # agent_bwd.cu front_bw
 SMEM_BYTES = 227 * 1024
 
 
+def front_bwd_smem(in_dim, TM, gru_ext=False):
+    """k_front_bwd's dynamic shared memory in bytes (front_bwd_launch: front_bwd_smem's floats + 16).  gru_ext: k_gru_wgrad beside it
+    (the recurrent QMIX step).  The actor-critic learners run it without (the GRU's h_{t-1} / dgi_n * r tiles here): above 128 columns
+    only the 32-row tile fits, 162 KB at 155-192 columns, 186 KB up to 256, 211 KB up to 320."""
+    return _front_bwd_smem_floats(in_dim, TM, gru_ext) * 4 + 16
+
+
+def front_bwd_pick_rm(M, in_dim, sms, gru_ext=False):
+    """agent_bwd.cu front_bwd_pick_rm: 16 RM rows per tile, RM in 2..4, minimising waves x (1 + RM) over the heights that fit 227 KB."""
+    best, best_cost = 2, 1e30
+    for rm in (2, 3, 4):
+        if front_bwd_smem(in_dim, 16 * rm, gru_ext) > SMEM_BYTES:
+            continue
+        cost = _cdiv(_cdiv(M, 16 * rm), sms) * (1.0 + rm)
+        if cost < best_cost - 1e-9:
+            best, best_cost = rm, cost
+    return best
+
+
 def front_bwd_max_in_dim(gru_ext):
     """agent_bwd.cu mx_front_bwd_max_in_dim: the widest input whose 32-row k_front_bwd tile fits (384 with k_gru_wgrad beside it, as in
     the recurrent QMIX step; 320 without, as in M-QMIX and both MADDPG learners).  The learners refuse wider inputs at creation."""
@@ -132,15 +151,13 @@ class TileRules(object):
         self.sms = int(sms)
 
     def front_bwd_rm(self, M, in_dim, gru_ext):
-        """front_bwd_pick_rm: 16 RM rows per tile, RM in 2..4, minimising waves x (1 + RM) over the heights that fit 227 KB."""
-        best, best_cost = 2, 1e30
-        for rm in (2, 3, 4):
-            if _front_bwd_smem_floats(in_dim, 16 * rm, gru_ext) * 4 + 16 > SMEM_BYTES:
-                continue
-            cost = _cdiv(_cdiv(M, 16 * rm), self.sms) * (1.0 + rm)
-            if cost < best_cost - 1e-9:
-                best, best_cost = rm, cost
-        return best
+        return front_bwd_pick_rm(M, in_dim, self.sms, gru_ext)
+
+    def front_bwd_launch(self, M, in_dim, gru_ext=False):
+        """One k_front_bwd launch over M rows of width in_dim: (RM, grid, dynamic shared memory in bytes), as a captured graph node
+        shows it ("k_front_bwd<RM> grid=(grid, 1, 1) ... smem=bytes")."""
+        rm = self.front_bwd_rm(M, in_dim, gru_ext)
+        return rm, min(self.sms, _cdiv(M, 16 * rm)), front_bwd_smem(in_dim, 16 * rm, gru_ext)
 
     def bwd_tc_ctas_per_sm(self, in_dim):
         """k_front_bwd_tc streams its weight operands through one buffer; two CTAs per SM when twice that fits."""
@@ -150,7 +167,8 @@ class TileRules(object):
 
     def agent_rows(self, M, in_dim, gru_ext=True):
         """The row tiling {kernel: (rows per tile, tiles, grid)} of the backward's row kernels and of the forward (its grid per net).
-        gru_ext: the recurrent QMIX step, whose k_gru_wgrad runs beside k_front_bwd (M-QMIX has no GRU: False)."""
+        gru_ext: the recurrent QMIX step, whose k_gru_wgrad runs beside k_front_bwd; False for M-QMIX (no GRU) and for both actor-critic
+        learners, whose k_front_bwd computes the GRU weight gradients itself (R-MADDPG / R-MATD3) or has none (MLP MADDPG / MATD3)."""
         sms = self.sms
         out = {}
         if in_dim > 128:           # FFMA throughout: k_front_fwd<2> (32-row tiles, the two nets share the SMs); k_front_bwd and
@@ -168,10 +186,12 @@ class TileRules(object):
             nc = _cdiv(M, 64)
             out["k_wgrad_tc"] = (64, nc, min(sms, nc))
             out["k_front_fwd_tc_wide"] = (128, nt, min(sms, nt))
-        else:                      # k_front_bwd + k_gru_wgrad: same tile height and grid
-            TM = 16 * self.front_bwd_rm(M, in_dim, True)
+        else:                      # k_front_bwd (+ k_gru_wgrad in the recurrent QMIX step: same tile height and grid)
+            TM = 16 * self.front_bwd_rm(M, in_dim, gru_ext)
             nt = _cdiv(M, TM)
-            out["k_front_bwd"] = out["k_gru_wgrad"] = (TM, nt, min(sms, nt))
+            out["k_front_bwd"] = (TM, nt, min(sms, nt))
+            if gru_ext:
+                out["k_gru_wgrad"] = out["k_front_bwd"]
             nf = _cdiv(M, 128)
             out["k_front_fwd_tc"] = (128, nf, min(max(sms // 2, 1), nf))
         return out
@@ -285,36 +305,83 @@ def pick_mixer_shapes(rules, Ns=(2, 3), Ts=range(1, 40), Bs=range(1, 80)):
 MADDPG_TARGETS = ["critic one tile", "critic tail 1", "critic tail 31", "critic tiles = sms+1", "actor tail 1", "actor tail 31"]
 
 
-def pick_maddpg_shapes(rules, N=3, Ts=range(8, 40), Bs=range(1, 200)):
-    """R-MADDPG (B, T) with T >= 8 (the critic's k_gru_bwd2 stores T1 = T steps per sequence) on the edges of k_head_bwd's 32-row tiles:
-    critic rows Mc = B T and actor rows Ma = B (T+1) N.  Returns [(targets, (B, T, N), layout, note)], fewest rows first."""
-    def hits(B, T):
-        Mc, Ma = B * T, B * (T + 1) * N
-        h = set()
-        _, ntc, _ = rules.head_rows(Mc)
-        if ntc == 1:
-            h.add("critic one tile")
-        if Mc % 32 == 1:
-            h.add("critic tail 1")
-        if Mc % 32 == 31:
-            h.add("critic tail 31")
-        if ntc == rules.sms + 1:
-            h.add("critic tiles = sms+1")
-        if Ma % 32 == 1:
-            h.add("actor tail 1")
-        if Ma % 32 == 31:
-            h.add("actor tail 31")
-        return h
-    cands = sorted(((B * B * (T + 1) * N, (B, T)) for T in Ts for B in Bs))
+FRONT_TARGETS = ["one tile", "tail 1", "tail TM-1", "tiles = sms", "tiles = sms+1"]
+
+
+def maddpg_front_spaces(rules, B, T, N, obs, cin):
+    """R-MADDPG / R-MATD3's k_front_bwd row spaces {space: (rows, rows per tile, tiles)}: the critic's B T rows and the agent-replaced
+    copies' N B T rows at the critic's width, the actor's B (T+1) N rows at its own.  No k_gru_wgrad beside it (gru_ext False): the kernel
+    computes the GRU weight gradients itself.  Above 128 columns FFMA k_front_bwd on 32-row tiles; at 65-128 the actor's and critic's
+    weight gradients run on k_wgrad_tc instead, so only widths outside that band are k_front_bwd edges (the copies' at every width)."""
     out = {}
+    for name, M, w in (("critic", B * T, cin), ("copies", N * B * T, cin), ("actor", B * (T + 1) * N, obs)):
+        if name == "copies" or not 64 < w <= 128:
+            TM = 16 * rules.front_bwd_rm(M, w, False)
+            out[name] = (M, TM, _cdiv(M, TM))
+    return out
+
+
+def _front_edges(rules, M, TM, nt):
+    """The k_front_bwd edges (FRONT_TARGETS) one row space of M rows in nt tiles of TM hits."""
+    return {e for e, ok in (("one tile", nt == 1), ("tail 1", M % TM == 1), ("tail TM-1", M % TM == TM - 1),
+                            ("tiles = sms", nt == rules.sms), ("tiles = sms+1", nt == rules.sms + 1)) if ok}
+
+
+def _head_edges(rules, B, T, N):
+    """The k_head_bwd edges (MADDPG_TARGETS) of the critic's B T and the actor's B (T+1) N rows."""
+    Mc, Ma = B * T, B * (T + 1) * N
+    _, ntc, _ = rules.head_rows(Mc)
+    return {t for t, ok in (("critic one tile", ntc == 1), ("critic tail 1", Mc % 32 == 1), ("critic tail 31", Mc % 32 == 31),
+                            ("critic tiles = sms+1", ntc == rules.sms + 1), ("actor tail 1", Ma % 32 == 1), ("actor tail 31", Ma % 32 == 31))
+            if ok}
+
+
+def pick_maddpg_shapes(rules, N=3, Ts=range(8, 40), Bs=range(1, 200), obs=None, cin=None):
+    """R-MADDPG (B, T) on the edges of k_head_bwd's 32-row tiles, with T >= 8 (the critic's k_gru_bwd2 stores T1 = T steps per
+    sequence): critic rows Mc = B T and actor rows Ma = B (T+1) N.  With the widths obs / cin also on the k_front_bwd edges of each
+    space of maddpg_front_spaces (labelled "critic front tail 1", ...), and one shape with episodes shorter than 8 (k_gru_bwd's
+    short-sequence variant).  An edge no shape hits takes the nearest one that occurs, and the note says so: a tile count the tile rule
+    skips (the nearest count above), or an odd tail of a space whose row count is always even (the actor's and the copies' at even N:
+    the nearest tail).  Returns [(targets, (B, T, N), layout, note)], fewest rows first."""
+    cands = sorted(((B * B * (T + 1) * N, (B, T)) for T in Ts for B in Bs))
+    front = lambda B, T: maddpg_front_spaces(rules, B, T, N, obs, cin)
+    out, notes = {}, {}
+
+    def place(shape, label, note=None):
+        out.setdefault((shape[0], shape[1], N), []).append(label)
+        if note:
+            notes[label] = note
+
     for tgt in MADDPG_TARGETS:
-        for _, (B, T) in cands:
-            if tgt in hits(B, T):
-                out.setdefault((B, T, N), []).append(tgt)
-                break
-        else:
-            raise AssertionError("no R-MADDPG shape in the search space hits %r" % tgt)
-    return [(tg, shape, dict(Mc=shape[0] * shape[1], Ma=shape[0] * (shape[1] + 1) * N), "") for shape, tg in sorted(out.items())]
+        hit = next((bt for _, bt in cands if bt[1] >= 8 and tgt in _head_edges(rules, bt[0], bt[1], N)), None)
+        if hit is None and tgt.startswith("actor tail") and N % 2 == 0:
+            continue                      # B (T+1) N rows at even N: no odd tail; the k_front_bwd tails of the actor cover its last tile
+        assert hit is not None, "no R-MADDPG shape in the search space hits %r" % tgt
+        place(hit, tgt)
+    if cin is None:
+        return [(tg, shape, dict(Mc=shape[0] * shape[1], Ma=shape[0] * (shape[1] + 1) * N), "") for shape, tg in sorted(out.items())]
+    short = next((bt for _, bt in cands if bt[1] < 8), None)
+    assert short is not None, "no R-MADDPG shape with episodes shorter than 8 in the search space"
+    place(short, "T < 8")
+    for space in front(1, 8):
+        for e in FRONT_TARGETS:
+            label = "%s front %s" % (space, e)
+            lay = lambda bt: front(bt[0], bt[1])[space]
+            hit = next((bt for _, bt in cands if e in _front_edges(rules, *lay(bt))), None)
+            if hit is not None:
+                place(hit, label)
+            elif e.startswith("tail"):
+                tail = lambda bt: lay(bt)[0] % lay(bt)[1]
+                ok = [bt for _, bt in cands if tail(bt)]
+                hit = min(ok, key=(lambda bt: tail(bt)) if e == "tail 1" else (lambda bt: lay(bt)[1] - tail(bt)))
+                place(hit, label, "%s cannot occur (an even row count); nearest: a last tile of %d of %d rows at B %d T %d"
+                      % (label, tail(hit), lay(hit)[1], hit[0], hit[1]))
+            else:
+                want = rules.sms + (e == "tiles = sms+1")
+                hit = min((bt for _, bt in cands if lay(bt)[2] >= want), key=lambda bt: (lay(bt)[2] - want, bt[0] * bt[0] * (bt[1] + 1)))
+                place(hit, label, "%s cannot occur (tile rule); nearest: %d tiles" % (label, lay(hit)[2]))
+    return [(tg, shape, dict(Mc=shape[0] * shape[1], Ma=shape[0] * (shape[1] + 1) * N), "; ".join(notes[t] for t in tg if t in notes))
+            for shape, tg in sorted(out.items())]
 
 
 def sample_episodes(B, T, N, TM, grid, every_up_to=16):
@@ -416,12 +483,14 @@ def maddpg_pair(cfg, B, T):
 
 
 def maddpg_isolated_episodes(L64, pol, tr, batch, episodes, B, T, tol=None):
-    """R-MADDPG with one episode isolated per run, from the same state each time.  Critic: PER weights one-hot on episode b, so the
+    """R-MADDPG / R-MATD3 with one episode isolated per run, from the same state each time (R-MATD3: both critic heads, the target-action
+    noise drawn in the trainer's order, the actor only on the updates actor_update_interval selects).  Critic: PER weights one-hot on episode b, so the
     critic gradient is exactly episode b's T rows.  Actor: every agent of every other episode is done from its first step, so the actor
     loss keeps episode b's (T N) rows plus only the first step of the others (the per-agent mask lags the done flag by one step, the first
     step is always live).  Both clipped gradients against the float64 update.  Returns the worst relative error per tensor."""
     import copy
     import maddpg_checks as mc
+    from offpolicy._b200 import capi
     from oracle.maddpg import sample_gumbel
     tol = GRAD_TOL if tol is None else tol
     cfg, N = L64.cfg, L64.cfg.n_agents
@@ -434,22 +503,29 @@ def maddpg_isolated_episodes(L64, pol, tr, batch, episodes, B, T, tol=None):
         for v, v0 in zip(pol.actor_vecs + pol.critic_vecs, vec0):
             v.copy_(v0)
         tr.num_updates["policy_0"] = 0
+        capi.check(capi.lib().mx_maddpg_set_num_updates(tr._eng["policy_0"].handle, 0))     # the handle's own count picks the actor update
         L = copy.deepcopy(L0)
         w = np.zeros(B, np.float32)
         w[b] = 1.0
         dones = batch[4].copy()
         dones[:, :, [x for x in range(B) if x != b], :] = 1.0
         bt = tuple(batch[:4]) + (dones,) + tuple(batch[5:7]) + (w, np.arange(B))
+        # the trainer's draws from torch's CPU generator, in its order: R-MATD3's target-action noise over the T+1 steps, then (when
+        # this update trains the actor) the Discrete actor's Gumbel draws over the first T
+        update = tr.num_updates["policy_0"] % tr.actor_update_interval == 0
         torch.manual_seed(77 + b)
-        anoise = sample_gumbel((T, N * B, cfg.act_dim)).numpy() if cfg.discrete else None
-        torch.manual_seed(77 + b)                    # the trainer draws the actor's Gumbel noise from torch's CPU generator
+        tnoise = tr.draw_target_noise(B).numpy() if cfg.td3 else None
+        anoise = sample_gumbel((T, N * B, cfg.act_dim)).numpy() if cfg.discrete and update else None
+        torch.manual_seed(77 + b)
         info, _, _ = tr.shared_train_policy_on_batch("policy_0", mc.ref_tuple(bt))
         ga, gc = tr.grad_views()
-        ref, _ = L.step(bt, None, anoise)
-        assert bool(info["update_actor"]) and bool(ref["update_actor"])
+        ref, _ = L.step(bt, tnoise, anoise)
+        assert bool(info["update_actor"]) == bool(ref["update_actor"]) == update, (info["update_actor"], ref["update_actor"], update)
         errs = {}
-        for tag, flat, P, entries, grads, gn in (("critic", gc, pol.Pc, pol._c_entries, L.critic_grads, ref["critic_grad_norm"]),
-                                                  ("actor", ga, pol.Pa, pol._a_entries, L.actor_grads, ref["actor_grad_norm"])):
+        nets = [("critic", gc, pol.Pc, pol._c_entries, L.critic_grads, ref["critic_grad_norm"])]
+        if update:
+            nets.append(("actor", ga, pol.Pa, pol._a_entries, L.actor_grads, ref["actor_grad_norm"]))
+        for tag, flat, P, entries, grads, gn in nets:
             coef = min(1.0, cfg.max_grad_norm / (float(gn) + 1e-6))
             views = mc.named_views(flat.detach().cpu().double(), entries)
             den = float(flat[P])

@@ -15,7 +15,8 @@ SPREAD = [(18, 5, 3)]
 
 def _check(worst, stats):
     assert worst["grad"] <= rk.GRAD_TOL and worst["td_ulps"] <= rk.TD_ULPS
-    print("worst", worst, "redraws", stats["redraws"], "smallest margin kept %.2e" % stats.get("min_margin", float("inf")))
+    print("worst", worst, "redraws", stats["redraws"], "of them ill-conditioned", stats.get("ill_conditioned", 0),
+          "smallest margin kept %.2e" % stats.get("min_margin", float("inf")))
 
 
 EDGES = rk.pick_batches(RULES, 3, 18, 69)
@@ -78,6 +79,63 @@ MULTI = {
 def test_isolated_transitions_several_policies(emu_engine, name):
     specs, S, p, td3 = MULTI[name]
     _check(*rk.run_case(emu_engine, None, RULES, specs, S, True, td3, [7], p=p))
+
+
+# Above 128 input columns (tc_bwd.cu WG_MAX_IN) a net runs FFMA k_front_fwd forward and FFMA k_front_bwd backward on 32-row tiles of
+# round_up(in, 64)-wide shared-memory rows (162 KB at 155-192 columns, 186 KB up to 256, 211 KB up to 320, the widest the learner takes).
+# simple_spread with N agents and N landmarks (--num_agents / --num_landmarks): observation 6 N, shared observation 6 N^2, critic input
+# 6 N^2 + 5 N -- 175 at N = 5, 246 at N = 6 (329 at N = 7 is refused).  Every batch size on an edge of the case's three row spaces.
+# (specs, S, discrete, td3, avail, policies isolated)
+WIDE = {
+    "spread5_matd3_disc": ([(30, 5, 5)], 150, True, True, False, ["policy_0"]),
+    "spread6_maddpg_disc_next_avail": ([(36, 5, 6)], 216, True, False, True, ["policy_0"]),
+    "spread5_maddpg_box": ([(30, 5, 5)], 150, False, False, False, ["policy_0"]),
+    "critic320_matd3_disc": ([(30, 5, 5)], 295, True, True, False, ["policy_0"]),
+    "actor132_maddpg_disc": ([(132, 5, 2)], 20, True, False, False, ["policy_0"]),
+    # one policy per agent: policy_0 writes the first action columns, policy_4 the last (act_offset 20)
+    "spread5_per_agent_matd3_disc": ([(30, 5, 1)] * 5, 150, True, True, False, ["policy_0", "policy_4"]),
+}
+
+
+def edge_tag(edges):
+    tag = {"one tile": "one", "tail 1": "tail1", "tail TM-1": "tailTMm1", "tiles = sms": "sms", "tiles = sms+1": "smsp1"}
+    return "_".join(e.split(" ", 1)[0] + "_" + tag[e.split(" ", 1)[1]] for e in edges)
+
+
+def wide_params(rules, Bmax=None):
+    """(case, policy, B) per batch size on an edge of that policy's row spaces (B <= Bmax(case), every edge when Bmax is None), the id
+    naming the edges."""
+    out = []
+    for name, (specs, S, disc, td3, avail, ps) in WIDE.items():
+        for p in ps:
+            for B, tg, note in rk.pick_batches(rules, *rk.geometry(specs, S, p)):
+                if Bmax is None or B <= Bmax(name):
+                    out.append(pytest.param(name, p, B, id="%s-%s-B%d-%s" % (name, p, B, edge_tag(tg))))
+    return out
+
+
+def test_wide_edges_cover_every_row_space():
+    """Above 128 columns the critic's and the copies' row kernel is k_front_bwd on 32-row tiles, and every (row space, edge) of each
+    wide case has a batch size.  At the parent commit row_tiles looked up k_wgrad_tc there and raised KeyError."""
+    for name, (specs, S, disc, td3, avail, ps) in WIDE.items():
+        for p in ps:
+            N, O, cin = rk.geometry(specs, S, p)
+            for B in (1, 31, 97, 129):
+                sp = rk.spaces(RULES, B, N, O, cin)
+                for space, w in (("critic", cin), ("copies", cin), ("actor", O)):
+                    if w > 128:
+                        assert sp[space][1:3] == ("k_front_bwd", 32), (name, space, B, sp[space])
+            got = {t for _, tg, _ in rk.pick_batches(RULES, N, O, cin) for t in tg}
+            assert got == {s + " " + e for s in ("critic", "actor", "copies") for e in rk.EDGE_TARGETS}, (name, p, got)
+
+
+# Emulated: simple_spread N = 5 MATD3 at every edge up to B 31 (the copies' and the actor's sms / sms + 1 tiles, the critic's 31-row
+# tail); the other cases up to B 11.  The critic's sms / sms + 1 tiles (B 97 / 129 here) and every other edge run on the device.
+@pytest.mark.parametrize("name,p,B", wide_params(RULES, lambda name: 31 if name == "spread5_matd3_disc" else 11))
+def test_isolated_transitions_above_128_columns(emu_engine, name, p, B):
+    specs, S, disc, td3, avail, _ = WIDE[name]
+    worst, stats = rk.run_case(emu_engine, None, RULES, specs, S, disc, td3, [B], p=p, avail=avail)
+    _check(worst, stats)
 
 
 @pytest.mark.parametrize("td3", [False, True])

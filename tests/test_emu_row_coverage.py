@@ -188,9 +188,11 @@ def _maddpg_cases():
             for tg, (B, T, N), lay, note in rc.pick_maddpg_shapes(RULES) for disc in (False, True)]
 
 
-def run_maddpg(engine, disc, B, T, N, stream=None, every_up_to=16, rules=RULES):
+def run_maddpg(engine, disc, B, T, N, stream=None, every_up_to=16, rules=RULES, td3=False, obs=None, S=None):
     from oracle.maddpg import MaddpgConfig, synth_batch_cont, synth_batch_disc
-    cfg = MaddpgConfig(n_agents=N, act_dim=5 if disc else 2, discrete=disc, gain=1.0, use_per=True)
+    kw = {} if obs is None else dict(obs_dim=obs, state_dim=S)
+    cfg = MaddpgConfig(n_agents=N, act_dim=5 if disc else 2, discrete=disc, td3=td3, actor_update_interval=2 if td3 else 1, gain=1.0,
+                       use_per=True, **kw)      # R_MATD3 trains the actor on every second update
     L64, pol, tr = rc.maddpg_pair(cfg, B, T)
     batch = (synth_batch_disc if disc else synth_batch_cont)(cfg, B, T, seed=40) + (None, None)
     batch = rc.last_episode_full_length(batch)
@@ -198,10 +200,68 @@ def run_maddpg(engine, disc, B, T, N, stream=None, every_up_to=16, rules=RULES):
     eps = rc.sample_episodes(B, T - 1, 1, 32, grid, every_up_to=every_up_to)       # critic rows: T per episode
     names = rc.kernels_run(engine.lib(), stream, lambda: rc.maddpg_isolated_episodes(L64, pol, tr, batch, eps[:1], B, T))
     rc.assert_kernels_ran(names, ["k_head_bwd", "k_gru_bwd", "k_front_bwd"])
+    cin = cfg.state_dim + N * cfg.act_dim
+    if cin > 128:          # FFMA forward and backward for the critic and its copies; the actor (<= 64 or > 128 here) on k_front_bwd too
+        assert "k_front_fwd" in names and not {"k_front_bwd_tc", "k_wgrad_tc"} & set(names), names
+    if cin > 128 and cfg.obs_dim > 128:     # every net above 128 columns: no tensor-core forward anywhere in the step
+        assert not [k for k in names if k.startswith("k_front_fwd_tc")], names
     worst = rc.maddpg_isolated_episodes(L64, pol, tr, batch, eps, B, T)
     k = max(worst, key=worst.get)
-    print("R-MADDPG %s B %d T %d N %d (critic rows %d, actor rows %d): %d episodes isolated; worst gradient %s %.2e (bound %.0e)"
-          % ("Discrete" if disc else "Box", B, T, N, B * T, B * (T + 1) * N, len(eps), k, worst[k], rc.GRAD_TOL))
+    print("R-%s %s obs %d critic %d B %d T %d N %d (critic rows %d, actor rows %d): %d episodes isolated; worst gradient %s %.2e (bound %.0e)"
+          % ("MATD3" if td3 else "MADDPG", "Discrete" if disc else "Box", cfg.obs_dim, cin, B, T, N, B * T, B * (T + 1) * N, len(eps), k,
+             worst[k], rc.GRAD_TOL))
+    return worst
+
+
+# R-MADDPG / R-MATD3 above 128 critic columns (FFMA k_front_fwd / k_front_bwd on 32-row tiles, the GRU weight gradients inside
+# k_front_bwd, the copies' data gradient through the critic's input LayerNorm): name: (N, obs, S, Discrete, TD3)
+MADDPG_WIDE = {
+    "spread5_rmaddpg_disc_critic175": (5, 30, 150, True, False),
+    "spread6_rmatd3_box_critic228": (6, 36, 216, False, True),
+    "actor140_critic316_rmaddpg_disc": (3, 140, 301, True, False),
+    "critic320_rmatd3_disc": (5, 30, 295, True, True),
+}
+
+
+def maddpg_wide_params(rules, keep=lambda B, T: True):
+    """(case, B, T) per shape on the k_head_bwd and k_front_bwd edges of the case's row spaces (episodes of 4 to 39 steps: T < 8 runs
+    k_gru_bwd's short-sequence variant, T >= 8 k_gru_bwd2), the id naming the edges."""
+    out = []
+    short = lambda t: t.replace("front ", "").replace("tiles = sms+1", "smsp1").replace("tiles = sms", "sms").replace("tail TM-1", "tailTMm1") \
+        .replace("one tile", "one").replace(" ", "")
+    for name, (N, obs, S, disc, td3) in MADDPG_WIDE.items():
+        cin = S + N * (5 if disc else 2)
+        for tg, (B, T, _), lay, note in rc.pick_maddpg_shapes(rules, N=N, Ts=range(4, 40), Bs=range(1, 200), obs=obs, cin=cin):
+            if keep(B, T):
+                out.append(pytest.param(name, B, T, id="%s-B%d-T%d-%s" % (name, B, T, "_".join(sorted({short(t) for t in tg})))))
+    return out
+
+
+def test_maddpg_wide_shapes_cover_every_edge():
+    """Each wide case has shapes on every k_front_bwd edge of its three spaces (an edge that cannot occur -- the odd tails of the actor's
+    and the copies' rows at an even agent count, a tile count the tile rule skips -- on the nearest one, named in the note), episodes
+    shorter than 8 among them, and 32-row tiles wherever a space is above 128 columns."""
+    for name, (N, obs, S, disc, td3) in MADDPG_WIDE.items():
+        cin = S + N * (5 if disc else 2)
+        shapes = rc.pick_maddpg_shapes(RULES, N=N, Ts=range(4, 40), Bs=range(1, 200), obs=obs, cin=cin)
+        got = {t for tg, _, _, _ in shapes for t in tg}
+        notes = " ".join(n for _, _, _, n in shapes)
+        assert "T < 8" in got, name
+        for space in ("critic", "actor", "copies"):
+            for e in rc.FRONT_TARGETS:
+                assert "%s front %s" % (space, e) in got, (name, space, e)
+        for space in ("actor", "copies"):
+            for e in ("tail 1", "tail TM-1"):
+                assert ("%s front %s cannot occur (an even row count)" % (space, e) in notes) == (N % 2 == 0), (name, space, e, notes)
+        for space, (M, TM, nt) in rc.maddpg_front_spaces(RULES, 3, 9, N, obs, cin).items():
+            assert TM == 32 or (space == "actor" and obs <= 64), (name, space, TM)
+
+
+@pytest.mark.parametrize("name,B,T", maddpg_wide_params(RULES, keep=lambda B, T: B == 1 and T <= 20))
+def test_maddpg_isolated_episodes_above_128_columns(emu_engine, name, B, T):
+    """Emulated: the one-episode shapes up to T 20 (one tile, the tails, T < 8); the multi-tile edges run on the device."""
+    N, obs, S, disc, td3 = MADDPG_WIDE[name]
+    run_maddpg(emu_engine, disc, B, T, N, td3=td3, obs=obs, S=S)
 
 
 @pytest.mark.parametrize("disc,B,T,N", _maddpg_cases())
@@ -224,3 +284,14 @@ def test_two_actions_per_lane_in_the_fused_mid_kernel(emu_engine, act):
     assert "k_mid" in names and "k_front_fwd_tc" in names and "k_front_fwd_tc1" not in names, names
     rc.isolated_episode_gradients(L64, tr, batch, list(range(B)), B, T, N)
     rc.per_row_forward(L64, tr, batch, B, T, N, False)
+
+
+@pytest.mark.parametrize("td3", [False, True], ids=["rmaddpg", "rmatd3"])
+def test_maddpg_oracle_lockstep_above_128_columns(emu_engine, td3):
+    """Whole R-MADDPG / R-MATD3 updates at simple_spread N = 5 (critic 175), three in a row, against the fp32 oracle (the H100 runs
+    the script's B 32, T 25)."""
+    import maddpg_checks as mdc
+    from oracle.maddpg import MaddpgConfig
+    cfg = MaddpgConfig(n_agents=5, obs_dim=30, act_dim=5, state_dim=150, discrete=True, td3=td3, actor_update_interval=2 if td3 else 1,
+                       gain=1.0, use_per=True)
+    print("worst gradient / bound %.2f" % mdc.check_oracle_lockstep(cfg, 3, 9))

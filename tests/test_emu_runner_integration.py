@@ -59,6 +59,9 @@ RUNS = {
     "rmatd3_no_feature_norm": ("rmatd3", 100, ["--actor_train_interval_step", "1", "--use_feature_normalization"], True),
     "mlp_maddpg": ("maddpg", 100, ["--runner", "mlp"], True),
     "mlp_matd3": ("matd3", 100, ["--runner", "mlp"], True),
+    # simple_spread with 5 agents (3 landmarks): observation 26, shared observation 130, critic input 130 + 5 x 5 = 155 -- above 128
+    # columns, FFMA k_front_fwd / k_front_bwd on 32-row tiles for the critic and its agent-replaced copies
+    "mlp_maddpg_5_agents": ("maddpg", 100, ["--runner", "mlp", "--agents", "5"], True),
 }
 
 

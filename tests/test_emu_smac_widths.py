@@ -7,6 +7,7 @@ SMAC observation widths with the reference env's defaults (obs_last_action, obs_
 that restatement, the others run the isolated-episode gradients, the per-row forward and the per-transition mixer values on its edges."""
 import numpy as np
 import pytest
+import torch
 
 import row_coverage_checks as rc
 
@@ -127,6 +128,16 @@ def test_input_width_limit_refused_at_creation(emu_engine):
     mdc.build(MaddpgConfig(n_agents=3, obs_dim=20, act_dim=5, state_dim=305, discrete=True), 2, 8)
     _refused(emu_engine, lambda: mdc.build(MaddpgConfig(n_agents=3, obs_dim=20, act_dim=5, state_dim=306, discrete=True), 2, 8), 321, 320)
     _refused(emu_engine, lambda: mdc.build(MaddpgConfig(n_agents=3, obs_dim=321, act_dim=5, state_dim=30, discrete=True), 2, 8), 321, 320)
+    # MLP MADDPG / MATD3 at simple_spread with N agents and N landmarks: critic input 6 N^2 + 5 N -- N = 7 gives 294 + 35 = 329, refused;
+    # the 320-column critic (295 + 5 x 5) builds and takes a step
+    import mlp_maddpg_checks as mlc
+    from offpolicy._b200.factory import build_mlp_maddpg
+    for td3 in (False, True):
+        _refused(emu_engine, lambda: build_mlp_maddpg(7, 42, 5, 294, 4, discrete=True, td3=td3), 329, 320)
+        torch.manual_seed(2)
+        args, pol, tr = build_mlp_maddpg(5, 30, 5, 295, 4, discrete=True, td3=td3)
+        info, _, _ = tr.shared_train_policy_on_batch("policy_0", mlc.synth_batch(np.random.default_rng(3), 5, 4, 30, 295, 5, True))
+        assert all(np.isfinite(float(info[k])) for k in ("critic_loss", "actor_loss")), info
 
 
 # ---- wide inputs -------------------------------------------------------------------------------------------------------------

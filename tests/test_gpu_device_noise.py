@@ -44,6 +44,9 @@ UPDATES = {
     "matd3_box": Case("mlp", [(3, 18, 2)], td3=True, discrete=False, **BIG),
     "rmatd3_spread": Case("rec", [(3, 18, 2)], S=54, B=32, E=5000, T=25, td3=True, discrete=False, rng="device", insert=0),
     "rmatd3_spread_disc": Case("rec", [(3, 18, 5)], S=54, B=32, E=5000, T=25, td3=True, rng="device", insert=0),
+    # simple_spread with 5 agents and 5 landmarks: critic input 150 + 25 = 175, above 128 columns (FFMA k_front_fwd / k_front_bwd)
+    "matd3_spread5_critic175": Case("mlp", [(5, 30, 5)], td3=True, **dict(BIG, S=150)),
+    "rmatd3_spread5_critic175": Case("rec", [(5, 30, 5)], S=150, B=32, E=5000, T=25, td3=True, rng="device", insert=0),
 }
 
 
@@ -52,7 +55,7 @@ def test_device_updates_equal_host_updates_fed_the_device_draws(gpu_engine, name
     dn.check_updates(UPDATES[name], 3)
 
 
-GRAPH = ["matd3_reference", "matd3_box", "rmatd3_spread", "rmatd3_spread_disc"]
+GRAPH = ["matd3_reference", "matd3_box", "rmatd3_spread", "rmatd3_spread_disc", "matd3_spread5_critic175", "rmatd3_spread5_critic175"]
 
 
 @pytest.mark.parametrize("name", GRAPH)

@@ -8,6 +8,7 @@ pytestmark = pytest.mark.gpu
 
 SL = [(1, 3, 3), (1, 11, 5)]                 # simple_speaker_listener: speaker obs 3 / Discrete(3), listener obs 11 / Discrete(5)
 SPREAD = [(1, 18, 5)] * 3                    # simple_spread, one policy per agent
+SPREAD5 = [(1, 30, 5)] * 5                   # simple_spread with 5 agents and 5 landmarks, one policy per agent
 # (case, device noise): train_mpe_rmaddpg.sh shapes (episode 25, batch 32, 5 000-episode store); MLP at batch 1 000 from 100 000
 # transitions
 CASES = {
@@ -17,6 +18,9 @@ CASES = {
     "matd3_speaker_listener_per": (BatchCase("mlp", SL, S=14, B=1000, E=100000, td3=True, per=True, rng="device"), True),
     "maddpg_spread_per": (BatchCase("mlp", SPREAD, S=54, B=1000, E=100000, per=True, rng="device"), True),
     "matd3_spread_per": (BatchCase("mlp", SPREAD, S=54, B=1000, E=100000, td3=True, per=True, rng="device"), True),
+    # simple_spread with 5 agents and 5 landmarks, one policy per agent: critic input 150 + 25 = 175 (FFMA k_front_fwd / k_front_bwd)
+    "matd3_spread5_per_agent_per": (BatchCase("mlp", SPREAD5, S=150, B=1000, E=100000, td3=True, per=True, rng="device"), True),
+    "rmatd3_spread5_per_agent": (BatchCase("rec", SPREAD5, S=150, B=32, E=5000, T=25, td3=True, rng="device"), True),
 }
 
 

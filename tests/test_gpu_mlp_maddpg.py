@@ -29,11 +29,11 @@ def test_lockstep_small(gpu_engine, discrete, td3, avail, over):
     mc.lockstep(args, pol, tr, [mc.synth_batch(rng, N, 32, O, S, A, discrete, avail=avail, ties=avail, per=args.use_per) for _ in range(3)])
 
 
-def _filled_buffer(B, size, discrete, seed):
+def _filled_buffer(B, size, discrete, seed, N=N, O=O, S=S, A=A):
     from offpolicy._b200.factory import Box, Discrete
     from offpolicy.utils.mlp_buffer import MlpReplayBuffer
     info = {"policy_0": dict(obs_space=Box(O), share_obs_space=Box(S), act_space=Discrete(A) if discrete else Box(A))}
-    buf = MlpReplayBuffer(info, {"policy_0": [0, 1, 2]}, size, True, False, max_batch=B)
+    buf = MlpReplayBuffer(info, {"policy_0": list(range(N))}, size, True, False, max_batch=B)
     rng = np.random.default_rng(seed)
     for _ in range(size // B):
         b = mc.synth_batch(rng, N, B, O, S, A, discrete)
@@ -48,11 +48,24 @@ def _filled_buffer(B, size, discrete, seed):
 def test_lockstep_train_mpe_maddpg_sizes(gpu_engine, discrete, td3):
     """B = 1000 from 100 000 stored transitions; the batch is the replay's device batch (valid_transition read through its indices).
     Losses to 1e-3; parameters to two Adam steps of lr (a gradient element within round-off of zero may take either sign)."""
+    _lockstep_b1000(discrete, td3, N, O, S)
+
+
+# simple_spread with N agents and N landmarks: observation 6 N, shared observation 6 N^2, critic input 6 N^2 + 5 N = 175 at N = 5 and 246
+# at N = 6 -- FFMA k_front_fwd / k_front_bwd on 32-row tiles for the critic and the agent-replaced copies
+@pytest.mark.parametrize("n_agents", [5, 6], ids=["spread5_critic175", "spread6_critic246"])
+@pytest.mark.parametrize("td3", [False, True], ids=["maddpg", "matd3"])
+def test_lockstep_simple_spread_above_128_columns(gpu_engine, n_agents, td3):
+    """Three whole updates at B = 1 000 from 100 000 stored transitions against the fp32 oracle, as at simple_spread's 3 agents."""
+    _lockstep_b1000(True, td3, n_agents, 6 * n_agents, 6 * n_agents * n_agents)
+
+
+def _lockstep_b1000(discrete, td3, N, O, S):
     from offpolicy._b200.factory import build_mlp_maddpg
     B = 1000
     torch.manual_seed(8)
     args, pol, tr = build_mlp_maddpg(N, O, A, S, B, discrete=discrete, td3=td3)
-    buf = _filled_buffer(B, 100_000, discrete, 9)
+    buf = _filled_buffer(B, 100_000, discrete, 9, N, O, S)
     np.random.seed(10)
     L = mc.oracle_from(args, pol)
     # one device batch at a time: a later sample() reuses the batch region

@@ -17,7 +17,8 @@ def _rules():
 
 def _check(worst, stats):
     assert worst["grad"] <= rk.GRAD_TOL and worst["td_ulps"] <= rk.TD_ULPS
-    print("worst", worst, "redraws", stats["redraws"], "smallest margin kept %.2e" % stats.get("min_margin", float("inf")))
+    print("worst", worst, "redraws", stats["redraws"], "of them ill-conditioned", stats.get("ill_conditioned", 0),
+          "smallest margin kept %.2e" % stats.get("min_margin", float("inf")))
 
 
 def test_simple_spread_matd3_edges(gpu_engine):
@@ -76,3 +77,67 @@ def test_batch_size_changes_on_one_learner(gpu_engine, td3):
                                    np.random.default_rng(5), stats, R, gpu_engine, gpu_engine.stream_ptr())
     assert worst <= rk.GRAD_TOL
     print("worst", worst, "redraws", stats["redraws"])
+
+
+def _wide_params():
+    """Every edge of simple_spread N = 5 MATD3 and of the 320-column critic (the critic's sms / sms + 1 tiles need B 4 193 / 4 225 at
+    132 SMs); the other wide cases up to B 1 100; and B = 1 000 for every case."""
+    import test_emu_mlp_maddpg_rows as er
+    if not torch.cuda.is_available():
+        return [pytest.param("none", "policy_0", 1, id="no-device")]
+    every = ("spread5_matd3_disc", "critic320_matd3_disc")
+    out = er.wide_params(_rules(), lambda name: 10 ** 9 if name in every else 1100)
+    for name, v in er.WIDE.items():
+        for p in v[5]:
+            out.append(pytest.param(name, p, 1000, id="%s-%s-B1000" % (name, p)))
+    return out
+
+
+@pytest.mark.parametrize("name,p,B", _wide_params())
+def test_isolated_transitions_above_128_columns(gpu_engine, name, p, B):
+    """Critic (and one actor) inputs above 128 columns: FFMA k_front_fwd / k_front_bwd on 32-row tiles of 162-211 KB, every isolated
+    pair in its space's last tile on the device's own grid (tests/test_emu_mlp_maddpg_rows.py WIDE)."""
+    import test_emu_mlp_maddpg_rows as er
+    specs, S, disc, td3, avail, _ = er.WIDE[name]
+    worst, stats = rk.run_case(gpu_engine, gpu_engine.stream_ptr(), _rules(), specs, S, disc, td3, [B], p=p, avail=avail)
+    print("%s %s B %d:" % (name, p, B), end=" ")
+    _check(worst, stats)
+
+
+@pytest.mark.parametrize("N,S,td3,disc", [(5, 150, True, True), (6, 216, False, True), (5, 295, True, True)],
+                         ids=["spread5_matd3_critic175", "spread6_maddpg_critic246", "critic320_matd3"])
+def test_wide_launches_match_the_tile_rules(gpu_engine, N, S, td3, disc):
+    """Every k_front_bwd launch of one captured MLP update at the batch sizes of the wide edges has the tile height, grid and dynamic
+    shared memory the Python tile rules restate (front_bwd_pick_rm / front_bwd_smem without k_gru_wgrad): critic B rows and the
+    agent-replaced copies N B rows at the critic's width, the actor's 2 B N rows at its own -- so the edges the isolated checks pick are
+    the ones the device runs."""
+    from checkpoint_maddpg_checks import Case
+    from offpolicy._b200.torch_rng import DeviceTorchGenerator
+    from test_gpu_launch_config import graph_configs
+    R = _rules()
+    O, cin = 6 * N, S + 5 * N
+    for B in sorted({B for B, _, _ in rk.pick_batches(R, N, O, cin) if B <= 1024}):      # the replay samples at most 1 024
+        case = Case(kind="mlp", specs=[(N, O, 5)], S=S, B=B, E=B + 64, td3=td3, discrete=disc, rng="device")
+        tr, buf, pols = case.build(1)
+        case.fill(buf, np.random.RandomState(5), case.E)
+        torch.manual_seed(11)
+        tr.use_device_noise(DeviceTorchGenerator(seed=3))
+        smp = buf.sample(B)
+        for _ in range(2):
+            tr.train_policy_on_batch("policy_0", smp)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph(keep_graph=True)
+        with torch.cuda.graph(g):
+            tr.train_policy_on_batch("policy_0", smp)
+        try:
+            nodes, _ = graph_configs(g.raw_cuda_graph())
+        finally:
+            g.reset()
+            torch.cuda.synchronize()
+        # critic above 128 columns, actor below 65: all three spaces on k_front_bwd
+        want = ["k_front_bwd<%d> grid=(%d, 1, 1) block=(256, 1, 1) smem=%d" % R.front_bwd_launch(M, w)
+                for M, w in ((B, cin), (N * B, cin), (2 * B * N, O))]
+        got = [n for n in nodes if n.startswith("k_front_bwd<")]
+        assert sorted(got) == sorted(want), (B, got, want)
+        assert not any(n.split(" ")[0] in ("k_front_bwd_tc", "k_wgrad_tc") for n in nodes), (B, nodes)
+        print("B %d:" % B, got)

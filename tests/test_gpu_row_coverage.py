@@ -157,3 +157,71 @@ def _maddpg_gpu_cases():
 def test_maddpg_isolated_episode_gradients(gpu_engine, oracle_threads, disc, B, T, N):
     """R-MADDPG critic and actor, Box and Discrete, T >= 8, on the edges of k_head_bwd's 32-row tiles at this device's SM count."""
     ec.run_maddpg(gpu_engine, disc, B, T, N, stream=gpu_engine.stream_ptr(), rules=_rules())
+
+
+def _maddpg_wide_gpu_cases():
+    if not torch.cuda.is_available():
+        return [pytest.param("none", 1, 8, id="no-device")]
+    return ec.maddpg_wide_params(_rules())
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,B,T", _maddpg_wide_gpu_cases())
+def test_maddpg_isolated_episodes_above_128_columns(gpu_engine, oracle_threads, name, B, T):
+    """R-MADDPG / R-MATD3 above 128 critic columns (tests/test_emu_row_coverage.py MADDPG_WIDE) on every k_head_bwd and k_front_bwd edge
+    of the critic's, the actor's and the copies' row spaces at this device's SM count, episodes shorter than 8 steps and longer."""
+    N, obs, S, disc, td3 = ec.MADDPG_WIDE[name]
+    ec.run_maddpg(gpu_engine, disc, B, T, N, stream=gpu_engine.stream_ptr(), rules=_rules(), td3=td3, obs=obs, S=S)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("disc", [True, False], ids=["disc", "box"])
+def test_rmatd3_oracle_lockstep_simple_spread5(gpu_engine, oracle_threads, disc):
+    """R-MATD3 whole updates at simple_spread N = 5 (critic 150 + 5 x act columns) and the script's B 32, T 25, three in a row against
+    the fp32 oracle."""
+    import maddpg_checks as mdc
+    from oracle.maddpg import MaddpgConfig
+    cfg = MaddpgConfig(n_agents=5, obs_dim=30, act_dim=5 if disc else 2, state_dim=150, discrete=disc, td3=True, actor_update_interval=2,
+                       gain=1.0, use_per=True)
+    print("worst gradient / bound %.2f" % mdc.check_oracle_lockstep(cfg, 32, 25))
+
+
+@pytest.mark.gpu
+def test_maddpg_wide_launches_match_the_tile_rules(gpu_engine):
+    """Every k_front_bwd launch of one captured R-MADDPG update at simple_spread N = 5 (critic 175) has the tile height, grid and dynamic
+    shared memory that maddpg_front_spaces restates -- the critic's B T and the copies' N B T rows at 175 columns, the actor's B (T+1) N
+    at 30, no k_gru_wgrad beside it -- at the shapes of the wide cases' edges, so those edges are the ones the device runs; and the
+    critic's launches run no tensor-core kernel."""
+    from checkpoint_maddpg_checks import Case
+    from offpolicy._b200.torch_rng import DeviceTorchGenerator
+    from test_gpu_launch_config import graph_configs
+    R = _rules()
+    N, obs, S = 5, 30, 150
+    cin = S + 5 * N
+    shapes = sorted({(B, T) for tg, (B, T, _), _, _ in rc.pick_maddpg_shapes(R, N=N, Ts=range(4, 40), Bs=range(1, 200), obs=obs, cin=cin)})
+    for B, T in shapes:
+        case = Case(kind="rec", specs=[(N, obs, 5)], S=S, B=B, E=max(64, 2 * B), T=T, rng="device")
+        tr, buf, pols = case.build(1)
+        case.fill(buf, np.random.RandomState(5), case.E)
+        torch.manual_seed(11)
+        tr.use_device_noise(DeviceTorchGenerator(seed=3))
+        smp = buf.sample(B)
+        for _ in range(2):
+            tr.train_policy_on_batch("policy_0", smp)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph(keep_graph=True)
+        with torch.cuda.graph(g):
+            tr.train_policy_on_batch("policy_0", smp)
+        try:
+            nodes, _ = graph_configs(g.raw_cuda_graph())
+        finally:
+            g.reset()
+            torch.cuda.synchronize()
+        sp = rc.maddpg_front_spaces(R, B, T, N, obs, cin)
+        want = ["k_front_bwd<%d> grid=(%d, 1, 1) block=(256, 1, 1) smem=%d" % R.front_bwd_launch(M, cin if name != "actor" else obs)
+                for name, (M, TM, nt) in sp.items()]
+        got = [n for n in nodes if n.startswith("k_front_bwd<")]
+        assert sorted(got) == sorted(want), (B, T, got, want)
+        assert not any(n.split(" ")[0] in ("k_front_bwd_tc", "k_wgrad_tc", "k_gru_wgrad<2>", "k_gru_wgrad<3>", "k_gru_wgrad<4>")
+                       for n in nodes), (B, T, nodes)
+        print("B %d T %d:" % (B, T), got)
