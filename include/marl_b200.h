@@ -89,7 +89,7 @@ typedef struct mx_replay_layout {
   int64_t off_b_idx;                        /* int64 [max_batch]   sampled episode indices             */
   int64_t off_b_weights;                    /* fp64  [max_batch]   PER importance weights              */
   int64_t off_b_wf32;                       /* fp32  [max_batch]   same, as consumed by the learner    */
-  int64_t off_rstats;                       /* fp64 [4]: masked reward sum, sumsq, count, pad          */
+  int64_t off_rstats;                       /* fp64 [4]: masked sum, sumsq of r - K, count, K          */
   int32_t tree_cap;                         /* next pow2 >= capacity                                   */
   int64_t total_bytes;
 } mx_replay_layout;

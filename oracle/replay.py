@@ -127,20 +127,16 @@ class SegTree(object):
         return rec(start, end, 1, 0, self.cap - 1)
 
     def find_prefixsum(self, mass):
-        """Root->leaf descent; `value[left] <= mass` goes right (segment_tree.py:130-146)."""
-        mass = np.array(mass, dtype=np.float64)
-        out = np.empty(mass.shape, dtype=np.int64)
-        for j in range(mass.size):
-            node, m = 1, mass[j]
-            while node < self.cap:
-                left = 2 * node
-                if self.v[left] <= m:
-                    m -= self.v[left]
-                    node = left + 1
-                else:
-                    node = left
-            out[j] = node - self.cap
-        return out
+        """Root->leaf descent; `value[left] <= mass` goes right (segment_tree.py:130-146).  All masses descend together, one tree level
+        per step: the same comparisons and subtractions, in the same order, as one descent per mass."""
+        m = np.array(mass, dtype=np.float64).reshape(-1)
+        node = np.ones(m.shape, dtype=np.int64)
+        while node.size and node[0] < self.cap:      # every leaf is at the same depth
+            lv = self.v[2 * node]
+            right = lv <= m
+            m = np.where(right, m - lv, m)
+            node = 2 * node + right
+        return (node - self.cap).reshape(np.shape(mass))
 
 
 class UniformReplay(object):
