@@ -380,7 +380,8 @@ int mx_maddpg_set_valid(mx_maddpg* h, const float* valid_dev);
 int64_t mx_maddpg_num_updates(const mx_maddpg* h);   /* updates done so far (self.num_updates[p_id], r_maddpg.py:125) */
 int mx_maddpg_set_num_updates(mx_maddpg* h, int64_t n);   /* restore the update count (checkpoint resume); n >= 0 */
 /* Named workspace region (byte offset, length in 4-byte words): "adam_ta" / "adam_tc", the actor / critic Adam step counters (fp64)
- * a checkpoint saves beside the parameter vectors.  Non-zero and mx_last_error for an unknown name. */
+ * a checkpoint saves beside the parameter vectors; "p2p_abort", the data-parallel exchange's sticky abort word (fp32, -1 after a peer
+ * time-out).  Non-zero and mx_last_error for an unknown name. */
 int mx_maddpg_ws_lookup(const mx_maddpg* h, const char* name, int64_t* byte_offset, int64_t* n_elems);
 /* device fp32[8]: critic_loss, critic_grad_norm, -, denom, actor_loss, actor_grad_norm, -, denom */
 const float* mx_maddpg_info(mx_maddpg* h);
@@ -388,6 +389,38 @@ const float* mx_maddpg_priorities(mx_maddpg* h);
 int mx_maddpg_grad_views(mx_maddpg* h, int64_t* actor_off_bytes, int64_t* critic_off_bytes);   /* parity tests: numerator grads in the workspace */
 int mx_maddpg_soft_update(mx_maddpg* h, void* stream);   /* rMADDPGPolicy.py:162-165 */
 int mx_maddpg_hard_update(mx_maddpg* h, void* stream);   /* rMADDPGPolicy.py:167-170 */
+
+/* Data-parallel training of the actor-critic learners (one process per GPU, each rank samples its own batch; DESIGN.md section 6).
+ * An update exchanges two flat buffers grad[P+4] (gradient numerators, then the loss scalars), the critic's and then the actor's:
+ * the actor's backward reads the critic after its Adam step.  Every rank sums the world's buffers in rank order, so every rank clips
+ * by the same norm and applies bit-identical Adam and Polyak steps.  `net` is MX_MADDPG_ACTOR or MX_MADDPG_CRITIC. */
+#define MX_MADDPG_ACTOR 0
+#define MX_MADDPG_CRITIC 1
+/* Peer memory: per network, every rank allocates one SYMMETRIC block of mx_maddpg_p2p_block_bytes(h, net) (zero-filled, mapped into
+ * every peer; laid out for up to 16 ranks) and hands the world's block addresses of that network, in rank order, to mx_maddpg_set_peers
+ * with a zeroed local uint32 counter of its own.  The exchange is keyed to that network's Adam step count (adam_ta / adam_tc).  From
+ * then on mx_maddpg_step[_ex] is complete: critic grads -> publish + reduce -> critic Adam -> actor grads -> publish + reduce -> actor
+ * Adam.  A peer that does not deliver within the p2p_timeout_ms option sets the sticky abort word (mx_maddpg_ws_lookup "p2p_abort")
+ * to -1: no update is applied from then on and the caller is expected to raise.  Without peers the learner runs on one GPU and
+ * launches exactly the kernels it launches with none of this set. */
+int64_t mx_maddpg_p2p_block_bytes(mx_maddpg* h, int32_t net);
+int mx_maddpg_set_peers(mx_maddpg* h, int32_t net, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev);
+int mx_maddpg_p2p_publish(mx_maddpg* h, int32_t net, void* stream);   /* push this rank's buffer to every peer, then raise its flag */
+int mx_maddpg_p2p_reduce(mx_maddpg* h, int32_t net, void* stream);    /* wait for every peer's flag, sum the buffers in rank order */
+/* The buffer one exchange sums, n_floats = P + 4 (P: the parameters the network's Adam step updates), for an external all-reduce. */
+float* mx_maddpg_grad_buffer(mx_maddpg* h, int32_t net, int64_t* n_floats);
+/* One update of mx_maddpg_step_ex split at its two exchanges, which the caller makes between the calls (an all-reduce of
+ * mx_maddpg_grad_buffer, e.g. NCCL; or mx_maddpg_p2p_publish on every rank before mx_maddpg_p2p_reduce on any):
+ *   MX_MADDPG_CRITIC_GRADS -> [exchange critic] -> MX_MADDPG_CRITIC_APPLY -> MX_MADDPG_ACTOR_GRADS -> [exchange actor] -> MX_MADDPG_ACTOR_APPLY
+ * The phases run in this order; *update_actor_out (set by every phase) tells whether the update trains the actor, and when it does not
+ * MX_MADDPG_CRITIC_APPLY ends the update.  batch and the noise pointers as for mx_maddpg_step_ex, the same on every call of one update
+ * (read by the two GRADS phases).  Each phase makes the launches mx_maddpg_step_ex makes for it. */
+#define MX_MADDPG_CRITIC_GRADS 0
+#define MX_MADDPG_CRITIC_APPLY 1
+#define MX_MADDPG_ACTOR_GRADS 2
+#define MX_MADDPG_ACTOR_APPLY 3
+int mx_maddpg_step_phase(mx_maddpg* h, int32_t phase, const mx_batch* batch, const float* target_noise_dev, const float* actor_noise_dev,
+                         int32_t* update_actor_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Rollout-time policy step (one env step of the runners' collect_rollout loops, runner/rnn/smac_runner.py:73-98,

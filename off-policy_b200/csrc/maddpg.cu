@@ -447,6 +447,7 @@ struct MxMaddpgWs {
   struct : MxPassWs { int64_t h0, dx; } r;      // agent-replaced copies, rows Mr = N*B*T (live slots); h0: critic state before the step,
                                                 // dx: gradient at the input rows
   int64_t gpart_a, gpart_c, grad_a, grad_c, spart, info, prio, adam_ta, adam_tc, scal_c, scal_a;
+  int64_t p2p_abort;        // data parallel: the sticky abort word of both exchanges (-1 after a peer time-out: no update is applied)
   int64_t tc_da2, tc_da1, tc_imgT, tc_acc, tc_acc_cols;      // scratch of the tensor-core backward (option wgrad_tc), shared by the critic and actor updates
   int64_t cent_acts, cent_nacts;        // [B*T][ca_ld] centralised action vectors assembled from all policies (cent_act_dim > 0)
   int64_t total;
@@ -463,6 +464,9 @@ struct mx_maddpg {
   int64_t num_updates;
   const float* valid = nullptr;     // cfg.mlp: valid_transition store [rows][n_agents] (mx_maddpg_set_valid)
   int force_update_actor = -1;      // graph capture: -1 = decide from num_updates, 0 / 1 = record this variant
+  MxP2pPeers p2p[2];                // data parallel (mx_maddpg_set_peers): the peers of the actor's [0] and the critic's [1] exchange
+  int phase_next = 0;               // mx_maddpg_step_phase: the phase the update in progress expects next (0: none in progress)
+  bool phase_actor = false;         //   and whether that update trains the actor
 };
 
 static inline int mx_imin_host(int a, int b) { return a < b ? a : b; }
@@ -629,6 +633,7 @@ static int64_t maddpg_ws_layout(const mx_maddpg_cfg* c, int64_t Pa, int64_t Pc, 
   W->r.out[0] = tk(Mr * K); W->r.dout = tk(Mr * K); W->r.dh = tk(Mr * MX_H); W->r.dgi = tk(Mr * MX_G); W->r.dx = tk(Mr * ldc);
   W->gpart_a = tk((int64_t)npart * Pa); W->gpart_c = tk((int64_t)npart * Pc); W->grad_a = tk(Pa + 8); W->grad_c = tk(Pc + 8);
   W->spart = tk(16); W->info = tk(8); W->prio = tk(B); W->adam_ta = tk(8); W->adam_tc = tk(8); W->scal_c = tk(8); W->scal_a = tk(8);
+  W->p2p_abort = tk(8);
   {
     const int64_t Mx = Ma > Mc ? Ma : Mc;
     const size_t ia = mx_tc_imageT_floats(c->obs_dim), ic = mx_tc_imageT_floats(critic_in_dim(c));
@@ -699,8 +704,11 @@ __global__ void k_set_scalars(float* grad_tail, const float* scal) {
   }
 }
 
+// The optimiser of one network in two halves around the data-parallel exchange: reduce_grads leaves the exchange payload grad[P+4]
+// (k_grad_reduce: numerators, Adam step count bumped; k_set_scalars: the loss scalars behind them), apply_grads clips by the norm of that
+// buffer and applies Adam (k_adam; normpart stays null, so the norm is always computed from the buffer, summed over the ranks or not).
 // front_parts / head_parts: the gradient partials k_front_bwd and k_head_bwd wrote
-static int optimise(mx_maddpg* h, bool actor, int front_parts, int head_parts, cudaStream_t s) {
+static OptimArgs optim_args(mx_maddpg* h, bool actor, int front_parts, int head_parts) {
   const mx_maddpg_cfg& c = h->cfg;
   const MxNetLayout& L = actor ? h->actor : h->critic;
   const int64_t P = actor ? h->Pa : h->Pc;
@@ -719,15 +727,38 @@ static int optimise(mx_maddpg* h, bool actor, int front_parts, int head_parts, c
   }
   o.spart = ws + h->W.spart; o.spart_n = 0;
   o.info = ws + h->W.info + (actor ? 4 : 0);
+  o.abort = ws + h->W.p2p_abort;
   o.adam_t = reinterpret_cast<double*>(ws + (actor ? h->W.adam_ta : h->W.adam_tc));
   o.err = nullptr; o.B = 0; o.T = 0; o.prio = nullptr;
   o.lr = c.lr; o.beta1 = c.adam_beta1; o.beta2 = c.adam_beta2; o.eps = c.adam_eps; o.max_grad_norm = c.max_grad_norm; o.tau = c.tau;
   o.weight_decay = c.weight_decay;
+  return o;
+}
+
+static int reduce_grads(mx_maddpg* h, bool actor, int front_parts, int head_parts, cudaStream_t s) {
+  const OptimArgs o = optim_args(h, actor, front_parts, head_parts);
   if (mx_launch_grad_reduce(o, s)) return 1;     // (its scalar block bumps the Adam step count; the loss scalars come from the loss kernel)
-  if (mx_launch("k_set_scalars", k_set_scalars, dim3(1), dim3(32), 0, s, MX_PLAIN, o.grad + o.P,
-                (const float*)(ws + (actor ? h->W.scal_a : h->W.scal_c))))
-    return 1;
-  return mx_launch_adam(o, s);
+  return mx_launch("k_set_scalars", k_set_scalars, dim3(1), dim3(32), 0, s, MX_PLAIN, o.grad + o.P,
+                   (const float*)(h->ws + (actor ? h->W.scal_a : h->W.scal_c)));
+}
+
+static int apply_grads(mx_maddpg* h, bool actor, cudaStream_t s) { return mx_launch_adam(optim_args(h, actor, 0, 0), s); }
+
+// one network's exchange payload: what k_grad_reduce + k_set_scalars left, keyed to that network's own Adam step count
+static MxP2pPayload p2p_payload(mx_maddpg* h, bool actor) {
+  const OptimArgs o = optim_args(h, actor, 0, 0);
+  MxP2pPayload pl;
+  pl.grad = o.grad; pl.P = o.P; pl.adam_t = o.adam_t; pl.abort = h->ws + h->W.p2p_abort;
+  return pl;
+}
+
+// with peers set (mx_maddpg_set_peers): push this rank's payload to every peer, then sum the world's in rank order; a no-op on one GPU
+static int exchange(mx_maddpg* h, bool actor, cudaStream_t s) {
+  const MxP2pPeers& peers = h->p2p[actor ? 0 : 1];
+  if (peers.world < 2) return 0;
+  const MxP2pPayload pl = p2p_payload(h, actor);
+  if (mx_p2p_publish(peers, pl, MX_P2P_MAX_WORLD, s)) return 1;
+  return mx_p2p_reduce(peers, pl, MX_P2P_MAX_WORLD, s);
 }
 
 // ---- the launches of one update: each builder fills its arguments from (network, pass) and the learner-wide settings; the phase lists
@@ -957,11 +988,12 @@ struct Step {               // one call of learner h over batch b on stream s
 };
 // ---- recurrent learner: shared_train_policy_on_batch (r_maddpg.py:114-331) ------------------------------------------------------------
 // Several policies (cent_act_dim > 0): the centralised action vectors were assembled by mx_maddpg_cent_contribute.
-static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor) {
+// Two halves around the critic's Adam step: critic_grads_rnn (A-E) leaves the critic's exchange payload, actor_grads_rnn (F) reads the
+// critic after that step and leaves the actor's.
+static int critic_grads_rnn(const Step& st, const float* target_noise_dev) {
   const MxMaddpgWs& W = st.W;
   float* ws = st.ws;
-  const int B = st.b->B, T = st.c.episode_len, N = st.c.n_agents;
-  const int Ma = B * (T + 1) * N, Mc = B * T, Mr = N * B * T;
+  const int B = st.b->B, T = st.c.episode_len, Mc = B * T;
 
   // ---------- A. actor: live + target over the T+1 steps ----------
   if (st.actor_fwd(BOTH, target_noise_dev)) return 1;
@@ -986,10 +1018,16 @@ static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const 
   if (st.head_bwd(CRITIC, W.c, Mc, &head_parts)) return 1;
   if (st.gru_bwd(CRITIC, W.c, B, T, 1, T, nullptr)) return 1;
   if (st.front_bwd(CRITIC, W.c, Mc, T, 1, T, nullptr, nullptr, &parts)) return 1;
-  if (optimise(st.h, false, parts, head_parts, st.s)) return 1;
+  return reduce_grads(st.h, false, parts, head_parts, st.s);
+}
+
+static int actor_grads_rnn(const Step& st, const float* actor_noise_dev) {
+  const MxMaddpgWs& W = st.W;
+  float* ws = st.ws;
+  const int B = st.b->B, T = st.c.episode_len, N = st.c.n_agents;
+  const int Ma = B * (T + 1) * N, Mc = B * T, Mr = N * B * T;
 
   // ---------- F. actor update with the UPDATED critic ----------
-  if (!update_actor) return 0;
   // live critic recurrence over the buffer sequence again (its parameters just changed)
   if (st.front_fwd(CRITIC, W.c, Mc, LIVE, false)) return 1;
   if (st.gru_fwd(CRITIC, W.c, LIVE, B, T - 1, 1, nullptr)) return 1;
@@ -1010,7 +1048,7 @@ static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const 
   if (st.head_bwd(ACTOR, W.a, Ma, &ahead_parts)) return 1;
   if (st.gru_bwd(ACTOR, W.a, B * N, T, N, T + 1, nullptr)) return 1;
   if (st.front_bwd(ACTOR, W.a, Ma, T, N, 0, nullptr, nullptr, &aparts)) return 1;
-  return optimise(st.h, true, aparts, ahead_parts, st.s);
+  return reduce_grads(st.h, true, aparts, ahead_parts, st.s);
 }
 
 // ---- cfg.mlp: shared_train_policy_on_batch of the transition-level trainer (maddpg.py:90-249) ---------------------------------------
@@ -1022,11 +1060,10 @@ static int maddpg_step_rnn(const Step& st, const float* target_noise_dev, const 
 // Several policies (cent_act_dim > 0): the centralised action vectors were assembled by mx_maddpg_cent_contribute, so the step runs
 // only the live actor and never reads its own target actions; the batch is this policy's (rewards, dones_env, shared observation,
 // PER weights, maddpg.py:103-107) and the valid_transition store is this policy's [rows][n_agents].
-static int maddpg_step_mlp(const Step& st, const float* target_noise_dev, const float* actor_noise_dev, bool update_actor) {
+static int critic_grads_mlp(const Step& st, const float* target_noise_dev) {
   const MxMaddpgWs& W = st.W;
   float* ws = st.ws;
-  const int B = st.b->B, N = st.c.n_agents, K = st.c.num_q, Ac = st.c.act_dim;
-  const int Ma = B * 2 * N, Mc = B, Mr = N * B;
+  const int Mc = st.b->B, K = st.c.num_q;
 
   // ---------- A. live + target actor on obs and next_obs; target actions a' from the next_obs rows (maddpg.py:64-74) ----------
   if (st.actor_fwd(st.c.cent_act_dim > 0 ? LIVE : BOTH, target_noise_dev)) return 1;
@@ -1044,8 +1081,14 @@ static int maddpg_step_mlp(const Step& st, const float* target_noise_dev, const 
   if (st.mlp_dgi_cols(W.c, Mc)) return 1;
   int parts = 0;
   if (st.front_bwd(CRITIC, W.c, Mc, 1, 1, 0, nullptr, nullptr, &parts)) return 1;
-  if (optimise(st.h, false, parts, 0, st.s)) return 1;
-  if (!update_actor) return 0;
+  return reduce_grads(st.h, false, parts, 0, st.s);
+}
+
+static int actor_grads_mlp(const Step& st, const float* actor_noise_dev) {
+  const MxMaddpgWs& W = st.W;
+  float* ws = st.ws;
+  const int B = st.b->B, N = st.c.n_agents, K = st.c.num_q, Ac = st.c.act_dim;
+  const int Ma = B * 2 * N, Mr = N * B;
 
   // ---------- D. actor loss through head 0 of the UPDATED critic on the agent-replaced copies, masked by valid_transition ----------
   if (st.mlp_head_cols(W.a.gi[0], Ma, Ac, nullptr, ws + W.a.out[0], nullptr)) return 1;
@@ -1061,31 +1104,132 @@ static int maddpg_step_mlp(const Step& st, const float* target_noise_dev, const 
   if (st.scatter_actor_grad()) return 1;
   int aparts = 0;
   if (st.front_bwd(ACTOR, W.a, Ma, 1, N, 0, nullptr, nullptr, &aparts)) return 1;
-  return optimise(st.h, true, aparts, 0, st.s);
+  return reduce_grads(st.h, true, aparts, 0, st.s);
 }
 
 extern "C" int mx_maddpg_step(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, int32_t* update_actor_out, void* stream) {
   return mx_maddpg_step_ex(h, b, target_noise_dev, nullptr, update_actor_out, stream);
 }
 
-extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev,
-                                 int32_t* update_actor_out, void* stream) {
+// the checks every update makes before its first launch, and whether it trains the actor
+static int check_step(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev, bool* update_actor) {
   const mx_maddpg_cfg& c = h->cfg;
-#if !MX_EMU
-  g_mx_pdl_auto = 1;      // ~40 small dependent launches per update: programmatic dependent launch measured 491 -> 469 us (R-MADDPG), 372 -> 355 us (R-MATD3)
-#endif
   if (!b || b->B <= 0 || b->B > c.max_batch) { mx_set_error("maddpg step: batch size outside [1, max_batch=%d]", c.max_batch); return 1; }
   if (!b->obs || !b->share || !b->acts || !b->rewards || !b->dones || !b->dones_env) { mx_set_error("maddpg step: missing batch field"); return 1; }
   if (c.use_per && !b->weights) { mx_set_error("maddpg step: use_per set but batch has no importance weights"); return 1; }
   if (c.target_noise > 0.f && !target_noise_dev) { mx_set_error("maddpg step: MATD3 target noise expected"); return 1; }
-  const bool update_actor = h->force_update_actor >= 0 ? h->force_update_actor != 0
-                                                     : (h->num_updates % (c.actor_update_interval > 0 ? c.actor_update_interval : 1)) == 0;
-  if (c.discrete && update_actor && !actor_noise_dev) { mx_set_error("maddpg step: discrete actor update needs the Gumbel draws (actor_noise_dev)"); return 1; }
+  *update_actor = h->force_update_actor >= 0 ? h->force_update_actor != 0
+                                             : (h->num_updates % (c.actor_update_interval > 0 ? c.actor_update_interval : 1)) == 0;
+  if (c.discrete && *update_actor && !actor_noise_dev) { mx_set_error("maddpg step: discrete actor update needs the Gumbel draws (actor_noise_dev)"); return 1; }
+  if (h->phase_next) { mx_set_error("maddpg step: a phased update (mx_maddpg_step_phase) is in progress, next phase %d", h->phase_next); return 1; }
+  return 0;
+}
+
+static int critic_grads(const Step& st, const float* target_noise_dev) {
+  return (st.c.mlp ? critic_grads_mlp : critic_grads_rnn)(st, target_noise_dev);
+}
+static int actor_grads(const Step& st, const float* actor_noise_dev) {
+  return (st.c.mlp ? actor_grads_mlp : actor_grads_rnn)(st, actor_noise_dev);
+}
+
+// critic grads -> [exchange] -> critic Adam -> actor grads (through the updated critic) -> [exchange] -> actor Adam; the exchanges run
+// only with peers set, so one GPU launches exactly the kernels of the undivided update
+extern "C" int mx_maddpg_step_ex(mx_maddpg* h, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev,
+                                 int32_t* update_actor_out, void* stream) {
+#if !MX_EMU
+  g_mx_pdl_auto = 1;      // ~40 small dependent launches per update: programmatic dependent launch measured 491 -> 469 us (R-MADDPG), 372 -> 355 us (R-MATD3)
+#endif
+  bool update_actor = false;
+  if (check_step(h, b, target_noise_dev, actor_noise_dev, &update_actor)) return 1;
   const Step st(h, b, (cudaStream_t)stream);
-  if ((c.mlp ? maddpg_step_mlp : maddpg_step_rnn)(st, target_noise_dev, actor_noise_dev, update_actor)) return 1;
+  if (critic_grads(st, target_noise_dev) || exchange(h, false, st.s) || apply_grads(h, false, st.s)) return 1;
+  if (update_actor && (actor_grads(st, actor_noise_dev) || exchange(h, true, st.s) || apply_grads(h, true, st.s))) return 1;
   if (update_actor_out) *update_actor_out = update_actor ? 1 : 0;
   if (h->force_update_actor < 0) h->num_updates += 1;      // (graph replays count in mx_graph_launch)
   return 0;
+}
+
+// One update as four calls, the exchanges left to the caller between them (an all-reduce of mx_maddpg_grad_buffer, or
+// mx_maddpg_p2p_publish / _reduce): MX_MADDPG_CRITIC_GRADS decides whether the update trains the actor; MX_MADDPG_CRITIC_APPLY ends an
+// update that does not; MX_MADDPG_ACTOR_GRADS / _APPLY follow otherwise.  Same launches as mx_maddpg_step_ex without its exchanges.
+extern "C" int mx_maddpg_step_phase(mx_maddpg* h, int32_t phase, const mx_batch* b, const float* target_noise_dev, const float* actor_noise_dev,
+                                    int32_t* update_actor_out, void* stream) {
+  if (!h) { mx_set_error("mx_maddpg_step_phase: null handle"); return 1; }
+  if (phase < MX_MADDPG_CRITIC_GRADS || phase > MX_MADDPG_ACTOR_APPLY) { mx_set_error("mx_maddpg_step_phase: phase %d outside [0, 3]", phase); return 1; }
+  if (phase != h->phase_next) {
+    mx_set_error("mx_maddpg_step_phase: phase %d out of order, the update in progress expects phase %d", phase, h->phase_next); return 1;
+  }
+#if !MX_EMU
+  g_mx_pdl_auto = 1;
+#endif
+  const cudaStream_t s = (cudaStream_t)stream;
+  bool done = false;
+  if (phase == MX_MADDPG_CRITIC_GRADS) {
+    bool update_actor = false;
+    if (check_step(h, b, target_noise_dev, actor_noise_dev, &update_actor)) return 1;
+    if (critic_grads(Step(h, b, s), target_noise_dev)) return 1;
+    h->phase_actor = update_actor;
+    h->phase_next = MX_MADDPG_CRITIC_APPLY;
+  } else if (phase == MX_MADDPG_CRITIC_APPLY) {
+    if (apply_grads(h, false, s)) return 1;
+    h->phase_next = h->phase_actor ? MX_MADDPG_ACTOR_GRADS : 0;
+    done = !h->phase_actor;
+  } else if (phase == MX_MADDPG_ACTOR_GRADS) {
+    if (!b || b->B <= 0 || b->B > h->cfg.max_batch) { mx_set_error("mx_maddpg_step_phase: the actor phase needs the update's batch"); return 1; }
+    if (actor_grads(Step(h, b, s), actor_noise_dev)) return 1;
+    h->phase_next = MX_MADDPG_ACTOR_APPLY;
+  } else {
+    if (apply_grads(h, true, s)) return 1;
+    h->phase_next = 0;
+    done = true;
+  }
+  if (update_actor_out) *update_actor_out = h->phase_actor ? 1 : 0;
+  if (done && h->force_update_actor < 0) h->num_updates += 1;
+  return 0;
+}
+
+// ---- data parallel: the two exchange payloads over peer memory (p2p.cu) -------------------------------------------------------------
+static bool net_ok(const char* who, const mx_maddpg* h, int32_t net) {
+  if (!h) { mx_set_error("%s: null handle", who); return false; }
+  if (net != MX_MADDPG_ACTOR && net != MX_MADDPG_CRITIC) { mx_set_error("%s: net %d is neither MX_MADDPG_ACTOR (0) nor MX_MADDPG_CRITIC (1)", who, net); return false; }
+  return true;
+}
+extern "C" int64_t mx_maddpg_p2p_block_bytes(mx_maddpg* h, int32_t net) {
+  if (!net_ok("mx_maddpg_p2p_block_bytes", h, net)) return -1;
+  return mx_p2p_block_floats(p2p_payload(h, net == MX_MADDPG_ACTOR).P, MX_P2P_MAX_WORLD) * 4;
+}
+extern "C" int mx_maddpg_set_peers(mx_maddpg* h, int32_t net, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev) {
+  if (!net_ok("mx_maddpg_set_peers", h, net)) return 1;
+  MxP2pPeers peers;
+  if (mx_p2p_set_peers("mx_maddpg_set_peers", &peers, rank, world, peer_blocks, counter_dev)) return 1;
+  const MxP2pPeers& other = h->p2p[net == MX_MADDPG_ACTOR ? 1 : 0];
+  if (other.world && (other.world != world || other.rank != rank)) {
+    mx_set_error("mx_maddpg_set_peers: rank %d / world %d differ from the other network's %d / %d", rank, world, other.rank, other.world);
+    return 1;
+  }
+  for (int p = 0; p < world; ++p)
+    if (peers.blocks[p] == other.blocks[p] || (p > 0 && peers.blocks[p] == peers.blocks[0])) {
+      mx_set_error("mx_maddpg_set_peers: block %d is shared with another network or rank; each network of each rank needs its own", p); return 1;
+    }
+  if (counter_dev == other.counter) { mx_set_error("mx_maddpg_set_peers: each network needs its own arrival counter"); return 1; }
+  h->p2p[net == MX_MADDPG_ACTOR ? 0 : 1] = peers;
+  return 0;
+}
+static int p2p_call(const char* who, mx_maddpg* h, int32_t net, void* stream, bool publish) {
+  if (!net_ok(who, h, net)) return 1;
+  const bool actor = net == MX_MADDPG_ACTOR;
+  const MxP2pPeers& peers = h->p2p[actor ? 0 : 1];
+  if (!peers.world) { mx_set_error("%s: mx_maddpg_set_peers was not called for net %d", who, net); return 1; }
+  const MxP2pPayload pl = p2p_payload(h, actor);
+  return (publish ? mx_p2p_publish : mx_p2p_reduce)(peers, pl, MX_P2P_MAX_WORLD, (cudaStream_t)stream);
+}
+extern "C" int mx_maddpg_p2p_publish(mx_maddpg* h, int32_t net, void* stream) { return p2p_call("mx_maddpg_p2p_publish", h, net, stream, true); }
+extern "C" int mx_maddpg_p2p_reduce(mx_maddpg* h, int32_t net, void* stream) { return p2p_call("mx_maddpg_p2p_reduce", h, net, stream, false); }
+extern "C" float* mx_maddpg_grad_buffer(mx_maddpg* h, int32_t net, int64_t* n_floats) {
+  if (!net_ok("mx_maddpg_grad_buffer", h, net)) return nullptr;
+  const MxP2pPayload pl = p2p_payload(h, net == MX_MADDPG_ACTOR);
+  if (n_floats) *n_floats = pl.P + 4;
+  return pl.grad;
 }
 
 // ---- several policies (share_policy = False, scripts/train_mpe_rmaddpg.sh:14 -> train/train_mpe.py:139-150) ------------------------------
@@ -1282,7 +1426,7 @@ extern "C" int mx_maddpg_set_num_updates(mx_maddpg* h, int64_t n) {
 extern "C" int mx_maddpg_ws_lookup(const mx_maddpg* h, const char* name, int64_t* byte_offset, int64_t* n_elems) {
   if (!h || !name) { mx_set_error("mx_maddpg_ws_lookup: null argument"); return 1; }
   struct Ent { const char* n; int64_t off, cnt; };
-  const Ent tab[] = {{"adam_ta", h->W.adam_ta, 8}, {"adam_tc", h->W.adam_tc, 8}};
+  const Ent tab[] = {{"adam_ta", h->W.adam_ta, 8}, {"adam_tc", h->W.adam_tc, 8}, {"p2p_abort", h->W.p2p_abort, 1}};
   for (const Ent& e : tab)
     if (!strcmp(e.n, name)) { *byte_offset = e.off * 4; *n_elems = e.cnt; return 0; }
   mx_set_error("mx_maddpg_ws_lookup: unknown region '%s'", name);

@@ -198,5 +198,27 @@ struct mx_qmix {
   int prep_pending = 0;    // mx_qmix_prefork() already launched the weight-image prep for the coming step
   int imgT_fresh = 0;      // the transposed images (tensor-core backward) were rebuilt with the forward ones for this step
 };
+// ---- data-parallel exchange over peer memory (p2p.cu), for any learner's flat gradient buffer ----
+#define MX_P2P_MAX_WORLD 16
+// what one exchange sums: grad[P + 4] (gradient numerators, then the four loss scalars), keyed to the network's Adam step count (slot
+// parity and flag value; already bumped by k_grad_reduce), and the learner's sticky abort word (-1 after a peer time-out)
+struct MxP2pPayload {
+  float* grad;
+  int64_t P;                  // a multiple of 4
+  const double* adam_t;
+  float* abort;
+};
+struct MxP2pPeers {         // the world's symmetric blocks in rank order and this rank's local arrival counter
+  int rank = 0, world = 0;
+  float* blocks[MX_P2P_MAX_WORLD] = {nullptr};
+  uint32_t* counter = nullptr;
+};
+int64_t mx_p2p_slot_floats(int64_t P);
+// floats of one symmetric block laid out for `layout_world` ranks: slots of both parities [2][layout_world][slot] | 64 flag words
+int64_t mx_p2p_block_floats(int64_t P, int layout_world);
+int mx_p2p_set_peers(const char* who, MxP2pPeers* out, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev);
+int mx_p2p_publish(const MxP2pPeers& peers, const MxP2pPayload& pl, int layout_world, cudaStream_t s);
+int mx_p2p_reduce(const MxP2pPeers& peers, const MxP2pPayload& pl, int layout_world, cudaStream_t s);
+
 int mx_replay_sample_per_state_beta(mx_replay* r, int32_t B, void* stream);   // PER draw whose exponent is the device scalar (captured sequences)
 int mx_qmix_prefork(mx_qmix* q, int B, void* stream);   // optional: start the parameter-only work of the next step before its batch is sampled

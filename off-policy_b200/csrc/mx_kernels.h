@@ -215,6 +215,7 @@ struct OptimArgs {
   const float* spart;
   int spart_n;
   float* info;             // [8]
+  const float* abort;      // k_adam applies nothing while *abort < 0 (a peer-memory exchange timed out); null: info[7] is that word
   double* adam_t;          // [4]
   // loss / PER finalisation
   const float* err;        // [B][T] masked TD errors

@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(1024) k_adam(OptimArgs a) {
   __shared__ float s_scale, s_step, s_bc2s;
   const int tid = threadIdx.x;
   MX_PDL_WAIT();
-  if (a.info[7] < 0.f) return;        // the peer-memory exchange timed out (p2p.cu): the sums are not trustworthy, apply nothing
+  if ((a.abort ? *a.abort : a.info[7]) < 0.f) return;     // the peer-memory exchange timed out (p2p.cu): the sums are not trustworthy, apply nothing
   const float denom = a.grad[a.P + 0];
   const float invd = 1.0f / denom;
   // ||g||^2 over the full vector, identical summation order in every CTA (no grid-wide barrier needed)

@@ -14,26 +14,30 @@
 // In the product path the whole exchange lives INSIDE the optimiser kernel (optim.cu: k_optim_fused -- the blocks that reduce the
 // gradient partials push their columns straight from registers and apply Adam to the summed columns); the two kernels below are the
 // same protocol as separate launches: start-up self-test, the emulated two-rank test, and `mx_set_option("optim_fused", 0)`.
+//
+// The helpers take a payload (buffer, P, Adam step count, abort word) rather than a learner.  The actor-critic learner (maddpg.cu)
+// exchanges two payloads per update, the critic's and then the actor's, each over its own block, flags and arrival counter and keyed
+// to its own Adam step count (the two counts advance at different rates when the actor trains every other update).  Its blocks are
+// laid out for MX_P2P_MAX_WORLD ranks, so they can be sized before the world is known; the flags sit behind those slots.
 #include <string.h>
 
 #include "mx_internal.h"
 #include "mx_kernels.h"
-
-#define MX_P2P_MAX_WORLD 16
 
 struct P2pArgs {
   float* grad;                 // [n] local flat buffer (k_grad_reduce output / k_adam input)
   float* blk[MX_P2P_MAX_WORLD];        // base of every rank's symmetric block (own block at index `rank`)
   long long n4;                // float4 per slot
   long long slot_floats;       // floats per slot (padded)
+  long long flags_off;         // floats from a block's base to its flag words (behind the slots of both parities)
   const double* adam_t;        // adam_t[0] = 1-based step count, already bumped by k_grad_reduce
   unsigned* counter;           // local: CTAs of k_p2p_push that have finished
-  float* info;                 // info[7] = -1 when a peer never arrived (time-out)
+  float* abort;                // sticky abort word: -1 when a peer never arrived (time-out)
   int rank, world;
   unsigned long long timeout_ns;   // option p2p_timeout_ms (default 10 s)
 };
 
-MX_DEVINL unsigned* p2p_flags(float* block, long long slot_floats, int world) { return reinterpret_cast<unsigned*>(block + 2 * (size_t)world * slot_floats); }
+MX_DEVINL unsigned* p2p_flags(float* block, long long flags_off) { return reinterpret_cast<unsigned*>(block + flags_off); }
 
 __global__ void __launch_bounds__(256) k_p2p_push(P2pArgs a) {
   const unsigned step = (unsigned)a.adam_t[0];
@@ -51,7 +55,7 @@ __global__ void __launch_bounds__(256) k_p2p_push(P2pArgs a) {
     if (threadIdx.x == 0) *a.counter = 0u;
     if ((int)threadIdx.x < a.world) {
       __threadfence_system();
-      volatile unsigned* f = p2p_flags(a.blk[threadIdx.x], a.slot_floats, a.world) + a.rank;
+      volatile unsigned* f = p2p_flags(a.blk[threadIdx.x], a.flags_off) + a.rank;
       *f = step;
     }
   }
@@ -73,7 +77,7 @@ __global__ void __launch_bounds__(256) k_p2p_sum(P2pArgs a) {
   if (threadIdx.x == 0) s_bad = 0;
   __syncthreads();
   if ((int)threadIdx.x < a.world) {
-    volatile unsigned* f = p2p_flags(a.blk[a.rank], a.slot_floats, a.world) + threadIdx.x;
+    volatile unsigned* f = p2p_flags(a.blk[a.rank], a.flags_off) + threadIdx.x;
 #if !MX_EMU
     unsigned long long t0, t1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
@@ -87,8 +91,8 @@ __global__ void __launch_bounds__(256) k_p2p_sum(P2pArgs a) {
 #endif
   }
   __syncthreads();
-  if (s_bad) {                           // fatal: k_adam applies nothing while info[7] < 0 and the host raises (qmix.py)
-    if (threadIdx.x == 0) a.info[7] = -1.f;
+  if (s_bad) {                           // fatal: k_adam applies nothing while the abort word is < 0 and the host raises
+    if (threadIdx.x == 0) *a.abort = -1.f;
     return;
   }
   const size_t off = (size_t)(step & 1u) * a.world * a.slot_floats;
@@ -102,35 +106,32 @@ __global__ void __launch_bounds__(256) k_p2p_sum(P2pArgs a) {
   }
 }
 
-extern "C" int64_t mx_qmix_p2p_block_bytes(const mx_qmix* q) {
-  const int64_t slot = mx_round_up64(q->P + 8, 64);
-  const int64_t world = q->cfg.world_size > 1 ? q->cfg.world_size : 1;
-  return (2 * world * slot + 64 + 2 * world * 2 * slot) * 4;      // slots of both parities | flags | flag-in-data line arrays of both parities (k_optim_fused)
-}
+// ---- the protocol for any payload: block sizing, peer validation and the two launches ----
+int64_t mx_p2p_slot_floats(int64_t P) { return mx_round_up64(P + 8, 64); }
+int64_t mx_p2p_block_floats(int64_t P, int layout_world) { return 2 * (int64_t)layout_world * mx_p2p_slot_floats(P) + 64; }
 
-extern "C" int mx_qmix_set_peers(mx_qmix* q, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev) {
-  if (!q || !peer_blocks || !counter_dev) { mx_set_error("mx_qmix_set_peers: null argument"); return 1; }
-  if (world < 2 || world > MX_P2P_MAX_WORLD || rank < 0 || rank >= world) { mx_set_error("mx_qmix_set_peers: rank %d / world %d unsupported (max %d)", rank, world, MX_P2P_MAX_WORLD); return 1; }
-  if (world != q->cfg.world_size) { mx_set_error("mx_qmix_set_peers: world %d != cfg.world_size %d", world, q->cfg.world_size); return 1; }
-  q->p2p_rank = rank; q->p2p_world = world; q->p2p_counter = counter_dev;
-  for (int p = 0; p < world; ++p) {
-    if (!peer_blocks[p]) { mx_set_error("mx_qmix_set_peers: null peer block %d", p); return 1; }
-    q->p2p_blocks[p] = (float*)peer_blocks[p];
-  }
+int mx_p2p_set_peers(const char* who, MxP2pPeers* out, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev) {
+  if (!peer_blocks || !counter_dev) { mx_set_error("%s: null argument", who); return 1; }
+  if (world < 2 || world > MX_P2P_MAX_WORLD || rank < 0 || rank >= world) { mx_set_error("%s: rank %d / world %d unsupported (max %d)", who, rank, world, MX_P2P_MAX_WORLD); return 1; }
+  for (int p = 0; p < world; ++p)
+    if (!peer_blocks[p]) { mx_set_error("%s: null peer block %d", who, p); return 1; }
+  out->rank = rank; out->world = world; out->counter = counter_dev;
+  for (int p = 0; p < world; ++p) out->blocks[p] = (float*)peer_blocks[p];
   return 0;
 }
 
-static P2pArgs p2p_args(mx_qmix* q) {
+static P2pArgs p2p_args(const MxP2pPeers& peers, const MxP2pPayload& pl, int layout_world) {
   P2pArgs a;
   memset(&a, 0, sizeof(a));
-  a.grad = q->ws + q->W.grad;
-  for (int p = 0; p < q->p2p_world; ++p) a.blk[p] = q->p2p_blocks[p];
-  a.n4 = (q->P + 4) / 4;
-  a.slot_floats = mx_round_up64(q->P + 8, 64);
-  a.adam_t = reinterpret_cast<const double*>(q->ws + q->W.adam_t);
-  a.counter = q->p2p_counter;
-  a.info = q->ws + q->W.info;
-  a.rank = q->p2p_rank; a.world = q->p2p_world;
+  a.grad = pl.grad;
+  for (int p = 0; p < peers.world; ++p) a.blk[p] = peers.blocks[p];
+  a.n4 = (pl.P + 4) / 4;
+  a.slot_floats = mx_p2p_slot_floats(pl.P);
+  a.flags_off = 2 * (long long)layout_world * a.slot_floats;
+  a.adam_t = pl.adam_t;
+  a.counter = peers.counter;
+  a.abort = pl.abort;
+  a.rank = peers.rank; a.world = peers.world;
   a.timeout_ns = (unsigned long long)(g_mx_p2p_timeout_ms > 0 ? g_mx_p2p_timeout_ms : 10000) * 1000000ull;
   return a;
 }
@@ -142,16 +143,53 @@ static int p2p_grid(const P2pArgs& a) {
   return grid < 1 ? 1 : grid;
 }
 
+int mx_p2p_publish(const MxP2pPeers& peers, const MxP2pPayload& pl, int layout_world, cudaStream_t s) {
+  P2pArgs a = p2p_args(peers, pl, layout_world);
+  return mx_launch("k_p2p_push", k_p2p_push, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
+}
+
+int mx_p2p_reduce(const MxP2pPeers& peers, const MxP2pPayload& pl, int layout_world, cudaStream_t s) {
+  P2pArgs a = p2p_args(peers, pl, layout_world);
+  return mx_launch("k_p2p_sum", k_p2p_sum, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
+}
+
+// ---- QMIX: one payload, the learner's grad[P+4]; its block also holds k_optim_fused's line arrays ----
+extern "C" int64_t mx_qmix_p2p_block_bytes(const mx_qmix* q) {
+  const int64_t slot = mx_p2p_slot_floats(q->P);
+  const int64_t world = q->cfg.world_size > 1 ? q->cfg.world_size : 1;
+  return (mx_p2p_block_floats(q->P, (int)world) + 2 * world * 2 * slot) * 4;      // slots of both parities | flags | flag-in-data line arrays of both parities (k_optim_fused)
+}
+
+extern "C" int mx_qmix_set_peers(mx_qmix* q, int32_t rank, int32_t world, void* const* peer_blocks, uint32_t* counter_dev) {
+  if (!q) { mx_set_error("mx_qmix_set_peers: null argument"); return 1; }
+  MxP2pPeers peers;
+  if (mx_p2p_set_peers("mx_qmix_set_peers", &peers, rank, world, peer_blocks, counter_dev)) return 1;
+  if (world != q->cfg.world_size) { mx_set_error("mx_qmix_set_peers: world %d != cfg.world_size %d", world, q->cfg.world_size); return 1; }
+  q->p2p_rank = rank; q->p2p_world = world; q->p2p_counter = counter_dev;
+  for (int p = 0; p < world; ++p) q->p2p_blocks[p] = peers.blocks[p];
+  return 0;
+}
+
+static void qmix_p2p(mx_qmix* q, MxP2pPeers* peers, MxP2pPayload* pl) {
+  peers->rank = q->p2p_rank; peers->world = q->p2p_world; peers->counter = q->p2p_counter;
+  for (int p = 0; p < q->p2p_world; ++p) peers->blocks[p] = q->p2p_blocks[p];
+  pl->grad = q->ws + q->W.grad; pl->P = q->P;
+  pl->adam_t = reinterpret_cast<const double*>(q->ws + q->W.adam_t);
+  pl->abort = q->ws + q->W.info + 7;
+}
+
 extern "C" int mx_qmix_p2p_publish(mx_qmix* q, void* stream) {
   if (!q->p2p_world) { mx_set_error("mx_qmix_p2p_publish: mx_qmix_set_peers was not called"); return 1; }
-  P2pArgs a = p2p_args(q);
-  cudaStream_t s = (cudaStream_t)stream;
-  return mx_launch("k_p2p_push", k_p2p_push, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
+  MxP2pPeers peers;
+  MxP2pPayload pl;
+  qmix_p2p(q, &peers, &pl);
+  return mx_p2p_publish(peers, pl, q->p2p_world, (cudaStream_t)stream);
 }
 
 extern "C" int mx_qmix_p2p_reduce(mx_qmix* q, void* stream) {
   if (!q->p2p_world) { mx_set_error("mx_qmix_p2p_reduce: mx_qmix_set_peers was not called"); return 1; }
-  P2pArgs a = p2p_args(q);
-  cudaStream_t s = (cudaStream_t)stream;
-  return mx_launch("k_p2p_sum", k_p2p_sum, dim3(p2p_grid(a)), dim3(256), 0, s, MX_PLAIN, a);
+  MxP2pPeers peers;
+  MxP2pPayload pl;
+  qmix_p2p(q, &peers, &pl);
+  return mx_p2p_reduce(peers, pl, q->p2p_world, (cudaStream_t)stream);
 }

@@ -77,6 +77,8 @@ class PolicyStepArgs(C.Structure):
 
 TRNG_WORDS = 640      # MX_TRNG_WORDS: the device copy of torch's CPU generator (key[624], left, next)
 TRNG_UNIFORM, TRNG_GUMBEL, TRNG_NORMAL = 0, 1, 2
+MADDPG_ACTOR, MADDPG_CRITIC = 0, 1    # MX_MADDPG_ACTOR / _CRITIC: the network of a data-parallel exchange
+MADDPG_CRITIC_GRADS, MADDPG_CRITIC_APPLY, MADDPG_ACTOR_GRADS, MADDPG_ACTOR_APPLY = 0, 1, 2, 3     # mx_maddpg_step_phase
 
 
 class TrngDraw(C.Structure):
@@ -151,6 +153,12 @@ def _declare(lib):
         "mx_maddpg_step": (C.c_int, [vp, C.POINTER(Batch), vp, C.POINTER(i32), vp]),
         "mx_maddpg_step_ex": (C.c_int, [vp, C.POINTER(Batch), vp, vp, C.POINTER(i32), vp]),
         "mx_maddpg_cent_contribute": (C.c_int, [vp, C.POINTER(Batch), vp, vp, vp]),
+        "mx_maddpg_step_phase": (C.c_int, [vp, i32, C.POINTER(Batch), vp, vp, C.POINTER(i32), vp]),
+        "mx_maddpg_p2p_block_bytes": (i64, [vp, i32]),
+        "mx_maddpg_set_peers": (C.c_int, [vp, i32, i32, i32, C.POINTER(vp), vp]),
+        "mx_maddpg_p2p_publish": (C.c_int, [vp, i32, vp]),
+        "mx_maddpg_p2p_reduce": (C.c_int, [vp, i32, vp]),
+        "mx_maddpg_grad_buffer": (vp, [vp, i32, C.POINTER(i64)]),
         "mx_maddpg_info": (vp, [vp]),
         "mx_maddpg_priorities": (vp, [vp]),
         "mx_maddpg_grad_views": (C.c_int, [vp, C.POINTER(i64), C.POINTER(i64)]),

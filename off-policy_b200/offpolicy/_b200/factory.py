@@ -162,19 +162,23 @@ def make_rec_buffers(N, O, A, S, T, E, per_alpha=None, norm=False, rng="numpy", 
                                       max_batch=max_batch)
 
 
-def maddpg_args(cfg, B):
-    """Namespace fields R_MADDPGPolicy / R_MADDPG / R_MATD3 read, from a config object with the oracle's MaddpgConfig attribute names."""
-    return types.SimpleNamespace(
+def maddpg_args(cfg, B, **over):
+    """Namespace fields R_MADDPGPolicy / R_MADDPG / R_MATD3 read, from a config object with the oracle's MaddpgConfig attribute names;
+    `over` sets args fields."""
+    args = types.SimpleNamespace(
         hidden_size=cfg.hidden, layer_N=1, use_ReLU=bool(cfg.relu), use_feature_normalization=bool(cfg.feature_norm), use_orthogonal=True, gain=cfg.gain,
         use_conv1d=False, stacked_frames=1, use_rnn_layer=True, recurrent_N=1, prev_act_inp=False, gamma=cfg.gamma, use_per=cfg.use_per,
         per_nu=cfg.per_nu, per_eps=cfg.per_eps, use_huber_loss=cfg.huber, huber_delta=cfg.huber_delta, max_grad_norm=cfg.max_grad_norm,
         lr=cfg.lr, opti_eps=cfg.opti_eps, weight_decay=cfg.weight_decay, tau=cfg.tau, use_popart=False, use_value_active_masks=False,
         use_same_share_obs=True, batch_size=B, episode_length=0, epsilon_start=1.0, epsilon_finish=0.05, epsilon_anneal_time=50000,
         act_noise_std=0.1, target_action_noise_std=cfg.target_noise)
+    for k, v in over.items():
+        setattr(args, k, v)
+    return args
 
 
-def build_maddpg(cfg, B, T):
-    """(args, policy, trainer) for R-MADDPG (cfg.td3 False) / R-MATD3 (True), one shared policy."""
+def build_maddpg(cfg, B, T, **over):
+    """(args, policy, trainer) for R-MADDPG (cfg.td3 False) / R-MATD3 (True), one shared policy; `over` sets args fields."""
     from offpolicy._b200 import capi
     if cfg.td3:
         from offpolicy.algorithms.r_matd3.algorithm.rMATD3Policy import R_MATD3Policy as Policy
@@ -182,7 +186,7 @@ def build_maddpg(cfg, B, T):
     else:
         from offpolicy.algorithms.r_maddpg.algorithm.rMADDPGPolicy import R_MADDPGPolicy as Policy
         from offpolicy.algorithms.r_maddpg.r_maddpg import R_MADDPG as Trainer
-    args = maddpg_args(cfg, B)
+    args = maddpg_args(cfg, B, **over)
     info = dict(obs_space=Box(cfg.obs_dim, -np.inf, np.inf), share_obs_space=Box(cfg.state_dim, -np.inf, np.inf),
                 act_space=Discrete(cfg.act_dim) if cfg.discrete else Box(cfg.act_dim), cent_obs_dim=cfg.state_dim, cent_act_dim=cfg.act_dim * cfg.n_agents)
     pol = Policy({"args": args, "device": capi.device()}, info)

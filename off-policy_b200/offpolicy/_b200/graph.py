@@ -78,6 +78,14 @@ class StepGraph(_Graph):
             self.handle = None
 
 
+def _refuse_data_parallel(who, trainer):
+    """A data-parallel update is not captured: its exchanges must order every rank's publish before any rank's reduce, which two
+    graphs on one device cannot promise; the eager update (shared_train_policy_on_batch) runs the exchanges."""
+    if getattr(trainer, "world_size", 1) > 1:
+        raise ValueError("%s: the trainer trains data-parallel over %d ranks; a data-parallel update is not captured as a CUDA graph, "
+                         "call shared_train_policy_on_batch instead" % (who, trainer.world_size))
+
+
 class MaddpgStepGraph(_Graph):
     """[sample ->] shared_train_policy_on_batch [-> PER write-back] [-> soft update] of one policy of an R_MADDPG / R_MATD3 or
     single-policy MADDPG / MATD3 trainer, as CUDA graphs: one per update_actor variant the trainer can ask for.
@@ -93,6 +101,7 @@ class MaddpgStepGraph(_Graph):
     RING = 4
 
     def __init__(self, buffer, trainer, batch_size, beta=0.4, soft_update=True, p_id="policy_0"):
+        _refuse_data_parallel("MaddpgStepGraph", trainer)
         self.graphs = {}
         pb = buffer.policy_buffers[p_id]
         e = trainer._eng[p_id]
@@ -179,6 +188,7 @@ class MaddpgBatchTrainGraph(_Graph):
     RING = 4
 
     def __init__(self, buffer, trainer, batch_size, beta=0.4, soft_update=True):
+        _refuse_data_parallel("MaddpgBatchTrainGraph", trainer)
         if not getattr(trainer, "multi", False):
             raise ValueError("MaddpgBatchTrainGraph: the trainer has one shared policy; its update is captured by MaddpgStepGraph")
         ids = list(trainer.policy_ids)
